@@ -78,6 +78,12 @@ typedef struct tb200_bvh_node {
     uint32_t right_leaf;         /* bits 0..30 right child node index, bit 31 leaf flag */
 } tb200_bvh_node;
 
+/* The most levels of interior nodes a BVH (scene level or mesh) may have: the traversal keeps its
+ * pending nodes in a fixed 32-entry stack, as the reference does.  Every BVH is also a tree: walked
+ * from node 0, no node is reached twice.  tb200_create, tb200_scene_cache_save and
+ * tb200_create_cached refuse a scene that breaks either rule; tb200_bvh_build never returns one. */
+#define TB200_MAX_BVH_LEVELS 31
+
 /* MeshGeometry (src/scene.h:121-139).  All pointers are borrowed host memory. */
 typedef struct tb200_mesh {
     const float* positions;      /* numVertices * 3 */
@@ -348,7 +354,8 @@ tb200_renderer* tb200_create_cached(const char* path, int device);         /* NU
  * leaf.left = triangle index, node boxes = exact unions of triangle boxes), usable as tb200_mesh::nodes,
  * by the reference's IntersectRayMesh, and in the .bin mesh cache.  `positions`, `indices`, `outNodes`
  * are HOST arrays.  The tree differs from the reference builder's (an equally valid input to the same
- * traversal).  Returns 0 on success; tb200_bvh_build_error() describes a failure. */
+ * traversal).  Returns 0 on success; tb200_bvh_build_error() describes a failure.  A tree with more
+ * than TB200_MAX_BVH_LEVELS levels of interior nodes is a failure: outNodes is then zeroed. */
 typedef struct tb200_bvh_build_info {
     int32_t numNodes;          /* 2*numTriangles - 1 */
     int32_t rounds;            /* clustering rounds */

@@ -912,11 +912,39 @@ void parallel_bands(int H, int nthreads, F body)
     for (auto& x : th) x.join();
 }
 
+// The walks above hold at most (interior levels + 1) entries in their int stack[32]: true when the tree
+// below node 0 keeps every child index in range, reaches no node twice and has at most 31 interior levels.
+bool tree_fits_stack(const tb200_bvh_node* nodes, int numNodes)
+{
+    if (numNodes <= 0) return false;
+    std::vector<char> seen(numNodes, 0);
+    std::vector<std::pair<int, int>> todo(1, std::make_pair(0, 1));   // (node, level)
+    while (!todo.empty()) {
+        const std::pair<int, int> it = todo.back();
+        todo.pop_back();
+        if (seen[it.first]) return false;
+        seen[it.first] = 1;
+        const tb200_bvh_node& n = nodes[it.first];
+        if (node_is_leaf(n)) continue;
+        if (it.second > 31 || n.left >= (uint32_t)numNodes || node_right(n) >= (uint32_t)numNodes) return false;
+        todo.push_back(std::make_pair((int)n.left, it.second + 1));
+        todo.push_back(std::make_pair((int)node_right(n), it.second + 1));
+    }
+    return true;
+}
+
 }  // namespace
 
 extern "C" {
 
-void* oracle_create(const tb200_scene* scene) { return new Oracle{scene}; }
+// NULL when a BVH of the scene would overrun the traversal stack
+void* oracle_create(const tb200_scene* scene)
+{
+    if (!tree_fits_stack(scene->bvhNodes, scene->numBvhNodes)) return nullptr;
+    for (int m = 0; m < scene->numMeshes; ++m)
+        if (!tree_fits_stack(scene->meshes[m].nodes, scene->meshes[m].numNodes)) return nullptr;
+    return new Oracle{scene};
+}
 
 // work counters since the last reset (all zero unless built with -DTB_ORACLE_COUNT)
 int oracle_counters(unsigned long long* out, int reset)

@@ -259,7 +259,10 @@ class PortScene:
 
     def __init__(self, scene_ptr, camera, options, keepalive=None):
         self.lib = load_port()
-        self.h = C.c_void_p(self.lib.oracle_create(scene_ptr))
+        h = self.lib.oracle_create(scene_ptr)
+        if not h:
+            raise RuntimeError("the CPU restatement refused the scene: a BVH is not a tree or is too deep for its stack")
+        self.h = C.c_void_p(h)
         self.camera = abi.copy_struct(camera)
         self.options = abi.copy_struct(options)
         self._keep = keepalive

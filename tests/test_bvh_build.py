@@ -20,6 +20,7 @@ import refdrv
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+MAX_LEVELS = 31   # TB200_MAX_BVH_LEVELS
 
 
 def _mesh_arrays(mesh):
@@ -50,16 +51,14 @@ def _check_structure(nodes, pos, idx):
     refs = np.bincount(np.concatenate([li, ri]), minlength=nodes.shape[0])
     assert refs[0] == 0 and (refs[1:] == 1).all()
     assert np.array_equal(lo[inner], np.minimum(lo[li], lo[ri])) and np.array_equal(hi[inner], np.maximum(hi[li], hi[ri]))
-    # depth (iterative): the walkers and the reference's own stack[32] want <= 32
-    depth = np.zeros(nodes.shape[0], np.int32)
-    order = [0]
-    maxd = 0
+    # levels of nodes (iterative); the traversal stack holds trees of up to 31 interior levels, 32 node levels
     frontier = np.array([0])
     d = 0
     while frontier.size:
         d += 1
         f = frontier[~leaf[frontier]]
         frontier = np.concatenate([left[f], right[f]]) if f.size else np.array([], np.int64)
+    assert d - 1 <= MAX_LEVELS, "%d interior levels" % (d - 1)
     return d
 
 
@@ -184,3 +183,92 @@ def test_bvh_build_rejects_bad_input_and_handles_tiny_meshes():
     bad = np.array([[0, 1, 9]], np.int32)
     with pytest.raises(tb.TinselB200Error):
         tb.bvh_build(pos, bad, np.zeros(1, NODE_DTYPE))
+
+
+def _nested(n):
+    """n triangles, each half the size of the last and inside it: PLOC merges them into a chain."""
+    s = 0.5 ** np.arange(n)
+    pos = np.stack([np.stack([-s, -s, np.zeros(n)], 1), np.stack([s, -s, np.zeros(n)], 1), np.stack([np.zeros(n), s, np.zeros(n)], 1)], 1)
+    return pos.reshape(-1, 3), np.arange(3 * n).reshape(n, 3)
+
+
+def _hard_meshes(rng):
+    """Builder inputs that degenerate: identical triangles (equal Morton codes), an axis-aligned coplanar grid
+    (zero-extent boxes), zero-area triangles, nested triangles."""
+    tri = rng.uniform(-1, 1, (1, 3, 3))
+    yield "duplicates", np.repeat(tri, 200, 0).reshape(-1, 3), np.arange(600).reshape(200, 3)
+    g = np.linspace(0.0, 1.0, 33)
+    gp = np.array([[x, y, 0.0] for y in g for x in g])
+    gi = [(j * 33 + i, j * 33 + i + 1, j * 33 + i + 34) for j in range(32) for i in range(32)]
+    gi += [(j * 33 + i, j * 33 + i + 34, j * 33 + i + 33) for j in range(32) for i in range(32)]
+    yield "grid", gp, np.array(gi)
+    p = rng.uniform(-1, 1, (300, 3))
+    z = np.stack([p, p, rng.uniform(-1, 1, (300, 3))], 1)          # repeated vertex: zero area
+    yield "zero_area", z.reshape(-1, 3), np.arange(900).reshape(300, 3)
+    yield "nested", *_nested(48)
+
+
+def test_bvh_build_degenerate_inputs_stay_within_the_depth_bound():
+    """Either a tree that passes _check_structure (whose depth assertion is the traversal's bound) or a clean
+    error that names the depth: never a tree tb200_create would refuse."""
+    rng = np.random.RandomState(5)
+    for name, pos, idx in _hard_meshes(rng):
+        pos, idx = np.ascontiguousarray(pos, np.float32), np.ascontiguousarray(idx, np.int32)
+        nodes = np.zeros(2 * idx.shape[0] - 1, NODE_DTYPE)
+        try:
+            tb.bvh_build(pos, idx, nodes)
+        except tb.TinselB200Error as e:
+            assert "levels of interior nodes" in str(e), (name, str(e))
+            assert not nodes.view(np.uint8).any(), name
+            continue
+        _check_structure(nodes, pos, idx)
+
+
+def test_bvh_build_on_a_large_random_mesh():
+    """1.5 M random triangles (about 30 PLOC rounds): structure, depth, and one frame bit-exact with the port on the tree."""
+    rng = np.random.RandomState(11)
+    n = 1500000
+    c = rng.uniform(-1.0, 1.0, (n, 1, 3)).astype(np.float32)
+    pos = (c + rng.uniform(-0.01, 0.01, (n, 3, 3)).astype(np.float32)).reshape(-1, 3)
+    idx = np.arange(3 * n, dtype=np.int32).reshape(n, 3)
+    nodes = np.zeros(2 * n - 1, NODE_DTYPE)
+    info = tb.bvh_build(pos, idx, nodes)
+    depth = _check_structure(nodes, pos, idx)
+    print("random %d triangles: build %.2f ms (%d rounds), depth %d" % (n, info.buildMs, info.rounds, depth))
+    import fuzzscene
+    nrm = np.tile(np.float32([0.0, 0.0, 1.0]), (3 * n, 1))
+    cdf = np.linspace(0, 1, n, dtype=np.float32)      # never sampled: the mesh is not a light
+    m = abi.Mesh()
+    m.positions, m.normals = pos.ctypes.data_as(abi.c_float_p), nrm.ctypes.data_as(abi.c_float_p)
+    m.indices, m.cdf = idx.ctypes.data_as(abi.c_int_p), cdf.ctypes.data_as(abi.c_float_p)
+    m.nodes = nodes.ctypes.data_as(C.POINTER(abi.BvhNode))
+    m.numVertices, m.numIndices, m.numNodes, m.area = 3 * n, 3 * n, 2 * n - 1, 1.0
+    prims = (abi.Primitive * 3)()
+    rng2 = np.random.RandomState(0)
+    bounds = [fuzzscene._floor(prims[0], rng2)]
+    prims[1].type, prims[1].mesh = abi.MESH, 0
+    fuzzscene._xf(prims[1].start, (0.0, 1.2, 0.0), (0, 0, 0, 1), 1.0)
+    fuzzscene._xf(prims[1].end, (0.0, 1.2, 0.0), (0, 0, 0, 1), 1.0)
+    prims[1].material = fuzzscene._material(rng2, False)
+    bounds.append((np.float32([-1.1, 0.1, -1.1]), np.float32([1.1, 2.3, 1.1])))
+    bounds.append(fuzzscene._sphere(prims[2], (0.0, 3.0, 2.0), 0.3, fuzzscene._material(rng2, True), 1))
+    sc, keep = fuzzscene.make_scene_struct(prims, fuzzscene._build_bvh(bounds), [])
+    meshes = (abi.Mesh * 1)(m)
+    sc.meshes, sc.numMeshes = C.cast(meshes, C.POINTER(abi.Mesh)), 1
+    base = tb.Snapshot(tb.scene_path("cornell"))
+    cam, opt = abi.copy_struct(base.camera), abi.copy_struct(base.options)
+    base.close()
+    cam.position[:] = [0.0, 1.2, 4.0]
+    cam.rotation[:] = [0.0, 0.0, 0.0, 1.0]
+    opt.width, opt.height, opt.maxDepth = 96, 64, 3
+    oracle = refdrv.PortScene(C.pointer(sc), cam, opt, keepalive=(keep, meshes, nodes, pos, nrm, idx, cdf))
+    os.environ["TINSEL_B200_PIPELINE"] = "wavefront"
+    r = tb.Renderer(C.pointer(sc))
+    r.Init(96, 64)
+    rad, ras = r.trace_frame(cam, opt, 0)
+    orad, oras = oracle.trace_frame(0, 8)
+    assert np.array_equal(ras, oras)
+    same = (rad.view(np.uint32) == orad.view(np.uint32)).all(-1) | (np.isnan(rad).any(-1) & np.isnan(orad).any(-1))
+    assert bool(same.all()), "%d samples differ on the 1.5 M triangle tree" % int((~same).sum())
+    r.close()
+    oracle.close()

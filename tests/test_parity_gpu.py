@@ -13,6 +13,7 @@ import pytest
 import tinsel_b200 as tb
 from tinsel_b200 import abi
 import refdrv
+import schedenv
 
 pytestmark = pytest.mark.gpu
 
@@ -267,26 +268,14 @@ def test_max_depth_edge_cases(depth, pipeline):
     snap.close()
 
 
-@pytest.mark.parametrize("cta", ["512", "768"])
-@pytest.mark.parametrize("sched", ["hard", "free", "ring", "split", "treelet", "offload", "offload1", "offload100"])
+@pytest.mark.parametrize("cta", schedenv.CTAS)
+@pytest.mark.parametrize("sched", schedenv.SCHEDS)
 def test_both_scheduling_modes_bit_exact(sched, cta):
     """Every scheduler variant x CTA size of the wavefront kernel (the per-scene heuristics of
-    api.cu build_scene pick one of them) produces the same bits: hard phases, free running, free
-    running with the split trace queue forced on for every scene that has a mesh, and the mesh-walk
-    offload (shader CTAs + walker CTAs, wavefront_walk.cuh) forced on for every mesh, with the
-    default number of walker CTAs, a single one, and as many as fit; "treelet" = free running with the top
-    of the biggest mesh's BVH staged in shared memory for the inline walk.  "free" at 512 threads runs the
-    lane-owned slot layout with bit-set queues on every scene without a split queue, "ring" the ring queues."""
-    offload = sched.startswith("offload")
-    os.environ["TINSEL_B200_SCHED"] = "free" if sched in ("split", "treelet", "ring") or offload else sched
-    os.environ["TINSEL_B200_QUEUES"] = "ring" if sched == "ring" else "lanes"
-    os.environ["TINSEL_B200_TREELET"] = "1" if sched == "treelet" else "0"   # top of the biggest mesh's BVH TMA-staged for the inline walk
-    os.environ["TINSEL_B200_SPLIT"] = "1" if sched == "split" else "0"
-    os.environ["TINSEL_B200_OFFLOAD"] = "2" if offload else "0"
-    if sched in ("offload1", "offload100"):
-        os.environ["TINSEL_B200_WALKERS"] = sched[len("offload"):]
-    os.environ["TINSEL_B200_CTA"] = cta
-    try:
+    api.cu build_scene pick one of them, see schedenv.sched_env) produces the same bits.  "free" at 512
+    threads runs the lane-owned slot layout with bit-set queues on every scene without a split queue, "ring"
+    the ring queues."""
+    with schedenv.sched_env(sched, cta):
         for name in ("veach", "meshlight", "many", "envmini", "glass", "table", "ajax", "motionblur"):
             if not _available(name):
                 continue
@@ -298,10 +287,6 @@ def test_both_scheduling_modes_bit_exact(sched, cta):
             r.close()
             ref.close()
             snap.close()
-    finally:
-        for k in ("TINSEL_B200_SCHED", "TINSEL_B200_SPLIT", "TINSEL_B200_CTA", "TINSEL_B200_OFFLOAD", "TINSEL_B200_WALKERS", "TINSEL_B200_TREELET",
-                  "TINSEL_B200_QUEUES"):
-            os.environ.pop(k, None)
 
 
 def test_box_filter_and_clamp():

@@ -574,7 +574,7 @@ bool setup_offload(tb200_renderer* r, const SceneImage& img)
         const DPrim& p = img.prims[i];
         if (p.type != TB200_MESH) continue;
         const MeshImage& mi = img.meshes[p.mesh];
-        if ((mi.numTris > 4096 || force) && mi.depth <= TB_STACK) {
+        if ((mi.numTris > 4096 || force) && mi.depth <= TB200_MAX_BVH_LEVELS) {
             sc.deferMask |= 1u << i;
             if (mi.numTris > bigTris) {
                 bigTris = mi.numTris;
@@ -844,7 +844,29 @@ bool image_load(const char* path, SceneImage* img)
     return true;
 }
 
-// every index a kernel will follow stays inside its array (a cache file is as untrusted as a tb200_scene)
+// levels: tb_tree_levels' result for the BVH called `what`
+bool bvh_levels_ok(int levels, const std::string& what, std::string* why)
+{
+    if (levels < 0) return *why = what + ": a BVH node is reached twice from the root (shared subtree or cycle)", false;
+    if (levels > TB200_MAX_BVH_LEVELS)
+        return *why = what + ": BVH has " + std::to_string(levels) + " levels of interior nodes, more than the " +
+                      std::to_string(TB200_MAX_BVH_LEVELS) + " the traversal stack holds", false;
+    return true;
+}
+
+// levels of the BvhPair tree below `root`, or -1 (see tb_tree_levels)
+int pair_levels(const std::vector<BvhPair>& pairs, uint32_t root)
+{
+    return tb_tree_levels(root, pairs.size(), [&pairs](uint32_t ref, uint32_t* c) {
+        if (ref & TB_LEAF) return false;
+        c[0] = pairs[ref].left;
+        c[1] = pairs[ref].right;
+        return true;
+    });
+}
+
+// every index a kernel will follow stays inside its array, and every BVH is a tree the traversal stack can
+// hold (a cache file is as untrusted as a tb200_scene)
 bool validate_image(const SceneImage& img, std::string* why)
 {
     const size_t np = img.prims.size();
@@ -853,12 +875,20 @@ bool validate_image(const SceneImage& img, std::string* why)
     if (!ref_ok(img.sceneRoot, img.scenePairs.size(), np)) return *why = "scene root reference out of range", false;
     for (const BvhPair& p : img.scenePairs)
         if (!ref_ok(p.left, img.scenePairs.size(), np) || !ref_ok(p.right, img.scenePairs.size(), np)) return *why = "scene BVH reference out of range", false;
-    for (const MeshImage& m : img.meshes) {
+    if (!bvh_levels_ok(pair_levels(img.scenePairs, img.sceneRoot), "scene", why)) return false;
+    for (size_t k = 0; k < img.meshes.size(); ++k) {
+        const MeshImage& m = img.meshes[k];
         const size_t nt = (size_t)std::max(0, m.numTris);
         if (nt == 0 || m.verts.size() != nt * 3 || m.norms.size() != nt * 3 || m.cdf.size() != nt) return *why = "mesh arrays do not match the triangle count", false;
         if (!ref_ok(m.rootRef, m.pairs.size(), nt)) return *why = "mesh root reference out of range", false;
         for (const BvhPair& p : m.pairs)
             if (!ref_ok(p.left, m.pairs.size(), nt) || !ref_ok(p.right, m.pairs.size(), nt)) return *why = "mesh BVH reference out of range", false;
+        const std::string name = "mesh " + std::to_string(k);
+        if (m.depth < 0 || m.depth > TB200_MAX_BVH_LEVELS)
+            return *why = name + ": stored BVH depth " + std::to_string(m.depth) + " is outside 0.." + std::to_string(TB200_MAX_BVH_LEVELS), false;
+        const int levels = pair_levels(m.pairs, m.rootRef);
+        if (!bvh_levels_ok(levels, name, why)) return false;
+        if (levels != m.depth) return *why = name + ": stored BVH depth does not match the tree", false;
     }
     for (const DPrim& p : img.prims) {
         if (p.type != TB200_SPHERE && p.type != TB200_PLANE && p.type != TB200_MESH) return *why = "unknown primitive type", false;
@@ -1196,7 +1226,8 @@ const char* tb200_last_error(void)
 }
 
 // Structural checks on the caller's scene before anything is uploaded: every index the kernels will
-// follow must stay inside its array (the reference trusts its own loader; a C ABI cannot).
+// follow must stay inside its array, and every BVH must be a tree no deeper than the traversal stack holds
+// (the reference trusts its own loader; a C ABI cannot).
 static bool validate_bvh(const tb200_bvh_node* nodes, int numNodes, int numItems, const char* what, std::string* why)
 {
     if (numNodes <= 0 || !nodes) {
@@ -1211,7 +1242,13 @@ static bool validate_bvh(const tb200_bvh_node* nodes, int numNodes, int numItems
             return false;
         }
     }
-    return true;
+    const int levels = tb_tree_levels(0u, (size_t)numNodes, [nodes](uint32_t i, uint32_t* c) {
+        if (nodes[i].right_leaf >> 31) return false;
+        c[0] = nodes[i].left;
+        c[1] = nodes[i].right_leaf & 0x7fffffffu;
+        return true;
+    });
+    return bvh_levels_ok(levels, what, why);
 }
 
 static bool validate_scene(const tb200_scene* s, std::string* why)

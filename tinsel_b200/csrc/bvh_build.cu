@@ -350,6 +350,28 @@ bool build_on_device(const float* positions, int numVertices, const int32_t* ind
     cudaEventElapsedTime(&ms, ev0, ev1);
     cudaEventDestroy(ev0);
     cudaEventDestroy(ev1);
+    // PLOC puts no bound on depth (a nested series of ever smaller triangles clusters into a chain), and
+    // tb200_create refuses a tree deeper than the traversal stack holds.  Levels in one pass: k_emit numbers
+    // interior nodes in reverse creation order and children are created before their parent, so every
+    // child's index is larger than its parent's.
+    {
+        std::vector<int> level((size_t)numInterior, 0);
+        int levels = 1;
+        level[0] = 1;
+        for (int i = 0; i < numInterior; ++i) {
+            const uint32_t kids[2] = {outNodes[i].left, outNodes[i].right_leaf & 0x7fffffffu};
+            for (uint32_t c : kids)
+                if (c < (uint32_t)numInterior) {
+                    level[c] = level[i] + 1;
+                    levels = std::max(levels, level[c]);
+                }
+        }
+        if (levels > TB200_MAX_BVH_LEVELS) {
+            memset(outNodes, 0, (size_t)(2 * numTris - 1) * sizeof(tb200_bvh_node));
+            return fail("the tree has " + std::to_string(levels) + " levels of interior nodes, more than the " +
+                        std::to_string(TB200_MAX_BVH_LEVELS) + " the traversal stack holds");
+        }
+    }
     if (info) {
         info->numNodes = 2 * numTris - 1;
         info->rounds = rounds;

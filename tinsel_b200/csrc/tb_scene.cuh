@@ -15,6 +15,10 @@
 //                 index -> vertex double indirection (intersection.h:638-644).
 #pragma once
 
+#include <algorithm>
+#include <utility>
+#include <vector>
+
 #include "tinsel_b200.h"
 #include "tb_math.cuh"
 
@@ -26,6 +30,37 @@
 #define TB_ORDERED_ATTR static __device__ __noinline__
 #endif
 #define TB_STACK 32  // the reference uses int stack[32] (intersection.h:688,759)
+// Interior levels a BVH may have (TB200_MAX_BVH_LEVELS, checked by validate_bvh / validate_image in api.cu).
+// The walks below pop one entry and push up to both children.  Visiting an interior node at level k
+// (root = 1) leaves at most k + 1 entries on the stack: one pending sibling per level above plus its own
+// two children.  So a tree with L interior levels needs L + 1 entries, and L <= TB_STACK - 1.
+static_assert(TB200_MAX_BVH_LEVELS == TB_STACK - 1, "the BVH depth bound must match the traversal stack");
+
+// Host side: interior levels of the binary tree below `root` (0 when the root is a leaf), or -1 when a node
+// is reached twice (a shared subtree or a cycle).  children(id, c) returns false for a leaf, else stores the
+// two child ids in c.  Ids >= numIds are leaves that need no tracking (the TB_LEAF references of BvhPair
+// records); every id below it is checked to be reached once.  Child ids must already be range-checked.
+template <class Children>
+inline int tb_tree_levels(uint32_t root, size_t numIds, Children children)
+{
+    std::vector<unsigned char> seen(numIds, 0);
+    std::vector<std::pair<uint32_t, int>> todo(1, std::make_pair(root, 1));
+    int levels = 0;
+    uint32_t c[2];
+    while (!todo.empty()) {
+        const std::pair<uint32_t, int> it = todo.back();
+        todo.pop_back();
+        if (it.first < numIds) {
+            if (seen[it.first]) return -1;
+            seen[it.first] = 1;
+        }
+        if (!children(it.first, c)) continue;
+        levels = std::max(levels, it.second);
+        todo.push_back(std::make_pair(c[0], it.second + 1));
+        todo.push_back(std::make_pair(c[1], it.second + 1));
+    }
+    return levels;
+}
 
 struct __align__(16) BvhPair {
     float4 a;   // L.lower.xyz, L.upper.x
