@@ -74,7 +74,9 @@ TB_DEV void sample_end(const LaunchParams& P, int px, int py, float rasterX, flo
 // functions the wavefront kernel uses, so that a parity failure can be bisected between "math"
 // and "scheduling".
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_mega(LaunchParams P)
+// (P is __grid_constant__: the stage functions take P.scene by reference, which would otherwise make a per-thread
+// copy of the parameters in local memory)
+__global__ void __launch_bounds__(128) k_mega(const __grid_constant__ LaunchParams P)
 {
     const unsigned long long idx = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= P.samplesPerFrame * (unsigned long long)P.numFrames) return;
@@ -119,7 +121,7 @@ void launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned long long*
 // ------------------------------------------------------------------------------------------------
 // eNormals (render.cpp:494-515): ray through the integer raster position, time 1.0, overwrite.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_normals(LaunchParams P)
+__global__ void __launch_bounds__(128) k_normals(const __grid_constant__ LaunchParams P)
 {
     const int W = P.film.width;
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;

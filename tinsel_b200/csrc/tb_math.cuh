@@ -164,9 +164,16 @@ TB_DEV uint32_t tb_sample_seed(uint32_t pixel, uint32_t frame)
 }
 
 // Out-of-line device copies of the double-precision transcendentals: they are called from a dozen
-// sites and inlining every copy bloats the kernel far past the instruction cache.
+// sites and inlining every copy bloats the kernel far past the instruction cache.  Results come back
+// as return values, which stay in registers; out-pointers would go through the caller's stack.
 #define TB_NOINLINE static __device__ __noinline__
-TB_NOINLINE void tb_sincosf(float x, float* s, float* c) { tbm_sincosf(x, s, c); }
+// (sinf(x), cosf(x))
+TB_NOINLINE float2 tb_sincosf(float x)
+{
+    float s, c;
+    tbm_sincosf(x, &s, &c);
+    return make_float2(s, c);
+}
 TB_NOINLINE float tb_expf(float x) { return tbm_expf(x); }
 
 #define TB_PI 3.141592653589793f
@@ -195,8 +202,8 @@ TB_DEV V3 uniform_sample_sphere(float u1, float u2)
     const float z = 1.f - 2.f * u1;
     const float r = sqrtf(tb_max(0.f, 1.f - z * z));
     const float phi = 2.f * TB_PI * u2;
-    float s, c;
-    tb_sincosf(phi, &s, &c);
+    const float2 sc = tb_sincosf(phi);
+    const float s = sc.x, c = sc.y;
     return v3(r * c, r * s, z);
 }
 
@@ -206,8 +213,8 @@ TB_DEV V3 uniform_sample_hemisphere(Rng& rng)
     const float z = rng_float(rng);
     const float w = sqrtf(1.0f - z * z);
     const float phi = TB_2PI * rng_float(rng);
-    float s, c;
-    tb_sincosf(phi, &s, &c);
+    const float2 sc = tb_sincosf(phi);
+    const float s = sc.x, c = sc.y;
     return v3(c * w, s * w, z);
 }
 
@@ -216,8 +223,8 @@ TB_DEV V3 cosine_sample_hemisphere(float u1, float u2)
 {
     const float r = sqrtf(u1);
     const float theta = TB_2PI * u2;
-    float s, c;
-    tb_sincosf(theta, &s, &c);
+    const float2 sc = tb_sincosf(theta);
+    const float s = sc.x, c = sc.y;
     const float sx = r * c, sy = r * s;
     const float z = sqrtf(tb_max(0.0f, 1.0f - sx * sx - sy * sy));
     return v3(sx, sy, z);

@@ -156,10 +156,17 @@ TB_DEV V3 bsdf_eval(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3
 }
 
 // BSDFPdf + BSDFEval for the same (V, L): one out-of-line copy serves NEE and the BSDF sample
-TB_NOINLINE void bsdf_eval_pdf(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3 L, V3* f, float* pdf)
+struct BsdfValue {
+    V3 f;        // BSDFEval
+    float pdf;   // BSDFPdf
+};
+
+TB_NOINLINE BsdfValue bsdf_eval_pdf(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3 L)
 {
-    *pdf = bsdf_pdf(mat, etaI, etaO, N, V, L);
-    *f = bsdf_eval(mat, etaI, etaO, N, V, L);
+    BsdfValue r;
+    r.pdf = bsdf_pdf(mat, etaI, etaO, N, V, L);
+    r.f = bsdf_eval(mat, etaI, etaO, N, V, L);
+    return r;
 }
 
 // the GGX half-vector lobe shared by both branches of BSDFSample, disney.h:183-205 / 256-279;
@@ -226,8 +233,8 @@ TB_DEV bool bsdf_sample_dir(const DMaterial& mat, float etaI, float etaO, V3 U, 
             type = TB_REFLECTED;
         }
     }
-    float sn, cs;
-    tb_sincosf(angleArg * TB_2PI, &sn, &cs);
+    const float2 sca = tb_sincosf(angleArg * TB_2PI);
+    const float sn = sca.x, cs = sca.y;
     if (lobe == LOBE_GGX) {
         light = sample_ggx_reflection(mat, r2, sn, cs, U, Vt, N, view);
     } else if (lobe == LOBE_COSINE) {
@@ -246,13 +253,12 @@ TB_DEV bool bsdf_sample_dir(const DMaterial& mat, float etaI, float etaO, V3 U, 
 
 // ---- probe / sky (probe.h, scene.h:161-181) -------------------------------------------------------
 
-// ProbeDirToUV, probe.h:105-113 (out of line: the double-precision acos/atan2 are large)
-TB_NOINLINE void probe_dir_to_uv(V3 dir, float& u, float& v)
+// ProbeDirToUV, probe.h:105-113 (out of line: the double-precision acos/atan2 are large); returns (u, v)
+TB_NOINLINE float2 probe_dir_to_uv(V3 dir)
 {
     const float theta = tbm_acosf(tb_clamp(dir.y, -1.0f, 1.0f));
     const float phi = (dir.x == 0.0f && dir.z == 0.0f) ? 0.0f : tbm_atan2f(dir.z, dir.x);
-    u = (TB_PI + phi) * TB_INV_PI * 0.5f;
-    v = theta * TB_INV_PI;
+    return make_float2((TB_PI + phi) * TB_INV_PI * 0.5f, theta * TB_INV_PI);
 }
 
 // ProbeEval, probe.h:128-134
@@ -311,9 +317,8 @@ TB_DEV void probe_sample(const DProbe& pr, V3& dir, V3& color, float& pdf, Rng& 
     // ProbeUVToDir, probe.h:115-125
     const float theta = v * TB_PI;
     const float phi = u * 2.0f * TB_PI;
-    float st, ct, sp, cp;
-    tb_sincosf(theta, &st, &ct);
-    tb_sincosf(phi, &sp, &cp);
+    const float2 sct = tb_sincosf(theta), scp = tb_sincosf(phi);
+    const float st = sct.x, ct = sct.y, sp = scp.x, cp = scp.y;
     dir = v3(-st * cp, ct, -st * sp);
 }
 
@@ -408,7 +413,12 @@ TB_DEV void path_miss(const DScene& sc, PathState& ps, int bounce)
 {
     float weight = 1.0f;
     float u = 0.0f, v = 0.0f;
-    if (sc.probe.valid) probe_dir_to_uv(ps.d, u, v);   // shared by ProbePdf and Sky::Eval (both call ProbeDirToUV(rayDir))
+    if (sc.probe.valid) {
+        // shared by ProbePdf and Sky::Eval (both call ProbeDirToUV(rayDir))
+        const float2 uv = probe_dir_to_uv(ps.d);
+        u = uv.x;
+        v = uv.y;
+    }
     if (sc.probe.valid && bounce > 0 && ps.rayType != TB_SPECULAR) {
         const float skyPdf = probe_pdf(sc.probe, u, v);
         const float cbsdf = 0.5f, csky = 0.5f;   // kBsdfSamples/N, kProbeSamples/N with N = 2
@@ -537,7 +547,11 @@ TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr
     }
     V3 f = v3s(0.0f);
     float bsdfPdf = 0.0f;
-    if (need) bsdf_eval_pdf(mat, sf.etaI, sf.etaO, sf.n, sf.wo, sr.d, &f, &bsdfPdf);
+    if (need) {
+        const BsdfValue b = bsdf_eval_pdf(mat, sf.etaI, sf.etaO, sf.n, sf.wo, sr.d);
+        f = b.f;
+        bsdfPdf = b.pdf;
+    }
 
     if (isProbe) {
         if (need && bsdfPdf > 0.0f) {
@@ -585,9 +599,9 @@ TB_DEV bool path_scatter(const DScene& sc, PathState& ps, const Surface& sf, V3 
     V3 f = v3s(0.0f);
     if (pdfFromBsdf || pdf > 0.0f) {
         // pdf = BSDFPdf(dir) (disney.h:291) and f = BSDFEval(dir) (render.cpp:341) share one call
-        float p2 = 0.0f;
-        bsdf_eval_pdf(prim.mat, sf.etaI, sf.etaO, sf.n, sf.wo, bsdfDir, &f, &p2);
-        if (pdfFromBsdf) pdf = p2;
+        const BsdfValue b = bsdf_eval_pdf(prim.mat, sf.etaI, sf.etaO, sf.n, sf.wo, bsdfDir);
+        f = b.f;
+        if (pdfFromBsdf) pdf = b.pdf;
     }
     ps.bsdfPdf = pdf;
     if (pdf <= 0.0f) return false;

@@ -116,6 +116,10 @@ struct Wf2Shared {
     unsigned int ansHead[2];
     int ansPending[2];
     int exitSignaled;
+    // the scene descriptor every stage reads, pointing at the staged tables below: one copy per CTA, filled by
+    // thread 0 in the prologue.  A per-thread copy would live in local memory (the stages take it by reference),
+    // where every field read is a dependent L1 / L2 round trip at the head of a stage.
+    DScene scene;
     // scene tables staged on chip by bulk copies (TMA) that complete on `stageBar`
     alignas(16) DPrim prims[TB_WF2_MAX_PRIMS + 1];   // +1: the copy length is rounded up to 16 bytes
     alignas(16) BvhPair pairs[TB_WF2_MAX_PAIRS];
@@ -531,7 +535,7 @@ TB_DEV void wf2_merge_answer(Wf2Shared& S, const DScene& sc, int s, bool isExt, 
 enum { WF2_MODE_GENERIC = 0, WF2_MODE_HARD = 1, WF2_MODE_SPLIT = 2, WF2_MODE_OFFLOAD = 3 };
 
 template <int THREADS, int MODE>
-__global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(LaunchParams P, unsigned long long total)
+__global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(const __grid_constant__ LaunchParams P, unsigned long long total)
 {
     extern __shared__ __align__(16) unsigned char wf_smem_raw[];
     Wf2Shared& S = *reinterpret_cast<Wf2Shared*>(wf_smem_raw);
@@ -547,18 +551,17 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(Laun
     // global to shared memory as TMA bulk copies (cp.async.bulk -> UBLKCP): thread 0 arms an mbarrier
     // with the byte count and issues up to three copies, everybody waits on the barrier's phase.  (The
     // walker CTAs of the offload mode stage the top of the big mesh's BVH the same way.)
-    DScene sc = P.scene;
-    const bool stagePrims = sc.numPrims <= TB_WF2_MAX_PRIMS;
-    const bool stagePairs = sc.numPairs > 0 && sc.numPairs <= TB_WF2_MAX_PAIRS;
-    const bool stageFlat = sc.numFlat > 0 && sc.numFlat <= 32;
+    const bool stagePrims = P.scene.numPrims <= TB_WF2_MAX_PRIMS;
+    const bool stagePairs = P.scene.numPairs > 0 && P.scene.numPairs <= TB_WF2_MAX_PAIRS;
+    const bool stageFlat = P.scene.numFlat > 0 && P.scene.numFlat <= 32;
     if (tid == 0) {
         const uint32_t bar = walk_smem_addr(&S.stageBar);
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         // device arrays are padded by one element (api.cu: upload_image), so rounding up stays inside them
-        const uint32_t primBytes = stagePrims ? (((uint32_t)sc.numPrims * (uint32_t)sizeof(DPrim) + 15u) & ~15u) : 0u;
-        const uint32_t pairBytes = stagePairs ? (uint32_t)sc.numPairs * (uint32_t)sizeof(BvhPair) : 0u;
-        const uint32_t flatBytes = stageFlat ? (uint32_t)sc.numFlat * (uint32_t)sizeof(ProgOp) : 0u;
+        const uint32_t primBytes = stagePrims ? (((uint32_t)P.scene.numPrims * (uint32_t)sizeof(DPrim) + 15u) & ~15u) : 0u;
+        const uint32_t pairBytes = stagePairs ? (uint32_t)P.scene.numPairs * (uint32_t)sizeof(BvhPair) : 0u;
+        const uint32_t flatBytes = stageFlat ? (uint32_t)P.scene.numFlat * (uint32_t)sizeof(ProgOp) : 0u;
         const bool stageTreelet = P.treeletBytes >= (int)sizeof(BvhPair) && P.scene.treeletMesh >= 0;
         const uint32_t treeBytes = stageTreelet ? (uint32_t)min(P.scene.treeletPairs, P.treeletBytes / (int)sizeof(BvhPair)) * (uint32_t)sizeof(BvhPair) : 0u;
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(primBytes + pairBytes + flatBytes + treeBytes) : "memory");
@@ -584,21 +587,25 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(Laun
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(walk_smem_addr(S.flat)),
                          "l"(P.scene.flat), "r"(flatBytes), "r"(bar)
                          : "memory");
+        // the CTA's scene descriptor (Wf2Shared::scene), published by the barrier below
+        DScene d = P.scene;
+        if (stagePrims) d.prims = S.prims;
+        if (stagePairs) d.pairs = S.pairs;
+        if (stageFlat) d.flat = S.flat;
+        // the top of the biggest mesh's BVH goes into whatever shared memory the slot arrays leave (P.treeletBytes,
+        // set by the launch from the device's limit): the first levels of every inline mesh walk are then shared-
+        // memory reads instead of dependent L2 round trips
+        d.treelet = nullptr;
+        if (P.treeletBytes >= (int)sizeof(BvhPair) && d.treeletMesh >= 0) {
+            unsigned char* tl = wf_smem_raw + ((sizeof(Wf2Shared) + 127) & ~size_t(127));
+            d.treeletPairs = min(d.treeletPairs, P.treeletBytes / (int)sizeof(BvhPair));
+            d.treelet = walk_opaque(tl);
+        } else {
+            d.treeletPairs = 0;
+        }
+        S.scene = d;
     }
-    if (stagePrims) sc.prims = S.prims;
-    if (stagePairs) sc.pairs = S.pairs;
-    if (stageFlat) sc.flat = S.flat;
-    // the top of the biggest mesh's BVH goes into whatever shared memory the slot arrays leave (P.treeletBytes,
-    // set by the launch from the device's limit): the first levels of every inline mesh walk are then shared-
-    // memory reads instead of dependent L2 round trips
-    sc.treelet = nullptr;
-    if (P.treeletBytes >= (int)sizeof(BvhPair) && sc.treeletMesh >= 0) {
-        unsigned char* tl = wf_smem_raw + ((sizeof(Wf2Shared) + 127) & ~size_t(127));
-        sc.treeletPairs = min(sc.treeletPairs, P.treeletBytes / (int)sizeof(BvhPair));
-        sc.treelet = walk_opaque(tl);
-    } else {
-        sc.treeletPairs = 0;
-    }
+    const DScene& sc = S.scene;
     // every slot starts in the R queue "finished with nothing to splat": stage R fills it with a
     // camera sample
 #ifdef TB_WF2_LANEQ
@@ -633,7 +640,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(Laun
             S.ansHead[1] = walk_ld1(P.walk.ansTail + blockIdx.x * 2 + 1);
         }
     }
-    __syncthreads();   // the barrier word is initialised (thread 0, above) before anybody polls it
+    __syncthreads();   // the barrier word and S.scene are initialised (thread 0, above) before anybody reads them
     {
         uint32_t landed = 0;
         while (!landed)

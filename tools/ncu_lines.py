@@ -20,19 +20,23 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.environ.get("TINSEL_B200_LIB") or os.path.join(ROOT, "tinsel_b200", "libtinsel_b200.so")
 
 
-def line_table(kernel):
+def sass_listing(kernel):
+    """[(section, address, (file, line) or None, instruction)] of the kernels whose section names contain `kernel`.
+    A kernel's out-of-line callees are copied into its section, so they are part of the listing."""
     tmp = tempfile.mkdtemp()
     subprocess.check_call(["cuobjdump", "-xelf", "all", LIB], cwd=tmp, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-    table = {}
+    listing = []
     for f in os.listdir(tmp):
         if not f.startswith("kernels"):
             continue
         out = subprocess.check_output(["nvdisasm", "-g", "-c", os.path.join(tmp, f)], text=True, stderr=subprocess.DEVNULL)
         cur = None
         inside = False
+        section = None
         for ln in out.splitlines():
             if ln.startswith(".text."):
                 inside = kernel in ln
+                section = ln[len(".text."):].rstrip(":")
                 cur = None
                 continue
             if not inside:
@@ -41,10 +45,14 @@ def line_table(kernel):
             if m:
                 cur = (os.path.basename(m.group(1)), int(m.group(2)))
                 continue
-            m = re.match(r"\s+/\*([0-9a-f]{4,6})\*/", ln)
+            m = re.match(r"\s+/\*([0-9a-f]{4,6})\*/\s*(.*?)\s*;?\s*$", ln)
             if m:
-                table[int(m.group(1), 16)] = cur
-    return table
+                listing.append((section, int(m.group(1), 16), cur, m.group(2)))
+    return listing
+
+
+def line_table(kernel):
+    return {addr: key for _, addr, key, _ in sass_listing(kernel)}
 
 
 def function_of_line():
