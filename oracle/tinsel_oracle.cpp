@@ -1008,6 +1008,38 @@ void oracle_trace_frame(void* h, const tb200_camera* cam, const tb200_options* o
     });
 }
 
+// Box-filter footprint counts of frames [frame0, frame0 + nframes) without tracing a path: each sample's
+// raster position exactly as trace_sample draws it, then add_sample's footprint (render.cpp:404-423),
+// adding 1 per covered pixel into caller-zeroed `counts` (H*W).  A box-filtered film's weight channel
+// must equal these counts, also at sample counts far beyond what tracing on the host can reach.
+void oracle_box_counts(const tb200_options* o, int frame0, int nframes, uint64_t* counts, int nthreads)
+{
+    const int W = o->width, H = o->height;
+    if (nthreads < 1) nthreads = 1;
+    if (nthreads > nframes) nthreads = nframes < 1 ? 1 : nframes;
+    std::vector<std::vector<uint64_t>> bufs(nthreads, std::vector<uint64_t>((size_t)W * H, 0));
+    std::vector<std::thread> th;
+    for (int t = 0; t < nthreads; ++t)
+        th.emplace_back([&, t] {
+            uint64_t* c = bufs[t].data();
+            for (long long k = frame0 + (long long)nframes * t / nthreads; k < frame0 + (long long)nframes * (t + 1) / nthreads; ++k)
+                for (int j = 0; j < H; ++j)
+                    for (int i = 0; i < W; ++i) {
+                        rng_t rng = rng_make(tb200_sample_seed((uint32_t)(j * W + i), (uint32_t)k));
+                        float x = rng_f(rng), y = rng_f(rng);
+                        x += i;
+                        y += j;
+                        int sx = imax2(0, int(x - o->filterWidth)), sy = imax2(0, int(y - o->filterWidth));
+                        int ex = imin2(int(x + o->filterWidth), W - 1), ey = imin2(int(y + o->filterWidth), H - 1);
+                        for (int px = sx; px <= ex; ++px)
+                            for (int py = sy; py <= ey; ++py) c[(size_t)py * W + px] += 1;
+                    }
+        });
+    for (auto& x : th) x.join();
+    for (int t = 0; t < nthreads; ++t)
+        for (size_t p = 0; p < (size_t)W * H; ++p) counts[p] += bufs[t][p];
+}
+
 // eNormals, render.cpp:494-515
 void oracle_render_normals(void* h, const tb200_camera* cam, const tb200_options* o, float* out)
 {

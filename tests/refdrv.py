@@ -231,6 +231,7 @@ def load_port():
     lib.oracle_render_seeded.argtypes = [C.c_void_p, C.POINTER(abi.Camera), C.POINTER(abi.Options), C.c_int, C.c_int, _f32p, C.c_int]
     lib.oracle_trace_frame.argtypes = [C.c_void_p, C.POINTER(abi.Camera), C.POINTER(abi.Options), C.c_int, _f32p, _f32p, C.c_int]
     lib.oracle_render_normals.argtypes = [C.c_void_p, C.POINTER(abi.Camera), C.POINTER(abi.Options), _f32p]
+    lib.oracle_box_counts.argtypes = [C.POINTER(abi.Options), C.c_int, C.c_int, C.POINTER(C.c_uint64), C.c_int]
     lib.oracle_random_u32.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_uint32)]
     lib.oracle_random_f32.argtypes = [C.c_int, C.c_int, _f32p]
     lib.oracle_material_ior.restype = C.c_float
@@ -311,6 +312,14 @@ class PortScene:
         o = self.options
         out = np.zeros((o.height, o.width, 4), np.float32)
         self.lib.oracle_render_normals(self.h, C.byref(self.camera), C.byref(o), _fp(out))
+        return out
+
+    def box_counts(self, frame0, nframes, nthreads=1):
+        """(H,W) uint64: how many box-filter terms each pixel receives from frames [frame0, frame0+nframes),
+        from the raster positions alone (no path is traced)."""
+        o = self.options
+        out = np.zeros((o.height, o.width), np.uint64)
+        self.lib.oracle_box_counts(C.byref(o), frame0, nframes, out.ctypes.data_as(C.POINTER(C.c_uint64)), nthreads)
         return out
 
     def close(self):

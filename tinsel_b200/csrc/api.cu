@@ -358,6 +358,9 @@ struct tb200_renderer {
     int tunePhase = 3;            // 0 warm-up (split), 1 measuring split, 2 measuring no split, 3 decided
     double tuneRate[2] = {0.0, 0.0};   // samples per ms with / without the split queue
     unsigned long long launchSamples = 0;   // samples of the launch whose time is in stats.gpuMs
+    // most samples (tile padding included) per launch: slot records keep a 32-bit sample index.
+    // TINSEL_B200_TEST_LAUNCH_SAMPLES lowers it, so that tests reach the split at small sizes.
+    unsigned long long maxLaunchSamples = 0x7fffffffull;
     tb200_stats stats;
 };
 
@@ -970,7 +973,7 @@ bool launch_frames(tb200_renderer* r, LaunchParams& P, bool recordStart = true)
     if (recordStart) TB_CUDA(cudaEventRecord(r->evStart, r->stream));
     if (P.samplesPerFrame > 0) {
         // slot records keep a 32-bit sample index: split very long jobs into several launches
-        const int framesPerLaunch = (int)std::max<unsigned long long>(1ull, 0x7fffffffull / P.samplesPerFrame);
+        const int framesPerLaunch = (int)std::max<unsigned long long>(1ull, r->maxLaunchSamples / P.samplesPerFrame);
         const int frame0 = P.frame0, frames = P.numFrames;
         for (int f = 0; f < frames; f += framesPerLaunch) {
             P.frame0 = frame0 + f;
@@ -1374,6 +1377,10 @@ static tb200_renderer* create_with(int device, const std::function<bool(tb200_re
     if (pipe && strcmp(pipe, "mega") == 0) r->pipeline = 0;
     const char* rb = getenv("TINSEL_B200_READBACK");
     if (rb && strcmp(rb, "plain") == 0) r->streamedReadback = 0;
+    if (const char* cap = getenv("TINSEL_B200_TEST_LAUNCH_SAMPLES")) {   // test hook: lowers the cap, never raises it
+        const unsigned long long n = strtoull(cap, nullptr, 10);
+        if (n > 0) r->maxLaunchSamples = std::min(n, r->maxLaunchSamples);
+    }
     unsigned int* hostFlags = nullptr;
     // cold slot state for every CTA a launch can have (one or two per SM, see launch_wavefront2)
     if (cudaMalloc((void**)&r->dCold, size_t(r->numSMs) * TB_WF2_MAX_CTAS_PER_SM * TB_WF2_SLOTS * 128) != cudaSuccess ||
