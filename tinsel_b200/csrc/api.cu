@@ -1985,6 +1985,25 @@ int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200
     return 0;
 }
 
+#ifdef TB_WF2_STAGE_CLOCKS
+// development builds only (-DTB_WF2_STAGE_CLOCKS, tools/stage_clocks.py): copies the lane-owned wavefront
+// layout's per-stage cycle counters of the current device into out[0..n) (n >= 15 words, see wavefront2.cuh:
+// Wf2Clocks) after the work queued so far has finished, and zeroes them when `reset` is set
+int tb200_stage_clocks(unsigned long long* out, int n, int reset)
+{
+    if (!out || n < TB_WF2_STAGE_CLOCK_WORDS) {
+        set_error("tb200_stage_clocks: need room for 15 counters");
+        return -1;
+    }
+    if (cudaDeviceSynchronize() != cudaSuccess) {
+        set_error(std::string("tb200_stage_clocks: ") + cudaGetErrorString(cudaGetLastError()));
+        return -1;
+    }
+    read_stage_clocks(out, reset != 0);
+    return TB_WF2_STAGE_CLOCK_WORDS;
+}
+#endif
+
 void tb200_set_frame(tb200_renderer* r, int frame)
 {
     if (!r) return;

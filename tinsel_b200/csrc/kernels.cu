@@ -338,6 +338,10 @@ namespace wf2_lq {
 #undef TB_WF2_COLD_SMEM
 }  // namespace wf2_lq
 
+#ifdef TB_WF2_STAGE_CLOCKS
+void read_stage_clocks(unsigned long long* out, bool reset) { wf2_lq::wf2_stage_clocks(out, reset); }
+#endif
+
 void launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
     // The lane-owned layout wins in the steady state (cornell 32 spp on an H100: 1131 vs 893 Msamples/s) and loses

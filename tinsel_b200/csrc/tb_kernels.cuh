@@ -67,6 +67,12 @@ void finalize_params(LaunchParams* p);
 void launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned long long* launchCount);
 // persistent CTA-resident wavefront pipeline with a dedicated traversal stage (the product path)
 void launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
+#ifdef TB_WF2_STAGE_CLOCKS
+// development builds: the per-stage cycle counters of the lane-owned wavefront layout (wavefront2.cuh), summed
+// over every launch since the last reset
+#define TB_WF2_STAGE_CLOCK_WORDS 15
+void read_stage_clocks(unsigned long long* out, bool reset);
+#endif
 // eNormals mode (render.cpp:494-515)
 void launch_normals(const LaunchParams& p, cudaStream_t stream, unsigned long long* launchCount);
 

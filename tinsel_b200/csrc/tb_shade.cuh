@@ -478,18 +478,20 @@ struct NeeCursor {
     V3 Lacc;         // running `L` of the current light
 };
 
-TB_DEV void nee_begin(NeeCursor& c)
+// firstLight: no primitive before it has lightSamples > 0 (0 when not known)
+TB_DEV void nee_begin(NeeCursor& c, int firstLight = 0)
 {
     c.slot = 0;
-    c.prim = 0;
+    c.prim = firstLight;
     c.sample = 0;
     c.sum = v3s(0.0f);
     c.Lacc = v3s(0.0f);
 }
 
 // Generates the next shadow ray (drawing the RNG exactly as the reference does).  Returns
-// false when all slots are exhausted.
-TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCursor& c, Rng& rng, ShadowRay& sr)
+// false when all slots are exhausted.  lightEnd: no primitive from there on has lightSamples > 0
+// (sc.numPrims when not known); the scan for the next light stops there.
+TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCursor& c, Rng& rng, ShadowRay& sr, int lightEnd)
 {
     if (c.slot == 0 && sc.probe.valid) {
         V3 wi, color;
@@ -505,11 +507,11 @@ TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCur
         return true;
     }
     // advance to the next primitive that still has samples to take
-    while (c.prim < sc.numPrims && c.sample >= sc.prims[c.prim].lightSamples) {
+    while (c.prim < lightEnd && c.sample >= sc.prims[c.prim].lightSamples) {
         c.prim++;
         c.sample = 0;
     }
-    if (c.prim >= sc.numPrims) return false;
+    if (c.prim >= lightEnd) return false;
     const DPrim& light = sc.prims[c.prim];
     V3 lightPos, lightNormal;
     prim_sample(sc, light, time, lightPos, lightNormal, rng);
@@ -524,6 +526,11 @@ TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCur
     sr.light = c.prim;
     c.slot++;
     return true;
+}
+
+TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCursor& c, Rng& rng, ShadowRay& sr)
+{
+    return nee_generate(sc, sf, time, c, rng, sr, sc.numPrims);
 }
 
 // Consumes the traced shadow ray of the slot generated last; accumulates into the cursor in the

@@ -19,6 +19,11 @@
 //   B  shadow result: connect the NEE sample; next NEE sample -> T, or BSDF sample, throughput
 //      update and next extension ray -> T, or termination -> R
 //
+// The lane-owned layout (wf2_lq, below) has no stage B: its stage A shades the whole bounce in place, in
+// k_mega's order -- every NEE sample is generated, traced and connected right there, then the BSDF sample
+// -> T, or termination -> R.  That saves the claim, push and slot-state round trip a shadow ray took through
+// stage T (the claims halve), though on cornell the fused stage A costs nearly all of it back (DESIGN §5.1).
+//
 // The queues are lock-free rings in shared memory: producers reserve cells with one warp-
 // aggregated atomicAdd on `tail` (ballot + prefix sum) and store lap-tagged slot ids, so a chunk
 // is always full while the queue holds >= 32 entries (compaction is implicit in the queue).
@@ -67,7 +72,16 @@ enum { WF2_PH_EXT = 0, WF2_PH_NEE = 1 };
 //   5: sky pdf, NEE sum.xyz                     6: NEE radiance accumulator.xyz
 // TB_WF2_COLD_SMEM: the same records in SHARED memory instead (stride 7 chunks), for builds with few enough
 // slots per CTA: the cold half then costs 7 128-bit accesses per stage instead of 27 32-bit ones.
-#ifdef TB_WF2_COLD_SMEM
+// TB_WF2_LANEQ: no shadow ray ever waits in a slot (stage A traces them in place), so only chunks 0-3 exist
+// and chunk 3 holds the RNG alone.
+#if defined(TB_WF2_LANEQ)
+#ifndef TB_WF2_COLD_SMEM
+#error "the lane-owned layout keeps the cold state in shared memory"
+#endif
+enum { CC_T = 0, CC_L = 1, CC_A = 2, CC_RNG = 3, CC_CHUNKS = 4 };
+TB_DEV float4 cold_ld(const float4* rec, int c) { return rec[c]; }
+TB_DEV void cold_st(float4* rec, int c, float x, float y, float z, float w) { rec[c] = make_float4(x, y, z, w); }
+#elif defined(TB_WF2_COLD_SMEM)
 enum { CC_T = 0, CC_L = 1, CC_A = 2, CC_RNG = 3, CC_SH = 4, CC_SUM = 5, CC_LA = 6, CC_CHUNKS = 7 };
 TB_DEV float4 cold_ld(const float4* rec, int c) { return rec[c]; }
 TB_DEV void cold_st(float4* rec, int c, float x, float y, float z, float w) { rec[c] = make_float4(x, y, z, w); }
@@ -92,16 +106,21 @@ struct Wf2Shared {
     // extension-ray hit
     float ht[TB_WF2_PATHS], hnx[TB_WF2_PATHS], hny[TB_WF2_PATHS], hnz[TB_WF2_PATHS];
     int hprim[TB_WF2_PATHS];
+#ifndef TB_WF2_LANEQ
     // pending shadow ray (origin is recomputed from the surface point) and its result
     float sdx[TB_WF2_PATHS], sdy[TB_WF2_PATHS], sdz[TB_WF2_PATHS];
     float st[TB_WF2_PATHS];
     int sprim[TB_WF2_PATHS];
+#endif
 #ifdef TB_WF2_COLD_SMEM
-    float4 cold[TB_WF2_PATHS * 7];
+    float4 cold[TB_WF2_PATHS * CC_CHUNKS];
 #endif
 #ifdef TB_WF2_LANEQ
     // stage queues as bit sets (lane-owned slots, see wf2_push below): one word per queue and lane
-    unsigned int lq[4][32];
+    unsigned int lq[3][32];
+    // every primitive with lightSamples > 0 lies in [lightBegin, lightEnd): stage A's NEE scan starts and stops
+    // there instead of loading every primitive's lightSamples in turn (a dependent chain on every hit)
+    int lightBegin, lightEnd;
 #else
     // stage queues: rings of lap-tagged slot ids
     uint16_t ring[7][TB_WF2_PATHS];
@@ -140,7 +159,11 @@ struct Wf2Shared {
 // TM (free-running mode, scenes with DScene::splitValid): rays that enter the big mesh's box; same
 // stage code as T, but a chunk taken from TM walks the mesh with all of its lanes and a chunk taken
 // from T with none.
+#ifdef TB_WF2_LANEQ
+enum { WF2_Q_T = 0, WF2_Q_A = 1, WF2_Q_R = 2, WF2_NUM_Q = 3 };   // no B, no hard phases, no split trace queue
+#else
 enum { WF2_Q_T = 0, WF2_Q_A = 1, WF2_Q_B = 2, WF2_Q_R = 3, WF2_Q_F0 = 4, WF2_Q_F1 = 5, WF2_Q_TM = 6 };
+#endif
 #define WF2_MASK (TB_WF2_PATHS - 1)
 #define WF2_LOG2_PATHS (TB_WF2_PATHS == 2048 ? 11 : TB_WF2_PATHS == 1024 ? 10 : TB_WF2_PATHS == 512 ? 9 : TB_WF2_PATHS == 256 ? 8 : 7)
 #define WF2_SLOT_BITS 11                      // queue cells: slot id in the low 11 bits, lap tag (1..31) above
@@ -166,6 +189,9 @@ TB_DEV uint16_t wf2_cell(unsigned int index, int slot)
 // their traversal coherence: those keep the ring queues.
 // The caller has fenced its slot-state writes (__threadfence_block).
 static_assert(TB_WF2_PATHS == 1024, "one word per lane and queue");
+#ifndef WF2_R_MIN_LANES
+#define WF2_R_MIN_LANES 24   // stage R waits for that many lanes with a finished slot while T or A has work
+#endif
 #ifndef WF2_STICK_LANES
 #define WF2_STICK_LANES 16     // a warp stays with the preferred stage while that many lanes have a slot waiting there
 #endif
@@ -197,6 +223,9 @@ TB_DEV void wf2_push(Wf2Shared& S, int q, bool flag, int slot)
 // is a scheduling heuristic, so the unoffset hit point is good enough as the shadow-ray origin.
 TB_DEV void wf2_push_trace(Wf2Shared& S, const DScene& sc, bool split, int q, bool flag, int s)
 {
+#ifdef TB_WF2_LANEQ
+    wf2_push(S, q, flag, s);   // no split trace queue in this layout
+#else
     if (!split) {
         wf2_push(S, q, flag, s);
         return;
@@ -218,11 +247,12 @@ TB_DEV void wf2_push_trace(Wf2Shared& S, const DScene& sc, bool split, int q, bo
     }
     wf2_push(S, q, flag && !big, s);
     wf2_push(S, WF2_Q_TM, flag && big, s);
+#endif
 }
 
 #ifdef TB_WF2_LANEQ
-// Claim one waiting slot per lane.  All four queues (T, A, B, R) are looked at in one go -- four independent
-// loads of the lane's own words and four ballots -- and the warp takes the CTA's preferred stage while at least
+// Claim one waiting slot per lane.  All three queues (T, A, R) are looked at in one go -- three independent
+// loads of the lane's own words and three ballots -- and the warp takes the CTA's preferred stage while at least
 // `stick` lanes have something there, else the stage with the most lanes ready (which becomes the preference:
 // the warps of a CTA herd through the stages, and share the instruction cache -- a per-warp preference instead
 // of the CTA-wide one is much slower).  Every lane then picks a set bit of its word -- starting at a position that
@@ -234,28 +264,30 @@ TB_DEV unsigned wf2_claim_fullest(Wf2Shared& S, int stick, int& slot, int& stage
     const int lane = threadIdx.x & 31;
     const int rot = (int)(threadIdx.x >> 5) * 2 + 1;
     for (;;) {
-        // the preference and the four queue words load side by side (no load depends on another)
+        // the preference and the three queue words load side by side (no load depends on another)
         int pref = *(volatile int*)&S.pref;   // every lane loads (a broadcast, no branch); lane 0's copy is the one used
         const unsigned m0 = *(volatile unsigned int*)&S.lq[0][lane], m1 = *(volatile unsigned int*)&S.lq[1][lane];
-        const unsigned m2 = *(volatile unsigned int*)&S.lq[2][lane], m3 = *(volatile unsigned int*)&S.lq[3][lane];
+        const unsigned m2 = *(volatile unsigned int*)&S.lq[2][lane];
         pref = __shfl_sync(0xffffffffu, pref, 0);
         // lanes ready per queue, one byte each (selections by shifts, not branches)
-        const unsigned cc = (unsigned)__popc(__ballot_sync(0xffffffffu, m0 != 0u)) | ((unsigned)__popc(__ballot_sync(0xffffffffu, m1 != 0u)) << 8) |
-                            ((unsigned)__popc(__ballot_sync(0xffffffffu, m2 != 0u)) << 16) | ((unsigned)__popc(__ballot_sync(0xffffffffu, m3 != 0u)) << 24);
+        unsigned cc = (unsigned)__popc(__ballot_sync(0xffffffffu, m0 != 0u)) | ((unsigned)__popc(__ballot_sync(0xffffffffu, m1 != 0u)) << 8) |
+                      ((unsigned)__popc(__ballot_sync(0xffffffffu, m2 != 0u)) << 16);
+        // R's work is per lane (the splat's atomics, a new camera ray), so a thin R chunk costs nearly what a full
+        // one does: R only counts as ready with WF2_R_MIN_LANES lanes, or when nothing else is (cornell: about +1.5 %)
+        if (((cc >> (8 * WF2_Q_R)) & 0xffu) < WF2_R_MIN_LANES && (cc & ~(0xffu << (8 * WF2_Q_R))) != 0u) cc &= ~(0xffu << (8 * WF2_Q_R));
         int q = pref;
         unsigned bc = (cc >> (8 * pref)) & 0xffu;
         if (bc < (unsigned)stick) {
 #pragma unroll
-            for (int k = 1; k < 4; ++k) {
-                const int qq = (pref + k) & 3;
+            for (int k = 1; k < WF2_NUM_Q; ++k) {
+                const int qq = pref + k < WF2_NUM_Q ? pref + k : pref + k - WF2_NUM_Q;
                 const unsigned cq = (cc >> (8 * qq)) & 0xffu;
                 q = cq > bc ? qq : q;
                 bc = cq > bc ? cq : bc;
             }
         }
         if (bc == 0u) return 0u;
-        const unsigned lo = (q & 1) ? m1 : m0, hi = (q & 1) ? m3 : m2;
-        const unsigned mine = (q & 2) ? hi : lo;
+        const unsigned mine = q == 0 ? m0 : q == 1 ? m1 : m2;
         bool got = false;
         if (mine != 0u) {
             const int k = (__ffs(__funnelshift_r(mine, mine, rot)) - 1 + rot) & 31;
@@ -388,6 +420,7 @@ static __device__ __noinline__ void wf2_band_pad(unsigned int* bandCount, volati
     }
 }
 
+#ifndef TB_WF2_LANEQ
 // the pending shadow ray and the NEE bookkeeping that waits for its result
 TB_DEV void wf2_store_shadow(Wf2Shared& S, float4* rec, int s, const ShadowRay& sr, const NeeCursor& c, Rng rng)
 {
@@ -398,6 +431,7 @@ TB_DEV void wf2_store_shadow(Wf2Shared& S, float4* rec, int s, const ShadowRay& 
     cold_st(rec, CC_SUM, sr.skyPdf, c.sum.x, c.sum.y, c.sum.z);
     cold_st(rec, CC_LA, c.Lacc.x, c.Lacc.y, c.Lacc.z, 0.0f);
 }
+#endif
 
 // finish the shading of a surface hit once all NEE samples are folded: BSDF sample, next ray
 // (path_scatter) or termination.  Returns true when the slot continues with a new extension ray.
@@ -469,6 +503,7 @@ TB_DEV int wf2_claim_answers(Wf2Shared& S, const WalkParams& W, int kind, int mi
     return n;
 }
 
+#ifndef TB_WF2_LANEQ
 // Fold a walker's answer into the partial hit stage T left in the slot (offload mode).  Afterwards
 // the slot holds exactly what trace_closest() would have produced for the pending ray.
 TB_DEV void wf2_merge_answer(Wf2Shared& S, const DScene& sc, int s, bool isExt, uint4 c0, uint4 c1, uint4 c2)
@@ -520,6 +555,7 @@ TB_DEV void wf2_merge_answer(Wf2Shared& S, const DScene& sc, int s, bool isExt, 
         S.sprim[s] = primM;
     }
 }
+#endif
 
 // THREADS: 512 (16 warps, up to 128 registers) for scenes held in shared memory, where more warps
 // only add instruction-cache pressure; 768 (24 warps, 80 registers) for scenes with deep mesh BVHs,
@@ -533,6 +569,60 @@ TB_DEV void wf2_merge_answer(Wf2Shared& S, const DScene& sc, int s, bool isExt, 
 //   WF2_MODE_SPLIT    free-running with the split trace queue TM (scenes with a big mesh)
 //   WF2_MODE_OFFLOAD  free-running shader CTAs + walker CTAs that do the big meshes' BVH walks (wavefront_walk.cuh)
 enum { WF2_MODE_GENERIC = 0, WF2_MODE_HARD = 1, WF2_MODE_SPLIT = 2, WF2_MODE_OFFLOAD = 3 };
+
+#if defined(TB_WF2_STAGE_CLOCKS) && defined(TB_WF2_LANEQ)
+// Per-stage cycle accounting of the lane-owned layout (development builds with -DTB_WF2_STAGE_CLOCKS, read by
+// tb200_stage_clocks, see tools/stage_clocks.py).  Every warp sums clock64() deltas in registers and adds its
+// totals here when it exits.  Stage kinds k: 0 R, 1 T, 2 A, 3 B (no B in this layout: its counters stay 0).
+//   [0] claims that got slots   [1] idle: empty claims and the back-off   [2 + k] cycles in stage k
+//   [6 + k] chunks of stage k   [10 + k] lanes active in those chunks      [14] warps
+enum { WF2_CLK_CLAIM = 0, WF2_CLK_IDLE = 1, WF2_CLK_CYCLES = 2, WF2_CLK_CHUNKS = 6, WF2_CLK_LANES = 10, WF2_CLK_WARPS = 14, WF2_CLK_N = 15 };
+static_assert(WF2_CLK_N == TB_WF2_STAGE_CLOCK_WORDS, "tb_kernels.cuh states the counter count");
+__device__ unsigned long long g_wf2StageClocks[WF2_CLK_N];
+
+// A warp's sums are 32 bits wide (fewer registers, so the accounting itself spills less): a warp lives for one
+// launch, and the tool's launches last far fewer than 2^32 cycles.
+struct Wf2Clocks {
+    static constexpr int kinds = 3;   // R, T, A: this layout has no stage B
+    unsigned int claim = 0, idle = 0, cyc[kinds] = {}, chunks[kinds] = {}, lanes[kinds] = {};
+
+    // the stage kind as a constant index, so the arrays stay in registers
+    TB_DEV void add(int stage, unsigned int dt, unsigned act)
+    {
+#pragma unroll
+        for (int k = 0; k < kinds; ++k) {
+            const int q = k == 0 ? (int)WF2_Q_R : k == 1 ? (int)WF2_Q_T : (int)WF2_Q_A;
+            if (stage == q) {
+                cyc[k] += dt;
+                chunks[k] += 1u;
+                lanes[k] += (unsigned)__popc(act);
+            }
+        }
+    }
+    TB_DEV void flush() const
+    {
+        if ((threadIdx.x & 31) != 0) return;
+        atomicAdd(&g_wf2StageClocks[WF2_CLK_CLAIM], (unsigned long long)claim);
+        atomicAdd(&g_wf2StageClocks[WF2_CLK_IDLE], (unsigned long long)idle);
+#pragma unroll
+        for (int k = 0; k < kinds; ++k) {
+            atomicAdd(&g_wf2StageClocks[WF2_CLK_CYCLES + k], (unsigned long long)cyc[k]);
+            atomicAdd(&g_wf2StageClocks[WF2_CLK_CHUNKS + k], (unsigned long long)chunks[k]);
+            atomicAdd(&g_wf2StageClocks[WF2_CLK_LANES + k], (unsigned long long)lanes[k]);
+        }
+        atomicAdd(&g_wf2StageClocks[WF2_CLK_WARPS], 1ull);
+    }
+};
+
+void wf2_stage_clocks(unsigned long long* out, bool reset)
+{
+    cudaMemcpyFromSymbol(out, g_wf2StageClocks, sizeof(g_wf2StageClocks));
+    if (reset) {
+        static const unsigned long long zero[WF2_CLK_N] = {};
+        cudaMemcpyToSymbol(g_wf2StageClocks, zero, sizeof(zero));
+    }
+}
+#endif
 
 template <int THREADS, int MODE>
 __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(const __grid_constant__ LaunchParams P, unsigned long long total)
@@ -604,13 +694,23 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
             d.treeletPairs = 0;
         }
         S.scene = d;
+#ifdef TB_WF2_LANEQ
+        int lb = 0, le = 0;
+        for (int i = P.scene.numPrims - 1; i >= 0; --i)
+            if (P.scene.prims[i].lightSamples > 0) {
+                if (le == 0) le = i + 1;
+                lb = i;
+            }
+        S.lightBegin = lb;
+        S.lightEnd = le;
+#endif
     }
     const DScene& sc = S.scene;
     // every slot starts in the R queue "finished with nothing to splat": stage R fills it with a
     // camera sample
 #ifdef TB_WF2_LANEQ
     for (int s = tid; s < TB_WF2_PATHS; s += THREADS) S.flags[s] = WF2_FLAG_EMPTY;
-    if (tid < 4 * 32) S.lq[tid >> 5][tid & 31] = (tid >> 5) == WF2_Q_R ? 0xffffffffu : 0u;
+    if (tid < WF2_NUM_Q * 32) S.lq[tid >> 5][tid & 31] = (tid >> 5) == WF2_Q_R ? 0xffffffffu : 0u;
     if (tid == 0) {
 #else
     for (int s = tid; s < TB_WF2_PATHS; s += THREADS) {
@@ -676,19 +776,29 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
     //    cost varies wildly (deep mesh BVHs) and the hot loop is small enough to stay cached.
 #ifdef TB_WF2_LANEQ
     static_assert(MODE == WF2_MODE_GENERIC, "the lane-owned layout serves the free-running scheduler only");
-    constexpr bool hard = false, split = false;
-    const int cycle = 0;
+    constexpr bool split = false;
+#ifdef TB_WF2_STAGE_CLOCKS
+    Wf2Clocks clk;
+#endif
     for (;;) {
         int s = 0, stage = -1;
-        const bool fromAnswer = false;
-        const uint4 ans0 = make_uint4(0u, 0u, 0u, 0u), ans1 = ans0, ans2 = ans0;
+#ifdef TB_WF2_STAGE_CLOCKS
+        const unsigned int t0 = (unsigned int)clock64();
+#endif
         const unsigned act = wf2_claim_fullest(S, WF2_STICK_LANES, s, stage);
         if (act == 0u) {
             if (*(volatile int*)&S.live <= 0) break;
             __nanosleep(200);
+#ifdef TB_WF2_STAGE_CLOCKS
+            clk.idle += (unsigned int)clock64() - t0;
+#endif
             continue;
         }
         const bool active = ((act >> lane) & 1u) != 0u;
+#ifdef TB_WF2_STAGE_CLOCKS
+        const unsigned int t1 = (unsigned int)clock64();
+        clk.claim += t1 - t0;
+#endif
 #else
     const bool hard = MODE == WF2_MODE_HARD ? true : (MODE == WF2_MODE_SPLIT || offload) ? false : (P.hardPhases != 0);
     constexpr bool split = MODE == WF2_MODE_SPLIT;
@@ -882,10 +992,30 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                 }
             }
             __threadfence_block();
+#ifdef TB_WF2_LANEQ
+            wf2_push(S, WF2_Q_T, fresh, s);
+#else
             wf2_push_trace(S, sc, split, hard ? WF2_Q_F0 + (cycle & 1) : WF2_Q_T, fresh, s);
+#endif
             // slots that could not be refilled die: the CTA exits when none is left
             const unsigned dead = __ballot_sync(0xffffffffu, active && !fresh);
             if (dead && lane == 0) atomicSub(&S.live, __popc(dead));
+#ifdef TB_WF2_LANEQ
+        } else if (stage == WF2_Q_T) {
+            // ===================== T: trace the extension ray (the only kind this layout queues) ==
+            if (active) {
+                if (maxDepth > 0) {
+                    const Hit h = trace_closest(sc, v3(S.ox[s], S.oy[s], S.oz[s]), v3(S.dx[s], S.dy[s], S.dz[s]), S.time[s], true);
+                    S.ht[s] = h.t;
+                    S.hnx[s] = h.n.x; S.hny[s] = h.n.y; S.hnz[s] = h.n.z;
+                    S.hprim[s] = h.prim;
+                } else {
+                    S.hprim[s] = -2;   // maxDepth == 0: no trace at all, radiance stays 0
+                }
+            }
+            __threadfence_block();
+            wf2_push(S, WF2_Q_A, active, s);
+#else
         } else if (stage == WF2_Q_T || stage >= WF2_Q_F0) {
             // ===================== T: trace the pending ray =======================================
             bool isExt = false, isNee = false;
@@ -942,10 +1072,13 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
             }
             wf2_push(S, WF2_Q_A, isExt, s);
             wf2_push(S, WF2_Q_B, isNee, s);
+#endif
         } else if (stage == WF2_Q_A) {
             // ===================== A: extension-ray results =======================================
             bool cont = false, fin = false;
+#ifndef TB_WF2_LANEQ
             if (offload && fromAnswer && active) wf2_merge_answer(S, sc, s, true, ans0, ans1, ans2);
+#endif
             if (active) {
                 float4* rec = coldBase + (size_t)s * CC_CHUNKS;
                 const float4 ct = cold_ld(rec, CC_T), cl = cold_ld(rec, CC_L);
@@ -986,8 +1119,35 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                     Surface sf;
                     path_hit(sc, ps, h, bounce, sf);
                     NeeCursor c;
-                    nee_begin(c);
                     ShadowRay sr;
+#ifdef TB_WF2_LANEQ
+                    nee_begin(c, S.lightBegin);
+                    const int lightEnd = S.lightEnd;
+                    // The whole bounce in place, in k_mega's order: every NEE sample traced and connected, then
+                    // the BSDF sample.  What the traces do not need stays in the slot and is read back after
+                    // them instead of being held in registers across them: the throughput and radiance path_hit
+                    // left, and the surface (wf2_surface rebuilds it bit for bit, as stage B of the other layouts
+                    // does).  s2 is s behind an empty asm, so the compiler cannot forward the stores to the reads.
+                    // (Measured on cornell: keeping it all in registers spills, 160 bytes.)
+                    cold_st(rec, CC_T, ps.T.x, ps.T.y, ps.T.z, ct.w);
+                    cold_st(rec, CC_L, ps.L.x, ps.L.y, ps.L.z, cl.w);
+                    const float time = ps.time;
+                    Rng rng = ps.rng;
+                    int s2 = s;
+                    while (nee_generate(sc, sf, time, c, rng, sr, lightEnd)) {
+                        const Hit sh = trace_closest(sc, sr.o, sr.d, time, false);
+                        asm volatile("" : "+r"(s2) : "f"(sh.t));
+                        sf = wf2_surface(S, sc, s2, ct.w);
+                        nee_connect(sc, sf, sr, sh, c);
+                    }
+                    asm volatile("" : "+r"(s2));
+                    const float4* rec2 = coldBase + (size_t)s2 * CC_CHUNKS;
+                    const float4 t2 = cold_ld(rec2, CC_T), l2 = cold_ld(rec2, CC_L), a2 = cold_ld(rec2, CC_A);
+                    cont = wf2_scatter(S, rec, sc, s, sf, v3(t2.x, t2.y, t2.z), v3(l2.x, l2.y, l2.z), rng, time, c.sum, (int)(S.flags[s] >> 8), maxDepth,
+                                       v3(a2.x, a2.y, a2.z), l2.w, f2u(a2.w));
+                    fin = !cont;
+#else
+                    nee_begin(c);
                     if (nee_generate(sc, sf, ps.time, c, ps.rng, sr)) {
                         cold_st(rec, CC_T, ps.T.x, ps.T.y, ps.T.z, ct.w);
                         cold_st(rec, CC_L, ps.L.x, ps.L.y, ps.L.z, cl.w);
@@ -999,12 +1159,15 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                         cont = wf2_scatter(S, rec, sc, s, sf, ps.T, ps.L, ps.rng, ps.time, c.sum, bounce, maxDepth, ps.absorb, ps.bsdfPdf, f2u(ca.w));
                         fin = !cont;
                     }
+#endif
                 }
             }
             __threadfence_block();
             wf2_push_trace(S, sc, split, WF2_Q_T, cont, s);
             wf2_push(S, WF2_Q_R, fin, s);
-        } else {
+        }
+#ifndef TB_WF2_LANEQ
+        else {
             // ===================== B: shadow-ray results ==========================================
             bool cont = false, fin = false;
             if (offload && fromAnswer && active) wf2_merge_answer(S, sc, s, false, ans0, ans1, ans2);
@@ -1052,7 +1215,14 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
             wf2_push_trace(S, sc, split, WF2_Q_T, cont, s);
             wf2_push(S, WF2_Q_R, fin, s);
         }
+#endif
+#if defined(TB_WF2_STAGE_CLOCKS) && defined(TB_WF2_LANEQ)
+        clk.add(stage, (unsigned int)clock64() - t1, act);
+#endif
     }
+#if defined(TB_WF2_STAGE_CLOCKS) && defined(TB_WF2_LANEQ)
+    clk.flush();
+#endif
     if (offload) {
         // this CTA posts no more requests: tell the walkers (once)
         if (lane == 0 && atomicExch(&S.exitSignaled, 1) == 0) {

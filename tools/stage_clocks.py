@@ -1,0 +1,94 @@
+#!/usr/bin/env python
+"""Where the cycles of the lane-owned wavefront kernel (wf2_lq::k_wavefront2<512, generic>) go, per stage.
+
+Builds the development variant with the kernel's own clock64() accounting (-DTB_WF2_STAGE_CLOCKS, off in the
+product build) as tinsel_b200/libtinsel_b200_clocks.so, renders cornell in the benchmark's shape with it
+(1024x1024, 32 spp per render_device call, TINSEL_B200_LIB pointing at the variant) and prints per stage:
+SM cycles per camera sample, visits (warp chunks) per sample and the mean number of lanes active per chunk.
+
+    python tools/stage_clocks.py [--steps N] [--lib PATH | --no-build]
+
+"SM cycles per sample" is warp cycles / warps per CTA / samples: the share of an SM's time a stage takes,
+per sample, so that the rows add up to the kernel's SM cycles per sample (one CTA per SM).  claim counts the
+claims that got slots, idle the empty claims and their back-off.  The clock reads themselves cost a little:
+compare two builds with this tool, and absolute speed with bench.py."""
+import argparse
+import ctypes as C
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+VARIANT = "libtinsel_b200_clocks.so"
+WORDS = 15                     # tb_kernels.cuh: TB_WF2_STAGE_CLOCK_WORDS
+WARPS_PER_CTA = 512 // 32
+STAGES = ["R", "T", "A", "B"]  # counter order (wavefront2.cuh: Wf2Clocks)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=8)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--spp", type=int, default=32)
+    ap.add_argument("--size", type=int, default=1024)
+    ap.add_argument("--lib", help="an already built clock variant (default: build tinsel_b200/%s)" % VARIANT)
+    ap.add_argument("--no-build", action="store_true", help="use tinsel_b200/%s as it is" % VARIANT)
+    args = ap.parse_args()
+
+    lib = args.lib or os.path.join(ROOT, "tinsel_b200", VARIANT)
+    if not args.lib and not args.no_build:
+        subprocess.check_call([sys.executable, "-m", "tinsel_b200.build", "--out", VARIANT, "-DTB_WF2_STAGE_CLOCKS"], cwd=ROOT)
+    os.environ["TINSEL_B200_LIB"] = os.path.abspath(lib)
+    os.environ.pop("TINSEL_B200_PIPELINE", None)
+    sys.path.insert(0, ROOT)
+    import tinsel_b200 as tb
+
+    native = tb.load_library()
+    if not hasattr(native, "tb200_stage_clocks"):
+        raise SystemExit("%s was not built with -DTB_WF2_STAGE_CLOCKS" % lib)
+    native.tb200_stage_clocks.restype = C.c_int
+    native.tb200_stage_clocks.argtypes = [C.POINTER(C.c_ulonglong), C.c_int, C.c_int]
+    counters = (C.c_ulonglong * WORDS)()
+
+    def read(reset):
+        if native.tb200_stage_clocks(counters, WORDS, 1 if reset else 0) != WORDS:
+            raise SystemExit("tb200_stage_clocks failed")
+        return list(counters)
+
+    w = h = args.size
+    snap = tb.Snapshot(tb.scene_path("cornell"))
+    cam, opt = snap.camera, snap.options
+    opt.width, opt.height = w, h
+    r = tb.Renderer(snap.scene)
+    r.Init(w, h)
+    for _ in range(args.warmup):
+        r.render_device(cam, opt, args.spp)
+    read(True)
+    gpu_ms = 0.0
+    for _ in range(args.steps):
+        r.render_device(cam, opt, args.spp)
+        gpu_ms += r.stats().gpuMs
+    c = read(True)
+    r.close()
+    snap.close()
+
+    samples = w * h * args.spp * args.steps
+    per = float(WARPS_PER_CTA) * samples
+    claim, idle = c[0], c[1]
+    cyc, chunks, lanes = c[2:6], c[6:10], c[10:14]
+    total = claim + idle + sum(cyc)
+    print("cornell %dx%d, %d spp x %d steps: %.1f Msamples/s with the clock reads, %d warps" % (
+        w, h, args.spp, args.steps, samples / gpu_ms / 1e3, c[14]))
+    print("%-10s %14s %8s %16s %12s" % ("stage", "SM cyc/sample", "share", "visits/sample", "mean lanes"))
+    print("%-10s %14.1f %7.1f%%" % ("claim", claim / per, 100.0 * claim / total))
+    print("%-10s %14.1f %7.1f%%" % ("idle", idle / per, 100.0 * idle / total))
+    for k, name in enumerate(STAGES):
+        if chunks[k] == 0:
+            continue
+        print("%-10s %14.1f %7.1f%% %16.3f %12.2f" % (name, cyc[k] / per, 100.0 * cyc[k] / total, lanes[k] / samples,
+                                                     lanes[k] / chunks[k]))
+    print("%-10s %14.1f" % ("total", total / per))
+
+
+if __name__ == "__main__":
+    main()
