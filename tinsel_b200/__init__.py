@@ -84,6 +84,8 @@ def load_library():
     lib.tb200_set_frame.argtypes = [C.c_void_p, C.c_int]
     lib.tb200_get_stats.restype = None
     lib.tb200_get_stats.argtypes = [C.c_void_p, C.POINTER(Stats)]
+    lib.tb200_last_kernel.restype = C.c_char_p
+    lib.tb200_last_kernel.argtypes = [C.c_void_p]
     lib.tb200_get_member_stats.restype = C.c_int
     lib.tb200_get_member_stats.argtypes = [C.c_void_p, C.c_int, C.POINTER(Stats), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.tb200_destroy.restype = None
@@ -293,6 +295,10 @@ class Renderer:
         s = Stats()
         self.lib.tb200_get_stats(self.h, C.byref(s))
         return s
+
+    def last_kernel(self):
+        """Name of the kernel the last launch ran (tb200_last_kernel)."""
+        return self.lib.tb200_last_kernel(self.h).decode()
 
     def close(self):
         if self.h:

@@ -181,6 +181,7 @@ EXPORTS = [
     "tb200_trace_frame",
     "tb200_set_frame",
     "tb200_get_stats",
+    "tb200_last_kernel",
     "tb200_destroy",
     "tb200_last_error",
     "tb200_sample_seed",

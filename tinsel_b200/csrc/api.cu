@@ -353,6 +353,9 @@ struct tb200_renderer {
     int hardPhases = 1;           // wavefront scheduling mode (see wavefront2.cuh)
     int wideCta = 0;              // 768-thread CTAs for deep mesh BVHs (see wavefront2.cuh)
     int laneQueues = 0;           // lane-owned slots + bit-set queues (see wavefront2.cuh)
+    uint32_t features = TB_FEAT_ALL;   // the scene's TB_FEAT_* features (scene_features)
+    int specialize = 1;           // scenes without any feature run the specialised lane-owned kernel (TINSEL_B200_SPECIALIZE=0: never)
+    const char* lastKernel = "";  // the kernel the last path-tracing launch ran (tb200_last_kernel)
     // Split trace queue on/off is decided by measurement (every variant produces the same bits): the
     // second and third sizeable launches after tb200_create time one setting each, the faster stays.
     int tunePhase = 3;            // 0 warm-up (split), 1 measuring split, 2 measuring no split, 3 decided
@@ -633,6 +636,22 @@ bool check_offload(tb200_renderer* r)
                                 : "mesh-walk offload: a walker CTA waited for requests without progress (watchdog); the frame is incomplete");
 }
 
+// The scene's features (tb_scene.cuh: TB_FEAT_*).  A scene without any of them runs the lane-owned kernel compiled
+// without them (wavefront2.cuh: wf2_lq::launch_layout); a NaN parameter counts as present.
+uint32_t scene_features(const SceneImage& img)
+{
+    uint32_t f = img.probeValid ? TB_FEAT_PROBE : TB_FEAT_NONE;
+    for (const DPrim& p : img.prims) {
+        const DMaterial& m = p.mat;
+        if (!p.isStatic) f |= TB_FEAT_MOTION;
+        if (m.transmission != 0.0f) f |= TB_FEAT_TRANSMISSION;
+        if (m.subsurface != 0.0f) f |= TB_FEAT_SUBSURFACE;
+        if (m.clearcoat != 0.0f) f |= TB_FEAT_CLEARCOAT;
+        if (m.absorption.x != 0.0f || m.absorption.y != 0.0f || m.absorption.z != 0.0f) f |= TB_FEAT_ABSORPTION;
+    }
+    return f;
+}
+
 // device upload of a scene image + the per-scene scheduling decisions (which read the environment)
 bool upload_image(tb200_renderer* r, const SceneImage& img)
 {
@@ -693,6 +712,10 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
         const char* queues = getenv("TINSEL_B200_QUEUES");
         if (queues && strcmp(queues, "ring") == 0) r->laneQueues = 0;
         if (queues && strcmp(queues, "lanes") == 0) r->laneQueues = 2;
+        // TINSEL_B200_SPECIALIZE=0 runs the generic lane-owned kernel on scenes without features too (A/B runs, tests)
+        r->features = scene_features(img);
+        const char* spec = getenv("TINSEL_B200_SPECIALIZE");
+        r->specialize = (spec && atoi(spec) == 0) ? 0 : 1;
     }
     // one element of padding each: the kernels' bulk copies round their length up to 16 bytes
     if (!upload(img.prims, &r->dPrims, h2d, 1)) return false;
@@ -943,6 +966,7 @@ bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_opti
     P->hardPhases = r->hardPhases;
     P->wideCta = r->wideCta;
     P->laneQueues = r->laneQueues;
+    P->specialized = (r->specialize && r->features == TB_FEAT_NONE) ? 1 : 0;
     P->firstRow = 0;
     P->numRows = o->height;
     P->film.rowLo = 0;
@@ -978,10 +1002,8 @@ bool launch_frames(tb200_renderer* r, LaunchParams& P, bool recordStart = true)
         for (int f = 0; f < frames; f += framesPerLaunch) {
             P.frame0 = frame0 + f;
             P.numFrames = std::min(framesPerLaunch, frames - f);
-            if (r->pipeline == 0)
-                launch_mega(P, r->stream, &launches);
-            else
-                launch_wavefront2(P, r->numSMs, r->stream, &launches);
+            const char* name = r->pipeline == 0 ? launch_mega(P, r->stream, &launches) : launch_wavefront2(P, r->numSMs, r->stream, &launches);
+            if (name) r->lastKernel = name;
         }
         P.frame0 = frame0;
         P.numFrames = frames;
@@ -2022,6 +2044,11 @@ void tb200_get_stats(tb200_renderer* r, tb200_stats* out)
         out->h2dBytes += p->stats.h2dBytes;
         out->gpuMs = std::max(out->gpuMs, p->stats.gpuMs);
     }
+}
+
+const char* tb200_last_kernel(tb200_renderer* r)
+{
+    return r ? r->lastKernel : "";
 }
 
 int tb200_get_member_stats(tb200_renderer* r, int member, tb200_stats* out, int* firstRow, int* numRows)

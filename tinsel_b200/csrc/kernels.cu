@@ -108,14 +108,15 @@ __global__ void __launch_bounds__(128) k_mega(const __grid_constant__ LaunchPara
     sample_end(P, px, py, rasterX, rasterY, ps.L);
 }
 
-void launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned long long* launchCount)
+const char* launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned long long* launchCount)
 {
     const unsigned long long total = p.samplesPerFrame * (unsigned long long)p.numFrames;
-    if (total == 0ull) return;
+    if (total == 0ull) return nullptr;
     const int block = 128;
     const unsigned long long grid = (total + block - 1) / block;
     k_mega<<<(unsigned)grid, block, 0, stream>>>(p);
     if (launchCount) ++*launchCount;
+    return "k_mega";
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -342,7 +343,7 @@ namespace wf2_lq {
 void read_stage_clocks(unsigned long long* out, bool reset) { wf2_lq::wf2_stage_clocks(out, reset); }
 #endif
 
-void launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
+const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
     // The lane-owned layout wins in the steady state (cornell 32 spp on an H100: 1131 vs 893 Msamples/s) and loses
     // while the slots fill and drain (1-spp frames, slabs of a multi-GPU render; measured in round 2): launches of
@@ -350,9 +351,8 @@ void launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, u
     const unsigned long long total = p.samplesPerFrame * (unsigned long long)p.numFrames;
     const bool small = total < 6ull * (unsigned long long)(numSMs > 0 ? numSMs : 132) * 1024ull;
     if (p.wideCta || wavefront2_wants_offload(p))
-        wf2_l2::launch_layout(p, numSMs, stream, launchCount);
-    else if (!p.hardPhases && !p.scene.splitValid && (p.laneQueues == 2 || (p.laneQueues == 1 && !small)))
-        wf2_lq::launch_layout(p, numSMs, stream, launchCount);
-    else
-        wf2_smem::launch_layout(p, numSMs, stream, launchCount);
+        return wf2_l2::launch_layout(p, numSMs, stream, launchCount);
+    if (!p.hardPhases && !p.scene.splitValid && (p.laneQueues == 2 || (p.laneQueues == 1 && !small)))
+        return wf2_lq::launch_layout(p, numSMs, stream, launchCount);
+    return wf2_smem::launch_layout(p, numSMs, stream, launchCount);
 }

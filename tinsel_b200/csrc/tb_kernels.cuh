@@ -56,6 +56,7 @@ struct LaunchParams {
     // cold half of the wavefront's slot state: 8 x float4 per slot, TB_WF2_PATHS slots per CTA of the launch
     float4* cold;
     int treeletBytes;     // shared memory behind the slot arrays that the prologue fills with the top of DScene::treeletMesh's BVH
+    int specialized;      // the scene has none of the TB_FEAT_* features: the lane-owned layout runs its instantiation without them
 };
 
 #define TB_MAX_BANDS 64
@@ -63,10 +64,11 @@ struct LaunchParams {
 // fills tilesX / tileRows / samplesPerFrame from the row range and shard
 void finalize_params(LaunchParams* p);
 
+// The launches below return the name of the kernel they ran (nullptr when there was no work), for tb200_last_kernel.
 // one thread per (pixel, frame): the whole path in registers.  Validation / fallback pipeline.
-void launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned long long* launchCount);
+const char* launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned long long* launchCount);
 // persistent CTA-resident wavefront pipeline with a dedicated traversal stage (the product path)
-void launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
+const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds: the per-stage cycle counters of the lane-owned wavefront layout (wavefront2.cuh), summed
 // over every launch since the last reset

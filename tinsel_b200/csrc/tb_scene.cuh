@@ -154,9 +154,26 @@ struct Hit {
     int prim;    // -1: miss
 };
 
+// Scene features that the trace and shading code tests for at run time (the host computes a scene's set in
+// api.cu: scene_features).  The device functions that test them take the set as a template parameter FEAT and
+// guard each such branch with a constant test of their bit: with a bit clear, the branches only that feature
+// can take -- and the code and registers behind them -- drop out of the instantiation.  Every test is still
+// made at run time in the default instantiation (TB_FEAT_ALL), which serves every scene.
+enum : uint32_t {
+    TB_FEAT_NONE = 0u,
+    TB_FEAT_PROBE = 1u << 0,          // the sky has an environment probe
+    TB_FEAT_MOTION = 1u << 1,         // a primitive moves (start != end transform)
+    TB_FEAT_TRANSMISSION = 1u << 2,   // a material has transmission != 0
+    TB_FEAT_SUBSURFACE = 1u << 3,     // a material has subsurface != 0
+    TB_FEAT_CLEARCOAT = 1u << 4,      // a material has clearcoat != 0
+    TB_FEAT_ABSORPTION = 1u << 5,     // a material has a non-zero absorption component
+    TB_FEAT_ALL = (1u << 6) - 1u,
+};
+
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV Xf prim_transform(const DPrim& p, float time)
 {
-    if (p.isStatic) return p.fixed;
+    if (!(FEAT & TB_FEAT_MOTION) || p.isStatic) return p.fixed;
     return interpolate_transform(p.start, p.end, time);
 }
 
@@ -387,6 +404,7 @@ struct PrimHit {
     V3 gn;     // MeshQuery::closestNormal (n*sign, unnormalised)
 };
 
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV bool prim_test(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, PrimHit& ph)
 {
     if (p.type == TB200_PLANE) {
@@ -397,7 +415,7 @@ TB_DEV bool prim_test(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, 
         ph.t = t;
         return t > 0.0f;
     }
-    const Xf xf = prim_transform(p, time);
+    const Xf xf = prim_transform<FEAT>(p, time);
     if (p.type == TB200_SPHERE) {
         // SolveQuadratic with a == 1 + IntersectRaySphere, intersection.h:30-83
         const V3 q = o - xf.p;
@@ -431,10 +449,11 @@ TB_DEV bool prim_test(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, 
     return true;
 }
 
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV V3 prim_normal(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, const PrimHit& ph)
 {
     if (p.type == TB200_PLANE) return v3(p.plane[0], p.plane[1], p.plane[2]);
-    const Xf xf = prim_transform(p, time);
+    const Xf xf = prim_transform<FEAT>(p, time);
     if (p.type == TB200_SPHERE) return normalize((o + d * ph.t) - xf.p);   // intersection.h:76-79
     const DMesh& m = sc.meshes[p.mesh];
     const float4 q0 = __ldg(&m.triNormals[ph.tri * 3 + 0]);
@@ -449,6 +468,7 @@ TB_DEV V3 prim_normal(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, 
 // Trace + QueryBVH, render.cpp:17-62 + intersection.h:751-799: near-first DFS over the scene
 // BVH with NO closest-t culling; the callback keeps `t < minT && t > 0` (first found wins ties).
 // This is the reference's visit order, bit for bit.
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_ORDERED_ATTR Hit trace_ordered(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
 {
     V3 rcp;
@@ -470,7 +490,7 @@ TB_ORDERED_ATTR Hit trace_ordered(const DScene& sc, V3 o, V3 d, float time, bool
         if (ref & TB_LEAF) {
             const int index = (int)(ref & ~TB_LEAF);
             PrimHit ph;
-            if (prim_test(sc, sc.prims[index], o, d, time, ph)) {
+            if (prim_test<FEAT>(sc, sc.prims[index], o, d, time, ph)) {
                 if (ph.t < minT && ph.t > 0.0f) {
                     minT = ph.t;
                     closest = index;
@@ -497,7 +517,7 @@ TB_ORDERED_ATTR Hit trace_ordered(const DScene& sc, V3 o, V3 d, float time, bool
     h.t = minT;
     h.prim = closest;
     V3 n = v3s(0.0f);
-    if (wantNormal && closest >= 0) n = prim_normal(sc, sc.prims[closest], o, d, time, best);
+    if (wantNormal && closest >= 0) n = prim_normal<FEAT>(sc, sc.prims[closest], o, d, time, best);
     h.n = face_forward(n, -d);
     return h;
 }
@@ -526,12 +546,13 @@ struct __align__(16) ProgOp {
     int bits;        // guard bit (TB_BIT_ALWAYS: unconditional) | own bit << 8 (BOX only)
 };
 
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
 {
     const int n = sc.numFlat;
     const bool guard = (fabsf(o.x) < 1.0e7f) & (fabsf(o.y) < 1.0e7f) & (fabsf(o.z) < 1.0e7f) & (d.x == d.x) & (d.y == d.y) &
                        (d.z == d.z);
-    if (n == 0 || !guard) return trace_ordered(sc, o, d, time, wantNormal);
+    if (n == 0 || !guard) return trace_ordered<FEAT>(sc, o, d, time, wantNormal);
 
     V3 rcp;
     rcp.x = 1.0f / d.x;
@@ -573,7 +594,7 @@ TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNorm
                 }
             }
             PrimHit* ph = &rec[ri ^ 1];
-            if (!prim_test(sc, sc.prims[kindPrim >> 8], o, d, time, *ph)) continue;
+            if (!prim_test<FEAT>(sc, sc.prims[kindPrim >> 8], o, d, time, *ph)) continue;
             t = ph->t;
             if (t > 0.0f && t < minT) ri ^= 1;   // the record just written becomes the best one
         }
@@ -586,14 +607,14 @@ TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNorm
             }
         }
     }
-    if (tie) return trace_ordered(sc, o, d, time, wantNormal);
+    if (tie) return trace_ordered<FEAT>(sc, o, d, time, wantNormal);
     Hit h;
     h.t = minT;
     h.prim = closest;
     V3 nrm = v3s(0.0f);
     if (wantNormal && closest >= 0) {
         rec[ri].t = minT;
-        nrm = prim_normal(sc, sc.prims[closest], o, d, time, rec[ri]);
+        nrm = prim_normal<FEAT>(sc, sc.prims[closest], o, d, time, rec[ri]);
     }
     h.n = face_forward(nrm, -d);
     return h;

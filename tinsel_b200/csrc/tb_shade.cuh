@@ -70,6 +70,7 @@ TB_DEV bool refract_dir(V3 wi, V3 n, float eta, V3& wt)
 }
 
 // BSDFPdf, disney.h:125-166
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV float bsdf_pdf(const DMaterial& mat, float etaI, float etaO, V3 n, V3 V, V3 L)
 {
     if (dot(L, n) <= 0.0f) {
@@ -88,7 +89,7 @@ TB_DEV float bsdf_pdf(const DMaterial& mat, float etaI, float etaO, V3 n, V3 V, 
     // Lerp(brdfPdf, pdfSpec*F, transmission): with transmission == 0 and a front-facing view the
     // Fresnel term is finite (both denominators of Fr are positive), so the lerp adds
     // (finite)*0 = +-0 and returns brdfPdf unchanged; Fr is skipped then.
-    if (mat.transmission == 0.0f && NV > 0.0f) return brdfPdf;
+    if ((!(FEAT & TB_FEAT_TRANSMISSION) || mat.transmission == 0.0f) && NV > 0.0f) return brdfPdf;
     const float F = fresnel_dielectric(NV, etaI, etaO);
     const float bsdfPdf = pdfSpec * F;
     return tb_lerp(brdfPdf, bsdfPdf, mat.transmission);
@@ -96,6 +97,7 @@ TB_DEV float bsdf_pdf(const DMaterial& mat, float etaI, float etaO, V3 n, V3 V, 
 
 // BSDFEval, disney.h:296-405 (Cdlum/Ctint/Cspec0 and the clearcoat alpha are per-material
 // constants computed on the host with the reference's double intermediates, api.cu)
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV V3 bsdf_eval(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3 L)
 {
     const float NDotL = dot(N, L);
@@ -107,7 +109,7 @@ TB_DEV V3 bsdf_eval(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3
     V3 bsdf = v3s(0.0f);
     V3 brdf = v3s(0.0f);
 
-    if (mat.transmission > 0.0f) {
+    if ((FEAT & TB_FEAT_TRANSMISSION) && mat.transmission > 0.0f) {
         if (NDotL <= 0) {
             const float F = fresnel_dielectric(NDotV, etaI, etaO);
             bsdf = v3s(mat.transmission * (1.0f - F) / tb_abs(NDotL) * (1.0f - mat.metallic));
@@ -121,9 +123,9 @@ TB_DEV V3 bsdf_eval(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3
         }
     }
 
-    if (mat.transmission < 1.0f) {
+    if (!(FEAT & TB_FEAT_TRANSMISSION) || mat.transmission < 1.0f) {
         if (NDotL <= 0) {
-            if (mat.subsurface > 0.0f) {
+            if ((FEAT & TB_FEAT_SUBSURFACE) && mat.subsurface > 0.0f) {
                 const float FL = schlick_fresnel(tb_abs(NDotL)), FV = schlick_fresnel(NDotV);
                 const float Fd = (1.0f - 0.5f * FL) * (1.0f - 0.5f * FV);
                 brdf = TB_INV_PI * mat.sqrtColor * mat.subsurface * Fd * (1.0f - mat.metallic);
@@ -144,7 +146,7 @@ TB_DEV V3 bsdf_eval(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3
             // clearcoat lobe: `+ mat.clearcoat*Gr*Fc*Dr`.  With clearcoat == 0 the term is 0*finite = +-0
             // (Gr, Fc, Dr are finite here: NDotL > 0, alpha in [.001,.1]) and adding it changes at most
             // the sign of a zero, which no branch or sum downstream can observe; skip the lobe then.
-            if (mat.clearcoat != 0.0f) {
+            if ((FEAT & TB_FEAT_CLEARCOAT) && mat.clearcoat != 0.0f) {
                 const float Dr = gtr1_clearcoat(mat, NDotH);
                 const float Fc = tb_lerp(.04f, 1.0f, FH);
                 const float Gr = smith_ggx(NDotL, .25f) * smith_ggx(NDotV, .25f);
@@ -161,11 +163,12 @@ struct BsdfValue {
     float pdf;   // BSDFPdf
 };
 
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_NOINLINE BsdfValue bsdf_eval_pdf(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3 L)
 {
     BsdfValue r;
-    r.pdf = bsdf_pdf(mat, etaI, etaO, N, V, L);
-    r.f = bsdf_eval(mat, etaI, etaO, N, V, L);
+    r.pdf = bsdf_pdf<FEAT>(mat, etaI, etaO, N, V, L);
+    r.f = bsdf_eval<FEAT>(mat, etaI, etaO, N, V, L);
     return r;
 }
 
@@ -188,13 +191,16 @@ TB_DEV V3 sample_ggx_reflection(const DMaterial& mat, float r2, float sinPhiHalf
 // lanes of the warp instead of three divergent ones (same values: the product is commutative).
 // Returns true when the pdf is BSDFPdf(light) (the caller evaluates it together with BSDFEval);
 // false when `pdf` is already final (specular refraction, or 0 for total internal reflection).
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV bool bsdf_sample_dir(const DMaterial& mat, float etaI, float etaO, V3 U, V3 Vt, V3 N, V3 view, V3& light, float& pdf,
                             int& type, Rng& rng)
 {
     enum { LOBE_GGX, LOBE_COSINE, LOBE_UNIFORM };
     int lobe;
     float angleArg, r1 = 0.0f, r2 = 0.0f, uz = 0.0f;
-    if (rng_float(rng) < mat.transmission) {
+    // the draws are made whatever FEAT says; only the comparisons with a constant 0 fold (x < 0 is false for x >= 0)
+    const float rt = rng_float(rng);
+    if ((FEAT & TB_FEAT_TRANSMISSION) && rt < mat.transmission) {
         const float F = fresnel_dielectric(dot(N, view), etaI, etaO);
         if (rng_float(rng) < F) {
             r1 = rng_float(rng);
@@ -216,7 +222,8 @@ TB_DEV bool bsdf_sample_dir(const DMaterial& mat, float etaI, float etaO, V3 U, 
         r1 = rng_float(rng);
         r2 = rng_float(rng);
         if (rng_float(rng) < 0.5f) {
-            if (rng_float(rng) < mat.subsurface) {
+            const float rs = rng_float(rng);
+            if ((FEAT & TB_FEAT_SUBSURFACE) && rs < mat.subsurface) {
                 // UniformSampleHemisphere(Random&), maths.h:1291-1302: z, then phi = k2Pi*Randf
                 uz = rng_float(rng);
                 angleArg = rng_float(rng);
@@ -323,18 +330,20 @@ TB_DEV void probe_sample(const DProbe& pr, V3& dir, V3& color, float& pdf, Rng& 
 }
 
 // Sky::Eval, scene.h:168-178, given uv = ProbeDirToUV(dir) when the sky has a probe
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV V3 sky_eval(const DScene& sc, V3 dir, float u, float v)
 {
-    if (sc.probe.valid) return probe_eval(sc.probe, u, v);
+    if ((FEAT & TB_FEAT_PROBE) && sc.probe.valid) return probe_eval(sc.probe, u, v);
     return tb_lerp(sc.horizon, sc.zenith, sqrtf(tb_abs(dir.y)));
 }
 
 // ---- light sampling (intersection.h:855-904) --------------------------------------------------
 
 // PrimitiveSample
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV void prim_sample(const DScene& sc, const DPrim& p, float time, V3& pos, V3& normal, Rng& rng)
 {
-    const Xf xf = prim_transform(p, time);
+    const Xf xf = prim_transform<FEAT>(p, time);
     if (p.type == TB200_SPHERE) {
         const float u1 = rng_float(rng);
         const float u2 = rng_float(rng);
@@ -409,25 +418,27 @@ TB_DEV void path_init(PathState& ps, V3 origin, V3 dir, float time, Rng rng)
 }
 
 // Miss branch, render.cpp:365-384.  Always terminates the path.
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV void path_miss(const DScene& sc, PathState& ps, int bounce)
 {
     float weight = 1.0f;
     float u = 0.0f, v = 0.0f;
-    if (sc.probe.valid) {
+    if ((FEAT & TB_FEAT_PROBE) && sc.probe.valid) {
         // shared by ProbePdf and Sky::Eval (both call ProbeDirToUV(rayDir))
         const float2 uv = probe_dir_to_uv(ps.d);
         u = uv.x;
         v = uv.y;
     }
-    if (sc.probe.valid && bounce > 0 && ps.rayType != TB_SPECULAR) {
+    if ((FEAT & TB_FEAT_PROBE) && sc.probe.valid && bounce > 0 && ps.rayType != TB_SPECULAR) {
         const float skyPdf = probe_pdf(sc.probe, u, v);
         const float cbsdf = 0.5f, csky = 0.5f;   // kBsdfSamples/N, kProbeSamples/N with N = 2
         weight = cbsdf * ps.bsdfPdf / (cbsdf * ps.bsdfPdf + csky * skyPdf);
     }
-    ps.L = ps.L + weight * sky_eval(sc, ps.d, u, v) * ps.T;
+    ps.L = ps.L + weight * sky_eval<FEAT>(sc, ps.d, u, v) * ps.T;
 }
 
 // Hit prologue, render.cpp:255-310: medium bookkeeping, Beer-Lambert, emission with MIS.
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV void path_hit(const DScene& sc, PathState& ps, const Hit& h, int bounce, Surface& sf)
 {
     const DPrim& prim = sc.prims[h.prim];
@@ -440,7 +451,8 @@ TB_DEV void path_hit(const DScene& sc, PathState& ps, const Hit& h, int bounce, 
     }
     // pathThroughput *= Exp(-rayAbsorption*t), render.cpp:272.  With zero absorption the argument is
     // -0*t = -0 and expf(-0) = 1 exactly, so the multiply is the identity and is skipped.
-    if (!(ps.absorb.x == 0.0f && ps.absorb.y == 0.0f && ps.absorb.z == 0.0f)) {
+    // Without FEAT_ABSORPTION every material's absorption is 0, so ps.absorb only ever holds +-0.
+    if ((FEAT & TB_FEAT_ABSORPTION) && !(ps.absorb.x == 0.0f && ps.absorb.y == 0.0f && ps.absorb.z == 0.0f)) {
         const V3 e = -ps.absorb * h.t;
         ps.T = ps.T * v3(tb_expf(e.x), tb_expf(e.y), tb_expf(e.z));
     }
@@ -491,9 +503,10 @@ TB_DEV void nee_begin(NeeCursor& c, int firstLight = 0)
 // Generates the next shadow ray (drawing the RNG exactly as the reference does).  Returns
 // false when all slots are exhausted.  lightEnd: no primitive from there on has lightSamples > 0
 // (sc.numPrims when not known); the scan for the next light stops there.
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCursor& c, Rng& rng, ShadowRay& sr, int lightEnd)
 {
-    if (c.slot == 0 && sc.probe.valid) {
+    if ((FEAT & TB_FEAT_PROBE) && c.slot == 0 && sc.probe.valid) {
         V3 wi, color;
         float pdf;
         probe_sample(sc.probe, wi, color, pdf, rng);
@@ -514,7 +527,7 @@ TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCur
     if (c.prim >= lightEnd) return false;
     const DPrim& light = sc.prims[c.prim];
     V3 lightPos, lightNormal;
-    prim_sample(sc, light, time, lightPos, lightNormal, rng);
+    prim_sample<FEAT>(sc, light, time, lightPos, lightNormal, rng);
     V3 wi = lightPos - sf.p;
     const float dSq = length_sq(wi);
     wi = wi / sqrtf(dSq);
@@ -530,15 +543,16 @@ TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCur
 
 TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCursor& c, Rng& rng, ShadowRay& sr)
 {
-    return nee_generate(sc, sf, time, c, rng, sr, sc.numPrims);
+    return nee_generate<>(sc, sf, time, c, rng, sr, sc.numPrims);
 }
 
 // Consumes the traced shadow ray of the slot generated last; accumulates into the cursor in the
 // reference's order (render.cpp:122-143 for the probe, :176-224 for area lights).
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr, const Hit& sh, NeeCursor& c)
 {
     const DMaterial& mat = sc.prims[sf.prim].mat;
-    const bool isProbe = sr.light < 0;
+    const bool isProbe = (FEAT & TB_FEAT_PROBE) && sr.light < 0;   // only the probe sample has no light
     // decide first whether BSDFPdf/BSDFEval are needed at all (both are pure), then evaluate them
     // once for whichever kind of sample this is
     float nl = 0.0f;
@@ -555,7 +569,7 @@ TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr
     V3 f = v3s(0.0f);
     float bsdfPdf = 0.0f;
     if (need) {
-        const BsdfValue b = bsdf_eval_pdf(mat, sf.etaI, sf.etaO, sf.n, sf.wo, sr.d);
+        const BsdfValue b = bsdf_eval_pdf<FEAT>(mat, sf.etaI, sf.etaO, sf.n, sf.wo, sr.d);
         f = b.f;
         bsdfPdf = b.pdf;
     }
@@ -590,6 +604,7 @@ TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr
 
 // After NEE: light-hit termination, BSDF sampling, throughput and medium update, next ray
 // (render.cpp:314-363).  Returns false when the path ends here.
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV bool path_scatter(const DScene& sc, PathState& ps, const Surface& sf, V3 neeSum)
 {
     ps.L = ps.L + ps.T * neeSum;
@@ -602,11 +617,11 @@ TB_DEV bool path_scatter(const DScene& sc, PathState& ps, const Surface& sf, V3 
     V3 bsdfDir = v3s(0.0f);
     int bsdfType = TB_REFLECTED;
     float pdf = 0.0f;
-    const bool pdfFromBsdf = bsdf_sample_dir(prim.mat, sf.etaI, sf.etaO, u, v, sf.n, sf.wo, bsdfDir, pdf, bsdfType, ps.rng);
+    const bool pdfFromBsdf = bsdf_sample_dir<FEAT>(prim.mat, sf.etaI, sf.etaO, u, v, sf.n, sf.wo, bsdfDir, pdf, bsdfType, ps.rng);
     V3 f = v3s(0.0f);
     if (pdfFromBsdf || pdf > 0.0f) {
         // pdf = BSDFPdf(dir) (disney.h:291) and f = BSDFEval(dir) (render.cpp:341) share one call
-        const BsdfValue b = bsdf_eval_pdf(prim.mat, sf.etaI, sf.etaO, sf.n, sf.wo, bsdfDir);
+        const BsdfValue b = bsdf_eval_pdf<FEAT>(prim.mat, sf.etaI, sf.etaO, sf.n, sf.wo, bsdfDir);
         f = b.f;
         if (pdfFromBsdf) pdf = b.pdf;
     }

@@ -435,6 +435,7 @@ TB_DEV void wf2_store_shadow(Wf2Shared& S, float4* rec, int s, const ShadowRay& 
 
 // finish the shading of a surface hit once all NEE samples are folded: BSDF sample, next ray
 // (path_scatter) or termination.  Returns true when the slot continues with a new extension ray.
+template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV bool wf2_scatter(Wf2Shared& S, float4* rec, const DScene& sc, int s, const Surface& sf, V3 T, V3 L, Rng rng, float time, V3 neeSum,
                         int bounce, int maxDepth, V3 absorb, float bsdfPdf, uint32_t sample)
 {
@@ -455,7 +456,7 @@ TB_DEV bool wf2_scatter(Wf2Shared& S, float4* rec, const DScene& sc, int s, cons
         ps.L = ps.L + ps.T * neeSum;
         go = false;
     } else {
-        go = path_scatter(sc, ps, sf, neeSum);
+        go = path_scatter<FEAT>(sc, ps, sf, neeSum);
     }
     cold_st(rec, CC_L, ps.L.x, ps.L.y, ps.L.z, ps.bsdfPdf);
     if (!go) return false;
@@ -624,7 +625,9 @@ void wf2_stage_clocks(unsigned long long* out, bool reset)
 }
 #endif
 
-template <int THREADS, int MODE>
+// FEAT: the scene features (TB_FEAT_*) compiled in.  The lane-owned layout has a second instantiation without any
+// of them, for scenes that have none (wf2_lq::launch_layout); every other instantiation has them all.
+template <int THREADS, int MODE, uint32_t FEAT = TB_FEAT_ALL>
 __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(const __grid_constant__ LaunchParams P, unsigned long long total)
 {
     extern __shared__ __align__(16) unsigned char wf_smem_raw[];
@@ -776,6 +779,10 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
     //    cost varies wildly (deep mesh BVHs) and the hot loop is small enough to stay cached.
 #ifdef TB_WF2_LANEQ
     static_assert(MODE == WF2_MODE_GENERIC, "the lane-owned layout serves the free-running scheduler only");
+#else
+    static_assert(FEAT == TB_FEAT_ALL, "only the lane-owned layout has a specialised instantiation");
+#endif
+#ifdef TB_WF2_LANEQ
     constexpr bool split = false;
 #ifdef TB_WF2_STAGE_CLOCKS
     Wf2Clocks clk;
@@ -1005,7 +1012,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
             // ===================== T: trace the extension ray (the only kind this layout queues) ==
             if (active) {
                 if (maxDepth > 0) {
-                    const Hit h = trace_closest(sc, v3(S.ox[s], S.oy[s], S.oz[s]), v3(S.dx[s], S.dy[s], S.dz[s]), S.time[s], true);
+                    const Hit h = trace_closest<FEAT>(sc, v3(S.ox[s], S.oy[s], S.oz[s]), v3(S.dx[s], S.dy[s], S.dz[s]), S.time[s], true);
                     S.ht[s] = h.t;
                     S.hnx[s] = h.n.x; S.hny[s] = h.n.y; S.hnz[s] = h.n.z;
                     S.hprim[s] = h.prim;
@@ -1093,7 +1100,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                         ps.L = v3(cl.x, cl.y, cl.z);
                         ps.rayType = (int)((fl >> 1) & 3u);
                         ps.bsdfPdf = cl.w;
-                        path_miss(sc, ps, bounce);
+                        path_miss<FEAT>(sc, ps, bounce);
                         cold_st(rec, CC_L, ps.L.x, ps.L.y, ps.L.z, cl.w);
                     }
                     fin = true;
@@ -1117,7 +1124,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                     h.n = v3(S.hnx[s], S.hny[s], S.hnz[s]);
                     h.prim = hprim;
                     Surface sf;
-                    path_hit(sc, ps, h, bounce, sf);
+                    path_hit<FEAT>(sc, ps, h, bounce, sf);
                     NeeCursor c;
                     ShadowRay sr;
 #ifdef TB_WF2_LANEQ
@@ -1134,16 +1141,16 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                     const float time = ps.time;
                     Rng rng = ps.rng;
                     int s2 = s;
-                    while (nee_generate(sc, sf, time, c, rng, sr, lightEnd)) {
-                        const Hit sh = trace_closest(sc, sr.o, sr.d, time, false);
+                    while (nee_generate<FEAT>(sc, sf, time, c, rng, sr, lightEnd)) {
+                        const Hit sh = trace_closest<FEAT>(sc, sr.o, sr.d, time, false);
                         asm volatile("" : "+r"(s2) : "f"(sh.t));
                         sf = wf2_surface(S, sc, s2, ct.w);
-                        nee_connect(sc, sf, sr, sh, c);
+                        nee_connect<FEAT>(sc, sf, sr, sh, c);
                     }
                     asm volatile("" : "+r"(s2));
                     const float4* rec2 = coldBase + (size_t)s2 * CC_CHUNKS;
                     const float4 t2 = cold_ld(rec2, CC_T), l2 = cold_ld(rec2, CC_L), a2 = cold_ld(rec2, CC_A);
-                    cont = wf2_scatter(S, rec, sc, s, sf, v3(t2.x, t2.y, t2.z), v3(l2.x, l2.y, l2.z), rng, time, c.sum, (int)(S.flags[s] >> 8), maxDepth,
+                    cont = wf2_scatter<FEAT>(S, rec, sc, s, sf, v3(t2.x, t2.y, t2.z), v3(l2.x, l2.y, l2.z), rng, time, c.sum, (int)(S.flags[s] >> 8), maxDepth,
                                        v3(a2.x, a2.y, a2.z), l2.w, f2u(a2.w));
                     fin = !cont;
 #else
@@ -1236,7 +1243,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
 // attribute applies to the current device only), so they are kept per device ordinal and set up once
 // per device under a lock: a host may own renderers on several GPUs, driven from several threads.
 #define TB_WF2_MAX_DEVICES 64
-template <int THREADS, int MODE>
+template <int THREADS, int MODE, uint32_t FEAT>
 static int wavefront2_ctas_per_sm()
 {
     static std::mutex lock;
@@ -1246,9 +1253,9 @@ static int wavefront2_ctas_per_sm()
     std::lock_guard<std::mutex> guard(lock);
     if (ctasPerSM[dev] == 0) {
         int n = 0;
-        cudaFuncSetAttribute(k_wavefront2<THREADS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        cudaFuncSetAttribute(k_wavefront2<THREADS, MODE, FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)std::max(wavefront2_smem_limit(), (size_t)TB_WF2_SMEM_BYTES));
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_wavefront2<THREADS, MODE>, THREADS, TB_WF2_SMEM_BYTES) != cudaSuccess || n < 1)
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_wavefront2<THREADS, MODE, FEAT>, THREADS, TB_WF2_SMEM_BYTES) != cudaSuccess || n < 1)
             n = 1;
         if (n > TB_WF2_MAX_CTAS_PER_SM) n = TB_WF2_MAX_CTAS_PER_SM;
         ctasPerSM[dev] = n;
@@ -1256,10 +1263,10 @@ static int wavefront2_ctas_per_sm()
     return ctasPerSM[dev];
 }
 
-template <int THREADS, int MODE>
+template <int THREADS, int MODE, uint32_t FEAT = TB_FEAT_ALL>
 static void launch_wavefront2_t(const LaunchParams& p0, int numSMs, cudaStream_t stream, unsigned long long total)
 {
-    const int ctasPerSM = wavefront2_ctas_per_sm<THREADS, MODE>();
+    const int ctasPerSM = wavefront2_ctas_per_sm<THREADS, MODE, FEAT>();
     // shared memory beyond the slot arrays holds the treelet (the shader role; walker CTAs lay out their own)
     LaunchParams p = p0;
     const size_t slotBytes = (TB_WF2_SMEM_BYTES + 127) & ~size_t(127);
@@ -1285,24 +1292,35 @@ static void launch_wavefront2_t(const LaunchParams& p0, int numSMs, cudaStream_t
     }
     if (want < (unsigned long long)grid) grid = (int)want;
     if (grid < 1) grid = 1;
-    k_wavefront2<THREADS, MODE><<<grid, THREADS, smemBytes, stream>>>(p, total);
+    k_wavefront2<THREADS, MODE, FEAT><<<grid, THREADS, smemBytes, stream>>>(p, total);
 }
 
-// the launches of this layout (see the top of the file for which scheduler variants each layout serves)
-void launch_layout(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
+// the launches of this layout (see the top of the file for which scheduler variants each layout serves); returns
+// the name of the kernel launched (nullptr: nothing to do)
+const char* launch_layout(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
     const unsigned long long total = p.samplesPerFrame * (unsigned long long)p.numFrames;
-    if (total == 0ull) return;
+    if (total == 0ull) return nullptr;
     cudaMemsetAsync(p.sampleCounter, 0, sizeof(unsigned long long), stream);
 #if !defined(TB_WF2_LANEQ)
     const bool split = !p.hardPhases && p.scene.splitValid;
 #endif
+    const char* name;
 #if defined(TB_WF2_LANEQ)
-    launch_wavefront2_t<TB_WF2_THREADS, WF2_MODE_GENERIC>(p, numSMs, stream, total);
+    // scenes with none of the TB_FEAT_* features run the instantiation without them (LaunchParams::specialized).
+    // Also 512 threads: at 640 (20 warps, 96 registers) it spills 128 bytes and measured no faster on cornell.
+    if (p.specialized) {
+        launch_wavefront2_t<TB_WF2_THREADS, WF2_MODE_GENERIC, TB_FEAT_NONE>(p, numSMs, stream, total);
+        name = "wf2_lq.specialized";
+    } else {
+        launch_wavefront2_t<TB_WF2_THREADS, WF2_MODE_GENERIC>(p, numSMs, stream, total);
+        name = "wf2_lq.generic";
+    }
 #elif defined(TB_WF2_COLD_SMEM)
     if (p.hardPhases) launch_wavefront2_t<TB_WF2_THREADS, WF2_MODE_HARD>(p, numSMs, stream, total);
     else if (split) launch_wavefront2_t<TB_WF2_THREADS, WF2_MODE_SPLIT>(p, numSMs, stream, total);
     else launch_wavefront2_t<TB_WF2_THREADS, WF2_MODE_GENERIC>(p, numSMs, stream, total);
+    name = "wf2_smem";
 #else
     if (wavefront2_wants_offload(p)) {
         if (p.wideCta) launch_wavefront2_t<TB_WF2_THREADS_WIDE, WF2_MODE_OFFLOAD>(p, numSMs, stream, total);
@@ -1312,6 +1330,8 @@ void launch_layout(const LaunchParams& p, int numSMs, cudaStream_t stream, unsig
     } else {
         launch_wavefront2_t<TB_WF2_THREADS_WIDE, WF2_MODE_GENERIC>(p, numSMs, stream, total);   // hard phases too (run-time flag)
     }
+    name = "wf2_l2";
 #endif
     if (launchCount) ++*launchCount;
+    return name;
 }

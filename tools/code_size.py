@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Static code size of one kernel instantiation by source function (SASS instructions, 16 B each):
 where the bytes are that compete for the 32 KB L1.5 instruction cache.
-    python tools/code_size.py [mangled-substring, default k_wavefront2ILi512ELi0E]
+    python tools/code_size.py [mangled-substring, default _ZN6wf2_lq12k_wavefront2ILi512ELi0ELj0E, the lane-owned kernel cornell runs]
 
 With --local: the local-memory instructions (LDL / STL) of one kernel instantiation, out-of-line callees
 included, by source function and line.  Needs no GPU.
-    python tools/code_size.py --local [mangled-substring, default _ZN6wf2_lq12k_wavefront2ILi512ELi0E]"""
+    python tools/code_size.py --local [mangled-substring, default _ZN6wf2_lq12k_wavefront2ILi512ELi0ELj0E]"""
 import re
 import sys
 from collections import Counter
@@ -66,6 +66,6 @@ if __name__ == "__main__":
     args = sys.argv[1:]
     if "--local" in args:
         args.remove("--local")
-        local_accesses(args[0] if args else "_ZN6wf2_lq12k_wavefront2ILi512ELi0E")
+        local_accesses(args[0] if args else "_ZN6wf2_lq12k_wavefront2ILi512ELi0ELj0E")
     else:
-        code_size(args[0] if args else "k_wavefront2ILi512ELi0E")
+        code_size(args[0] if args else "_ZN6wf2_lq12k_wavefront2ILi512ELi0ELj0E")

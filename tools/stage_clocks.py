@@ -1,5 +1,7 @@
 #!/usr/bin/env python
-"""Where the cycles of the lane-owned wavefront kernel (wf2_lq::k_wavefront2<512, generic>) go, per stage.
+"""Where the cycles of the lane-owned wavefront kernel go, per stage.  Cornell runs its instantiation without the
+scene features (wf2_lq::k_wavefront2<512, generic, TB_FEAT_NONE>; TINSEL_B200_SPECIALIZE=0: the generic one), and
+the clock accounting is compiled into both; the table's first line names the kernel that ran.
 
 Builds the development variant with the kernel's own clock64() accounting (-DTB_WF2_STAGE_CLOCKS, off in the
 product build) as tinsel_b200/libtinsel_b200_clocks.so, renders cornell in the benchmark's shape with it
@@ -69,6 +71,7 @@ def main():
         r.render_device(cam, opt, args.spp)
         gpu_ms += r.stats().gpuMs
     c = read(True)
+    kernel = r.last_kernel()
     r.close()
     snap.close()
 
@@ -77,8 +80,8 @@ def main():
     claim, idle = c[0], c[1]
     cyc, chunks, lanes = c[2:6], c[6:10], c[10:14]
     total = claim + idle + sum(cyc)
-    print("cornell %dx%d, %d spp x %d steps: %.1f Msamples/s with the clock reads, %d warps" % (
-        w, h, args.spp, args.steps, samples / gpu_ms / 1e3, c[14]))
+    print("cornell %dx%d, %d spp x %d steps, %s: %.1f Msamples/s with the clock reads, %d warps" % (
+        w, h, args.spp, args.steps, kernel, samples / gpu_ms / 1e3, c[14]))
     print("%-10s %14s %8s %16s %12s" % ("stage", "SM cyc/sample", "share", "visits/sample", "mean lanes"))
     print("%-10s %14.1f %7.1f%%" % ("claim", claim / per, 100.0 * claim / total))
     print("%-10s %14.1f %7.1f%%" % ("idle", idle / per, 100.0 * idle / total))
