@@ -284,6 +284,24 @@ int tb200_nlm(tb200_renderer* r, float falloff, int radius, float* out);
 int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options,
                       int frame, float* radiance, float* raster);
 
+/* ---- batched closest-hit ray query ---------------------------------------------------------
+ * Per ray i, exactly Trace(scene, Ray(origin, dir, time)) of src/render.cpp:17-62, bit for bit:
+ *   prims[i]       index of the closest primitive with t > 0, or -1 on a miss
+ *   hits[i].t      its distance in units of |dir| (dir is used as given, never normalised)
+ *   hits[i].normal the shading normal after FaceForward(n, -dir)
+ * A miss leaves t = FLT_MAX and the face-forwarded zero normal.  `time` drives the motion-blur
+ * interpolation of primitive transforms; `pad` is ignored.
+ * `rays`, `hits` and `prims` are DEVICE memory of the renderer's device (a multi-device renderer: its
+ * head, devices[0]); `rays` and `hits` 16-byte aligned.  Host or foreign-device pointers, null pointers,
+ * numRays < 0 and spans past the end of their allocation are refused before anything is launched.
+ * The work runs on the renderer's stream (tb200_set_stream) and the call returns when the results are
+ * in place.  Needs no tb200_init; leaves the accumulator, the frame counter, stats.frames,
+ * stats.samples and tb200_last_kernel as they are; adds 1 to stats.kernelLaunches and sets stats.gpuMs
+ * to the query kernel's time.  numRays == 0 launches nothing.  Returns 0 on success. */
+typedef struct tb200_ray { float origin[3]; float time; float dir[3]; float pad; } tb200_ray;   /* 32 B */
+typedef struct tb200_hit { float t; float normal[3]; } tb200_hit;                               /* 16 B */
+int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, int64_t numRays);
+
 /* Sets the frame counter (frame k seeds sample k of every pixel). */
 void tb200_set_frame(tb200_renderer* r, int frame);
 

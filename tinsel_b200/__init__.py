@@ -80,6 +80,8 @@ def load_library():
     lib.tb200_nlm.argtypes = [C.c_void_p, C.c_float, C.c_int, f32p]
     lib.tb200_trace_frame.restype = C.c_int
     lib.tb200_trace_frame.argtypes = [C.c_void_p, C.POINTER(Camera), C.POINTER(Options), C.c_int, f32p, f32p]
+    lib.tb200_trace_rays.restype = C.c_int
+    lib.tb200_trace_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_set_frame.restype = None
     lib.tb200_set_frame.argtypes = [C.c_void_p, C.c_int]
     lib.tb200_get_stats.restype = None
@@ -192,8 +194,10 @@ class Renderer:
             self.h = self.lib.tb200_create(scene, device)
         if not self.h:
             raise TinselB200Error("tb200_create failed: " + last_error())
+        self.device = devices[0] if devices is not None and cache is None else device   # the head: trace_rays runs there
         self.width = self.height = 0
         self._pinned = None
+        self._external_stream = False
 
     def _check(self, rc, what):
         if rc != 0:
@@ -222,6 +226,7 @@ class Renderer:
             self._check(self.lib.tb200_set_stream(self.h, None, 0), "tb200_set_stream")
         else:
             self._check(self.lib.tb200_set_stream(self.h, C.c_void_p(cuda_stream_handle), 1), "tb200_set_stream")
+        self._external_stream = cuda_stream_handle is not None
 
     def set_slab(self, first_row, num_rows):
         self._check(self.lib.tb200_set_slab(self.h, first_row, num_rows), "tb200_set_slab")
@@ -287,6 +292,44 @@ class Renderer:
         self._check(self.lib.tb200_trace_frame(self.h, C.byref(camera), C.byref(options), frame, _fp(rad), _fp(ras)),
                     "tb200_trace_frame")
         return rad, ras
+
+    def trace_rays(self, rays, hits=None, prims=None):
+        """Closest hit of every ray (tb200_trace_rays): Trace (src/render.cpp:17-62) bit for bit.
+        rays: contiguous float32 CUDA tensor (N, 8) on the head device -- origin.xyz, time, dir.xyz, pad.
+        Returns (hits (N, 4) float32: t, normal.xyz; prims (N,) int32: closest primitive, -1 on a miss), in
+        `hits` / `prims` when given.  On the renderer's private stream the call first waits for torch's current
+        stream, so that tensors written there are complete; after set_stream the work is ordered on that stream."""
+        import torch
+        dev = torch.device("cuda", self.device)
+
+        def check(x, name, shape, dtype):
+            if not isinstance(x, torch.Tensor):
+                raise TypeError("%s must be a torch tensor" % name)
+            if x.dtype != dtype:
+                raise TypeError("%s must be %s, not %s" % (name, dtype, x.dtype))
+            if tuple(x.shape) != shape:
+                raise ValueError("%s must have shape %s, not %s" % (name, shape, tuple(x.shape)))
+            if x.device != dev:
+                raise ValueError("%s must be on %s (the renderer's head device), not %s" % (name, dev, x.device))
+            if not x.is_contiguous():
+                raise ValueError("%s must be contiguous" % name)
+
+        if not isinstance(rays, torch.Tensor) or rays.dim() != 2:
+            raise ValueError("rays must be a (N, 8) tensor")
+        n = rays.shape[0]
+        check(rays, "rays", (n, 8), torch.float32)
+        if hits is None:
+            hits = torch.empty((n, 4), dtype=torch.float32, device=dev)
+        if prims is None:
+            prims = torch.empty((n,), dtype=torch.int32, device=dev)
+        check(hits, "hits", (n, 4), torch.float32)
+        check(prims, "prims", (n,), torch.int32)
+        if n == 0:
+            return hits, prims
+        if not self._external_stream:
+            torch.cuda.current_stream(dev).synchronize()
+        self._check(self.lib.tb200_trace_rays(self.h, rays.data_ptr(), hits.data_ptr(), prims.data_ptr(), n), "tb200_trace_rays")
+        return hits, prims
 
     def set_frame(self, frame):
         self.lib.tb200_set_frame(self.h, frame)

@@ -140,6 +140,16 @@ class Stats(C.Structure):
     ]
 
 
+class Ray(C.Structure):
+    """tb200_ray: one ray of tb200_trace_rays (32 bytes)."""
+    _fields_ = [("origin", C.c_float * 3), ("time", C.c_float), ("dir", C.c_float * 3), ("pad", C.c_float)]
+
+
+class Hit(C.Structure):
+    """tb200_hit: what tb200_trace_rays returns per ray besides the primitive index (16 bytes)."""
+    _fields_ = [("t", C.c_float), ("normal", C.c_float * 3)]
+
+
 class BvhBuildInfo(C.Structure):
     _fields_ = [("numNodes", C.c_int32), ("rounds", C.c_int32), ("kernelLaunches", C.c_uint64), ("buildMs", C.c_double)]
 
@@ -179,6 +189,7 @@ EXPORTS = [
     "tb200_finish",
     "tb200_nlm",
     "tb200_trace_frame",
+    "tb200_trace_rays",
     "tb200_set_frame",
     "tb200_get_stats",
     "tb200_last_kernel",

@@ -2007,6 +2007,94 @@ int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200
     return 0;
 }
 
+// cuMemGetAddressRange (driver API), reached through the runtime so that the library needs no -lcuda
+typedef int (*MemRangeFn)(unsigned long long* base, size_t* size, unsigned long long ptr);
+
+static MemRangeFn mem_range_fn()
+{
+    static MemRangeFn fn = [] {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult status = cudaDriverEntryPointSymbolNotFound;
+        if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &p, cudaEnableDefault, &status) != cudaSuccess ||
+            status != cudaDriverEntryPointSuccess) {
+            cudaGetLastError();
+            p = nullptr;
+        }
+        return (MemRangeFn)p;
+    }();
+    return fn;
+}
+
+// `bytes` from `ptr` lie inside one allocation of device memory on r's device
+static bool check_device_span(const tb200_renderer* r, const void* ptr, size_t bytes, size_t align, const char* what)
+{
+    const std::string name = std::string("tb200_trace_rays: ") + what;
+    if (!ptr) return set_error(name + " is null");
+    if ((uintptr_t)ptr % align != 0) return set_error(name + " is not aligned to " + std::to_string(align) + " bytes");
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, ptr) != cudaSuccess) {
+        cudaGetLastError();
+        return set_error(name + " is not a CUDA pointer");
+    }
+    if (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)
+        return set_error(name + " is not device memory (host memory is not accepted)");
+    if (attr.device != r->device)
+        return set_error(name + " lies on device " + std::to_string(attr.device) + ", not on the renderer's device " + std::to_string(r->device));
+    const MemRangeFn range = mem_range_fn();
+    if (!range) return set_error("tb200_trace_rays: cuMemGetAddressRange is not available from the driver");
+    unsigned long long base = 0;
+    size_t size = 0;
+    if (range(&base, &size, (unsigned long long)(uintptr_t)ptr) != 0) return set_error(name + ": the driver knows no allocation at this address");
+    const unsigned long long p = (unsigned long long)(uintptr_t)ptr;
+    if (bytes > size || p - base > size - bytes)
+        return set_error(name + ": " + std::to_string(bytes) + " bytes from this address run past the end of its allocation");
+    return true;
+}
+
+int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, int64_t numRays)
+{
+    if (!r) {
+        set_error("tb200_trace_rays: null renderer");
+        return -1;
+    }
+    if (numRays < 0 || numRays > (int64_t)(SIZE_MAX / sizeof(tb200_ray))) {
+        set_error("tb200_trace_rays: numRays " + std::to_string((long long)numRays) + " is out of range");
+        return -1;
+    }
+    if (numRays == 0) return 0;
+    cudaSetDevice(r->device);   // a multi-device renderer answers on its head, which holds a full copy of the scene
+    const size_t n = (size_t)numRays;
+    if (!check_device_span(r, rays, n * sizeof(tb200_ray), 16, "rays") || !check_device_span(r, hits, n * sizeof(tb200_hit), 16, "hits") ||
+        !check_device_span(r, prims, n * sizeof(int32_t), 4, "prims"))
+        return -1;
+    static_assert(sizeof(tb200_ray) == 32 && sizeof(tb200_hit) == 16, "the query kernel reads two float4 per ray and writes one");
+    QueryParams Q;
+    Q.scene = r->scene;
+    Q.rays = reinterpret_cast<const float4*>(rays);
+    Q.hits = reinterpret_cast<float4*>(hits);
+    Q.prims = prims;
+    Q.numRays = numRays;
+    Q.counter = r->dCounter;   // the wavefront's work counter: free between launches on this stream
+    unsigned long long launches = 0;
+    if (cudaEventRecord(r->evStart, r->stream) != cudaSuccess) {
+        set_error(std::string("tb200_trace_rays: ") + cudaGetErrorString(cudaGetLastError()));
+        return -1;
+    }
+    launch_trace_rays(Q, r->numSMs, r->stream, &launches);
+    r->stats.kernelLaunches += launches;
+    float ms = 0.0f;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaEventRecord(r->evStop, r->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, r->evStart, r->evStop);
+    if (e != cudaSuccess) {
+        set_error(std::string("tb200_trace_rays: ") + cudaGetErrorString(e));
+        return -1;
+    }
+    r->stats.gpuMs = ms;
+    return 0;
+}
+
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds only (-DTB_WF2_STAGE_CLOCKS, tools/stage_clocks.py): copies the lane-owned wavefront
 // layout's per-stage cycle counters of the current device into out[0..n) (n >= 15 words, see wavefront2.cuh:

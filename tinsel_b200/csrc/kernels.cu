@@ -356,3 +356,8 @@ const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t st
         return wf2_lq::launch_layout(p, numSMs, stream, launchCount);
     return wf2_smem::launch_layout(p, numSMs, stream, launchCount);
 }
+
+// ------------------------------------------------------------------------------------------------
+// Batched closest-hit ray query: see tb_query.cuh
+// ------------------------------------------------------------------------------------------------
+#include "tb_query.cuh"

@@ -98,3 +98,14 @@ struct NlmParams {
     float falloff;
 };
 void launch_nlm(const NlmParams& p, cudaStream_t stream, unsigned long long* launchCount);
+
+// Batched closest-hit query (tb200_trace_rays, tb_query.cuh): Trace (render.cpp:17-62) of every ray.
+struct QueryParams {
+    DScene scene;
+    const float4* rays;   // 2 per ray: origin.xyz, time; dir.xyz, pad
+    float4* hits;         // 1 per ray: t, normal.xyz
+    int* prims;           // 1 per ray: closest primitive, -1 on a miss
+    long long numRays;
+    unsigned long long* counter;   // work counter, cleared by the launch
+};
+const char* launch_trace_rays(const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);

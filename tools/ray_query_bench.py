@@ -1,0 +1,145 @@
+#!/usr/bin/env python
+"""Throughput of the batched closest-hit query (Renderer.trace_rays / tb200_trace_rays), one JSON line per scene:
+    python tools/ray_query_bench.py [--scenes cornell,veach,meshlight,ajax,env] [--calls 10] [--warmup 3]
+
+Per scene: Mrays/s for 2^24 coherent camera rays (a raster-order 4096 x 4096 grid, jittered) and 2^24 random rays
+(origins in and around the scene bounds, uniform directions), from CUDA events around `--calls` timed calls after
+the warm-up; the bytes each ray moves (32 in, 20 out) against the H100 SXM's 3.35 TB/s; the CPU restatement's
+rate on every host core (tests/rayoracle.py); a bit-exact check of 2^16 rays against it; and the GPU's name and power
+limit, read in the same run.  ajax and env are skipped when their snapshots are not present.  Needs a GPU."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import tinsel_b200 as tb  # noqa: E402
+import rayoracle  # noqa: E402
+import raysets  # noqa: E402
+
+HBM_BYTES_PER_S = 3.35e12
+BYTES_PER_RAY = 32 + 16 + 4
+
+
+def gpu_info():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                             text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, power = [x.strip() for x in out.split(",")]
+        return name, power
+    except Exception as e:   # the rates are still measured; the line says what could not be read
+        import torch
+        return torch.cuda.get_device_name(0), "unknown (%s)" % type(e).__name__
+
+
+def camera_rays_device(torch, camera, side, seed):
+    """side*side camera rays in raster order (neighbouring rays are neighbouring pixels), on the device."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    n = side * side
+    idx = torch.arange(n, device="cuda")
+    px = (idx % side).float() + torch.rand(n, device="cuda", generator=g)
+    py = (idx // side).float() + torch.rand(n, device="cuda", generator=g)
+    f = float(np.tan(camera.fov * 0.5))
+    d = torch.stack([(2.0 * px / side - 1.0) * f, (1.0 - 2.0 * py / side) * f, -torch.ones(n, device="cuda")], 1)
+    d = d / d.norm(dim=1, keepdim=True)
+    q = torch.tensor(camera.rotation[:], device="cuda")
+    u = q[:3].expand(n, 3)
+    t = 2.0 * torch.cross(u, d, dim=1)
+    d = d + q[3] * t + torch.cross(u, t, dim=1)
+    rays = torch.zeros((n, 8), device="cuda")
+    rays[:, 0:3] = torch.tensor(camera.position[:], device="cuda")
+    rays[:, 3] = camera.shutterStart + (camera.shutterEnd - camera.shutterStart) * torch.rand(n, device="cuda", generator=g)
+    rays[:, 4:7] = d
+    return rays
+
+
+def random_rays_device(torch, scene, n, seed):
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    lo, hi = raysets.scene_bounds(scene)
+    pad = 0.2 * (hi - lo) + 1e-3
+    lo_t = torch.tensor(lo - pad, device="cuda", dtype=torch.float32)
+    span = torch.tensor((hi - lo) + 2 * pad, device="cuda", dtype=torch.float32)
+    d = torch.randn((n, 3), device="cuda", generator=g)
+    rays = torch.zeros((n, 8), device="cuda")
+    rays[:, 0:3] = lo_t + span * torch.rand((n, 3), device="cuda", generator=g)
+    rays[:, 3] = torch.rand(n, device="cuda", generator=g)
+    rays[:, 4:7] = d / d.norm(dim=1, keepdim=True)
+    return rays
+
+
+def time_calls(torch, r, rays, hits, prims, warmup, calls):
+    """ms per call from CUDA events around `calls` calls on the caller's stream, and the kernel's own median time."""
+    stream = torch.cuda.current_stream()
+    r.set_stream(stream.cuda_stream)
+    for _ in range(warmup):
+        r.trace_rays(rays, hits, prims)
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    kernel = []
+    start.record(stream)
+    for _ in range(calls):
+        r.trace_rays(rays, hits, prims)
+        kernel.append(r.stats().gpuMs)
+    end.record(stream)
+    end.synchronize()
+    r.set_stream(None)
+    return start.elapsed_time(end) / calls, float(np.median(kernel))
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--scenes", default="cornell,veach,meshlight,ajax,env")
+    ap.add_argument("--calls", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--log2-rays", type=int, default=24)
+    args = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("ray_query_bench: no CUDA device (the rates are GPU measurements)")
+    rayoracle.load()
+    gpu, power = gpu_info()
+    n = 1 << args.log2_rays
+    side = 1 << (args.log2_rays // 2)
+    for name in args.scenes.split(","):
+        path = tb.scene_path(name)
+        if not os.path.exists(path):
+            continue
+        snap = tb.Snapshot(path)
+        scene = snap.scene.contents
+        r = tb.Renderer(snap.scene)
+        port = rayoracle.RayOracle.from_snapshot(path)
+        line = {"scene": name, "rays": n, "gpu": gpu, "power_limit": power,
+                "library": os.path.basename(os.environ.get("TINSEL_B200_LIB", tb.LIB_PATH))}
+        hits = torch.empty((n, 4), device="cuda")
+        prims = torch.empty((n,), device="cuda", dtype=torch.int32)
+        for kind in ("camera", "random"):
+            rays = camera_rays_device(torch, snap.camera, side, 1) if kind == "camera" else random_rays_device(torch, scene, n, 2)
+            ms, kms = time_calls(torch, r, rays, hits, prims, args.warmup, args.calls)
+            line[kind] = {"ms_per_call": round(ms, 4), "kernel_ms": round(kms, 4), "mrays_per_s": round(n / ms / 1e3, 1),
+                          "bytes_per_ray": BYTES_PER_RAY, "hbm_floor_ms": round(n * BYTES_PER_RAY / HBM_BYTES_PER_S * 1e3, 4),
+                          "share_of_hbm_floor": round(n * BYTES_PER_RAY / HBM_BYTES_PER_S * 1e3 / kms, 4) if kms > 0 else None}
+            # the CPU restatement on every host core, on the first 2^20 rays of the same batch
+            sub = rays[: min(n, 1 << 20)].cpu().numpy()
+            t0 = time.perf_counter()
+            want_h, want_p = port.trace_rays(sub)
+            line[kind]["cpu_mrays_per_s"] = round(len(sub) / (time.perf_counter() - t0) / 1e6, 2)
+            k = min(n, 1 << 16)
+            got_h, got_p = hits[:k].cpu().numpy(), prims[:k].cpu().numpy()
+            line[kind]["bit_exact_2^16"] = len(raysets.mismatches(got_h, got_p, want_h[:k], want_p[:k])) == 0
+            line[kind]["hit_fraction"] = round(float((prims >= 0).float().mean()), 4)
+            del rays
+        line["cpu_threads"] = os.cpu_count()
+        print(json.dumps(line), flush=True)
+        r.close()
+        port.close()
+        snap.close()
+
+
+if __name__ == "__main__":
+    main()
