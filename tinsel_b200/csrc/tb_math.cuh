@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <float.h>
+#include <string.h>
 
 #include "tb200_detmath.h"
 
@@ -96,11 +97,35 @@ struct Xf {
     float s;
 };
 
+TB_HD uint32_t tb_float_bits(float f)
+{
+#if defined(__CUDA_ARCH__)
+    return __float_as_uint(f);
+#else
+    uint32_t u;
+    memcpy(&u, &f, sizeof(u));
+    return u;
+#endif
+}
+
+// rotate(q, v), or rotate(qconj(q), v) when `inverse`, for the rotation of a transform.  When q is (+0, +0, +0, +1)
+// bit for bit and v is finite, every sum in both qmuls adds only exact zeros to the one product v.c * 1, and the +0
+// among them turns a -0 into +0: the result is v + 0.0f, in either direction.  Any other quaternion (a -0 component
+// included) and a non-finite v (0 * inf is NaN) take the full rotation.
+TB_HD V3 rotate_xf(Q4 q, V3 v, bool inverse)
+{
+    const bool unrotated = (tb_float_bits(q.x) | tb_float_bits(q.y) | tb_float_bits(q.z)) == 0u && tb_float_bits(q.w) == 0x3f800000u;
+    if (unrotated && fabsf(v.x) <= FLT_MAX && fabsf(v.y) <= FLT_MAX && fabsf(v.z) <= FLT_MAX) return v + v3s(0.0f);
+    return rotate(inverse ? qconj(q) : q, v);
+}
+// 1.0f / s, without the IEEE division for the common unit scale (1.0f / 1.0f is 1.0f)
+TB_HD float inverse_scale(float s) { return s == 1.0f ? 1.0f : 1.0f / s; }
+
 // maths.h:601-619
-TB_HD V3 transform_vector(const Xf& t, V3 v) { return rotate(t.r, t.s * v); }
-TB_HD V3 transform_point(const Xf& t, V3 v) { return t.p + rotate(t.r, t.s * v); }
-TB_HD V3 inverse_transform_vector(const Xf& t, V3 v) { return (1.0f / t.s) * rotate(qconj(t.r), v); }
-TB_HD V3 inverse_transform_point(const Xf& t, V3 v) { return (1.0f / t.s) * rotate(qconj(t.r), v - t.p); }
+TB_HD V3 transform_vector(const Xf& t, V3 v) { return rotate_xf(t.r, t.s * v, false); }
+TB_HD V3 transform_point(const Xf& t, V3 v) { return t.p + rotate_xf(t.r, t.s * v, false); }
+TB_HD V3 inverse_transform_vector(const Xf& t, V3 v) { return inverse_scale(t.s) * rotate_xf(t.r, v, true); }
+TB_HD V3 inverse_transform_point(const Xf& t, V3 v) { return inverse_scale(t.s) * rotate_xf(t.r, v - t.p, true); }
 
 // maths.h:1566-1569 with Quat Lerp (maths.h:79-83 over Quat ops) and Normalize(Quat) (maths.h:547-553)
 #if defined(__CUDA_ARCH__)

@@ -392,6 +392,58 @@ static __device__ __noinline__ MeshHit ray_mesh(const DMesh& m, const unsigned c
     return out;
 }
 
+// ray_mesh() for a BVH that is one leaf, or one interior pair over two leaves (a quad: cornell's light), inline and
+// without the stack.  The reference pops the root, pushes each child whose box passes `tChild < tmax` (tmax is
+// still FLT_MAX), the nearer one last when both do, then pops and tests the triangles in turn; no box test follows,
+// so the truncation of the ray changes nothing.  Returns false, having done nothing, for any other tree.
+TB_DEV bool ray_mesh_small(const DMesh& m, V3 origin, V3 dir, MeshHit& out)
+{
+    // the leaves in the order the reference pops them; a reference without TB_LEAF ends the list
+    uint32_t first = m.rootRef, second = 0u;
+    if (!(first & TB_LEAF)) {
+        const BvhPair* pr = &m.pairs[first];
+        const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
+        if (!(kids.x & kids.y & TB_LEAF)) return false;
+        const float4 a = pr->a, b = pr->b, c = pr->c;
+        V3 rcp;
+        rcp.x = 1.0f / dir.x;
+        rcp.y = 1.0f / dir.y;
+        rcp.z = 1.0f / dir.z;
+        float tLeft, tRight;
+        const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < FLT_MAX;
+        const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < FLT_MAX;
+        const bool both = hitLeft && hitRight;
+        const bool swap = both && (tLeft < tRight);   // left pushed last: it pops first
+        first = hitRight ? (swap ? kids.x : kids.y) : (hitLeft ? kids.x : 0u);
+        second = both ? (swap ? kids.y : kids.x) : 0u;
+    }
+    float closestT = FLT_MAX;
+    out.tri = -1;
+    out.u = out.v = out.w = 0.0f;
+    out.n = v3s(0.0f);
+#pragma unroll 1
+    for (uint32_t ref = first; ref & TB_LEAF; ref = second, second = 0u) {
+        const uint32_t i = ref & ~TB_LEAF;
+        const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
+        const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
+        const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
+        float t, u, v, w, sign;
+        V3 n;
+        if (ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n)) {
+            if (t > 0.0f && t < closestT) {
+                closestT = t;
+                out.u = u;
+                out.v = v;
+                out.w = w;
+                out.tri = (int)i;
+                out.n = n * sign;
+            }
+        }
+    }
+    out.t = closestT;
+    return true;
+}
+
 // PrimitiveIntersect, intersection.h:951-1020, split in two: prim_test() decides hit / t exactly
 // as the reference does, prim_normal() produces *outNormal for a recorded hit.  The reference
 // computes the normal of every candidate (no side effects); only the winner's is ever used, so
@@ -437,8 +489,12 @@ TB_DEV bool prim_test(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, 
     // mesh
     const V3 lo = inverse_transform_point(xf, o);
     const V3 ld = inverse_transform_vector(xf, d);
-    const bool staged = p.mesh == sc.treeletMesh && sc.treelet != nullptr;
-    const MeshHit mh = ray_mesh(sc.meshes[p.mesh], sc.treelet, staged ? (uint32_t)sc.treeletPairs : 0u, lo, ld);
+    const DMesh& m = sc.meshes[p.mesh];
+    MeshHit mh;
+    if (!ray_mesh_small(m, lo, ld, mh)) {
+        const bool staged = p.mesh == sc.treeletMesh && sc.treelet != nullptr;
+        mh = ray_mesh(m, sc.treelet, staged ? (uint32_t)sc.treeletPairs : 0u, lo, ld);
+    }
     if (mh.tri < 0) return false;
     ph.t = mh.t;
     ph.tri = mh.tri;
