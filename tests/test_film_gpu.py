@@ -30,7 +30,7 @@ CAP_KEY = "TINSEL_B200_TEST_LAUNCH_SAMPLES"
 @pytest.fixture(scope="module")
 def scenes(tmp_path_factory):
     """name -> snapshot path; "big-mesh" is a fuzz scene with a mesh of more than 4096 triangles, so that the
-    split trace queue, the treelet and the offload engage."""
+    split trace queue and the treelet engage."""
     paths = {n: tb.scene_path(n) for n in ("cornell", "veach", "meshlight", "motionblur", "many")}
     d = tmp_path_factory.mktemp("film")
     paths["big-mesh"] = str(d / "big.tsnap")

@@ -280,7 +280,7 @@ def test_both_scheduling_modes_bit_exact(sched, cta):
             if not _available(name):
                 continue
             snap, cam, opt, ref, r = _setup(name, "wavefront")
-            for frame in (3, 4):   # two launches: the offload queues' counters and lap tags run on across launches
+            for frame in (3, 4):   # two launches of one renderer: the second starts from the device buffers the first left
                 rad, _ = r.trace_frame(cam, opt, frame)
                 rrad, _ = ref.trace_frame(frame, nthreads=8)
                 assert (rad.view(np.uint32) == rrad.view(np.uint32)).all(), (name, frame)

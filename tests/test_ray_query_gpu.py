@@ -141,7 +141,7 @@ def test_mesh_with_device_built_bvh_matches_port():
     base.close()
 
 
-@pytest.mark.parametrize("variant", ["no_flat", "offload", "cached", "group"])
+@pytest.mark.parametrize("variant", ["no_flat", "cached", "group"])
 @pytest.mark.parametrize("name", ["cornell", "meshlight", "fuzz_instanced"])
 def test_variants_give_the_same_bits(variant, name, monkeypatch, tmp_path):
     if name.startswith("fuzz_"):
@@ -155,10 +155,6 @@ def test_variants_give_the_same_bits(variant, name, monkeypatch, tmp_path):
     rays = np.concatenate(list(_ray_sets(snap.scene.contents, snap.camera, port, rng).values()))
     if variant == "no_flat":
         monkeypatch.setenv("TINSEL_B200_NO_FLAT", "1")
-        r = tb.Renderer(snap.scene)
-    elif variant == "offload":
-        monkeypatch.setenv("TINSEL_B200_OFFLOAD", "2")
-        monkeypatch.setenv("TINSEL_B200_SCHED", "free")
         r = tb.Renderer(snap.scene)
     elif variant == "cached":
         cache = str(tmp_path / "s.tcache")

@@ -113,9 +113,9 @@ DMaterial make_material(const tb200_material& m)
 }
 
 // BVHNode[] (bvh.h:9-19) -> BvhPair[]; see tb_scene.cuh.  Returns the root reference.  Pairs are laid out
-// in breadth-first order from the root, so that the first K records are the top of the tree: the walker
-// CTAs of the offload mode stage exactly that prefix in shared memory with one bulk copy
-// (wavefront_walk.cuh), and the upper levels share cache lines for everybody else.  Record indices are
+// in breadth-first order from the root, so that the first K records are the top of the tree: the treelet
+// (DScene::treelet) stages exactly that prefix in shared memory with bulk copies, and the upper levels
+// share cache lines for everybody else.  Record indices are
 // private to this layout; topology, child order and therefore visit order are the reference's.
 // *depth (optional) receives the number of levels of interior nodes.
 uint32_t build_pairs(const tb200_bvh_node* nodes, int numNodes, std::vector<BvhPair>* out, int* depth = nullptr)
@@ -343,12 +343,6 @@ struct tb200_renderer {
     std::string workerError;              // a peer's failure message, handed to the calling thread
     bool peerAccess = false;
 
-    // mesh-walk offload (wavefront_walk.cuh): queues in device memory, walker CTAs per launch
-    WalkParams walk;
-    void* dWalkBlock = nullptr;   // one allocation behind every pointer of `walk`
-    size_t walkBlockBytes = 0;
-    int numWalkers = 0;           // 0: the offload mode is off
-
     int pipeline = 2;             // 0 = mega (validation), 2 = wavefront (product)
     int hardPhases = 1;           // wavefront scheduling mode (see wavefront2.cuh)
     int wideCta = 0;              // 768-thread CTAs for deep mesh BVHs (see wavefront2.cuh)
@@ -391,9 +385,6 @@ void free_device(tb200_renderer* r)
     r->dCold = nullptr;
     cudaFree(r->dBandCount);
     r->dBandCount = nullptr;
-    cudaFree(r->dWalkBlock);
-    r->dWalkBlock = nullptr;
-    r->numWalkers = 0;
     cudaFree(r->dFiltered);
     cudaFree(r->dRgb8);
     cudaFree(r->dDither);
@@ -556,86 +547,6 @@ bool image_from_scene(const tb200_scene* s, SceneImage* img)
     return true;
 }
 
-// Mesh-walk offload (wavefront_walk.cuh): decided per scene.  Eligible: free-running scenes whose scene
-// level runs as the flat program (<= 16 primitives) and that hold a mesh of more than 4096 triangles whose
-// BVH is no deeper than the reference's own traversal stack (a deeper tree overflows `int stack[32]`,
-// intersection.h:688, in the reference itself).  TINSEL_B200_OFFLOAD=0 turns it off, =1 offloads every
-// mesh (tests); TINSEL_B200_WALKERS=n sets the number of walker CTAs.
-bool setup_offload(tb200_renderer* r, const SceneImage& img)
-{
-    DScene& sc = r->scene;
-    sc.deferMask = 0u;
-    r->numWalkers = 0;
-    memset(&r->walk, 0, sizeof(r->walk));
-    r->walk.treeletMesh = -1;
-    // Measured in round 2: with the walk offloaded ajax, env and meshlight all ran slower than with the inline
-    // walk, so the mode is OFF unless asked for:
-    // TINSEL_B200_OFFLOAD=1 offloads every eligible mesh of more than 4096 triangles, =2 every mesh (tests).
-    const char* env = getenv("TINSEL_B200_OFFLOAD");
-    const int want = env ? atoi(env) : 0;
-    const bool force = want == 2;
-    if (want <= 0 || r->hardPhases || sc.numFlat <= 0 || img.prims.size() > 16) return true;
-    int bigMesh = -1, bigTris = 0;
-    for (size_t i = 0; i < img.prims.size(); ++i) {
-        const DPrim& p = img.prims[i];
-        if (p.type != TB200_MESH) continue;
-        const MeshImage& mi = img.meshes[p.mesh];
-        if ((mi.numTris > 4096 || force) && mi.depth <= TB200_MAX_BVH_LEVELS) {
-            sc.deferMask |= 1u << i;
-            if (mi.numTris > bigTris) {
-                bigTris = mi.numTris;
-                bigMesh = p.mesh;
-            }
-        }
-    }
-    if (sc.deferMask == 0u) return true;
-
-    // queues: a request ring with more cells than the device has path slots (one request per slot at most),
-    // two answer rings of TB_WF2_SLOTS cells per shader CTA, a handful of counters
-    const int ctas = std::max(1, r->numSMs);
-    unsigned int log2 = 10;
-    while ((1ull << log2) < (unsigned long long)ctas * TB_WF2_SLOTS) ++log2;
-    const size_t reqBytes = (size_t(1) << log2) * 48, ansBytes = size_t(ctas) * 2 * TB_WF2_SLOTS * 48;
-    const size_t ctrBytes = (size_t(ctas) * 2 + 16) * sizeof(unsigned int);
-    r->walkBlockBytes = reqBytes + ansBytes + ctrBytes;
-    TB_CUDA(cudaMalloc(&r->dWalkBlock, r->walkBlockBytes));
-    TB_CUDA(cudaMemset(r->dWalkBlock, 0, r->walkBlockBytes));
-    char* base = (char*)r->dWalkBlock;
-    WalkParams& W = r->walk;
-    W.reqRing = (uint4*)base;
-    W.reqLog2 = log2;
-    W.ansRing = (uint4*)(base + reqBytes);
-    unsigned int* ctr = (unsigned int*)(base + reqBytes + ansBytes);
-    W.reqTail = ctr + 0;
-    W.reqHead = ctr + 1;
-    W.shadersDone = ctr + 2;
-    W.walkersDone = ctr + 3;
-    W.abortFlag = ctr + 4;
-    W.ansTail = ctr + 16;
-    W.treeletMesh = bigMesh;
-    W.treeletPairs = bigMesh >= 0 ? (int)img.meshes[bigMesh].pairs.size() : 0;
-    const char* nw = getenv("TINSEL_B200_WALKERS");
-    r->numWalkers = nw ? atoi(nw) : (ctas * 3) / 8;
-    r->numWalkers = std::max(1, std::min(r->numWalkers, ctas - 1));
-    r->tunePhase = 3;   // the split-queue tuner belongs to the inline walk
-    return true;
-}
-
-// After a launch of the offload mode has been waited for: did a watchdog fire?  (It never should: the
-// flag means shader and walker CTAs stopped waiting for each other after seconds without progress.)
-bool check_offload(tb200_renderer* r)
-{
-    if (r->numWalkers <= 0 || !r->dWalkBlock) return true;
-    unsigned int flag = 0;
-    TB_CUDA(cudaMemcpyAsync(&flag, r->walk.abortFlag, sizeof(flag), cudaMemcpyDeviceToHost, r->stream));
-    TB_CUDA(cudaStreamSynchronize(r->stream));
-    if (flag == 0u) return true;
-    cudaMemsetAsync(r->dWalkBlock, 0, r->walkBlockBytes, r->stream);   // queues and counters back to a clean state
-    cudaStreamSynchronize(r->stream);
-    return set_error(flag == 1u ? "mesh-walk offload: a shader CTA waited for the walkers without progress (watchdog); the frame is incomplete"
-                                : "mesh-walk offload: a walker CTA waited for requests without progress (watchdog); the frame is incomplete");
-}
-
 // The scene's features (tb_scene.cuh: TB_FEAT_*).  A scene without any of them runs the lane-owned kernel compiled
 // without them (wavefront2.cuh: wf2_lq::launch_layout); a NaN parameter counts as present.
 uint32_t scene_features(const SceneImage& img)
@@ -731,11 +642,9 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
     if (!upload(flat, &r->dFlat, h2d, 1)) return false;
     sc.flat = r->dFlat;
     sc.numFlat = (int)flat.size();
-    if (!setup_offload(r, img)) return false;
-    // treelet: the top of the largest mesh's BVH staged in the shared memory the slot arrays leave, for the INLINE
+    // treelet: the top of the largest mesh's BVH staged in the shared memory the slot arrays leave, for the
     // mesh walk.  Measured in round 2: slower on every scene (ajax, env, meshlight) because the top levels already
-    // live in L1, and claiming the last 45 KB of shared memory shrinks L1 from 60 to 28 KB.  Off unless TINSEL_B200_TREELET=1.  (The walker CTAs
-    // of the offload mode always stage theirs: they have nothing else in shared memory.)
+    // live in L1, and claiming the last 45 KB of shared memory shrinks L1 from 60 to 28 KB.  Off unless TINSEL_B200_TREELET=1.
     sc.treelet = nullptr;
     sc.treeletMesh = -1;
     sc.treeletPairs = 0;
@@ -985,8 +894,6 @@ bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_opti
     }
     P->shard = r->shard;
     P->numShards = r->numShards;
-    P->walk = r->walk;
-    P->walk.numWalkers = r->numWalkers;
     finalize_params(P);
     return true;
 }
@@ -1040,7 +947,6 @@ void tune_update(tb200_renderer* r)
 bool finish_timing(tb200_renderer* r)
 {
     TB_CUDA(cudaStreamSynchronize(r->stream));
-    if (!check_offload(r)) return false;
     float ms = 0.0f;
     TB_CUDA(cudaEventElapsedTime(&ms, r->evStart, r->evStop));
     r->stats.gpuMs = ms;
@@ -1074,7 +980,7 @@ bool read_back(tb200_renderer* r, float* output)
         TB_CUDA(cudaMemcpyAsync((char*)output + size_t(row0) * rowBytes, accum + size_t(row0) * rowBytes, bytes, cudaMemcpyDeviceToHost, r->stream));
     TB_CUDA(cudaStreamSynchronize(r->stream));
     r->stats.d2hBytes += bytes;
-    return check_offload(r);
+    return true;
 }
 
 // One frame of the wavefront kernel with the read-back streamed underneath it: samples are handed
@@ -1139,7 +1045,7 @@ bool render_streamed(tb200_renderer* r, LaunchParams& P, float* output, bool rec
     TB_CUDA(cudaStreamSynchronize(r->copyStream));
     if (copyFailed) TB_CUDA(cudaErrorUnknown);
     r->stats.d2hBytes += size_t(own1 - own0) * rowBytes;
-    return check_offload(r);
+    return true;
 }
 
 }  // namespace
@@ -2003,7 +1909,6 @@ int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200
         return -1;
     }
     r->stats.d2hBytes += n * 5 * sizeof(float);
-    if (!check_offload(r)) return -1;
     return 0;
 }
 

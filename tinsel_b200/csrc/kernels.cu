@@ -302,18 +302,12 @@ static size_t wavefront2_smem_limit()
     return (size_t)v;
 }
 
-// offload mode (wavefront_walk.cuh): a launch uses it when the renderer set it up for this scene
-static inline bool wavefront2_wants_offload(const LaunchParams& p)
-{
-    return p.walk.numWalkers > 0 && !p.hardPhases && p.scene.deferMask != 0u && p.scene.numFlat > 0;
-}
-
 // Three layouts of the wavefront's slot state and queues, one compilation of wavefront2.cuh each:
 //  * wf2_smem: 1024 slots per CTA, hot + cold state in shared memory.  Scenes held on chip (cornell, veach):
 //    they are issue-bound, and fetching the cold half from L2 slows them down.
 //  * wf2_l2: 2048 slots per CTA, the cold half (27 of 45 words) in a 128-byte record per slot in global
-//    memory, L2-resident.  Scenes with deep mesh BVHs (ajax, env) and the offload mode: their
-//    rays take long, and twice the paths in flight hide it.
+//    memory, L2-resident.  Scenes with deep mesh BVHs (ajax, env): their rays take long, and twice the
+//    paths in flight hide it.
 //  * wf2_lq: wf2_smem's state with LANE-OWNED slots and bit-set stage queues instead of rings, free-running
 //    scheduler only: no shared-memory bank conflicts and far cheaper queue operations, at the price of the
 //    rings' FIFO order (scenes held on chip do not care; deep BVHs such as ajax do).
@@ -350,7 +344,7 @@ const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t st
     // fewer than six samples per slot keep the rings.
     const unsigned long long total = p.samplesPerFrame * (unsigned long long)p.numFrames;
     const bool small = total < 6ull * (unsigned long long)(numSMs > 0 ? numSMs : 132) * 1024ull;
-    if (p.wideCta || wavefront2_wants_offload(p))
+    if (p.wideCta)
         return wf2_l2::launch_layout(p, numSMs, stream, launchCount);
     if (!p.hardPhases && !p.scene.splitValid && (p.laneQueues == 2 || (p.laneQueues == 1 && !small)))
         return wf2_lq::launch_layout(p, numSMs, stream, launchCount);

@@ -3,26 +3,10 @@
 
 #include "tb_film.cuh"
 
-// Mesh-walk offload of the wavefront kernel (wavefront_walk.cuh): the queues between shader CTAs and
-// walker CTAs, in global memory.  numWalkers == 0: the launch does not use it.
 // path slots per CTA of the wavefront kernel, at most (the layouts of kernels.cu use 1024 and 2048): the host
-// sizes the cold slot state and the offload queues with it
+// sizes the cold slot state with it
 #define TB_WF2_SLOTS 2048
 #define TB_WF2_MAX_CTAS_PER_SM 2   // the launch never places more CTAs per SM (the host sizes the cold state with it)
-struct WalkParams {
-    uint4* reqRing;                // (1 << reqLog2) cells x 3 chunks of 16 bytes
-    unsigned int reqLog2;
-    unsigned int* reqTail;
-    unsigned int* reqHead;
-    uint4* ansRing;                // [shader CTA][2][1024] cells x 3 chunks
-    unsigned int* ansTail;         // [shader CTA][2]
-    unsigned int* shadersDone;     // shader CTAs that have exited (this launch)
-    unsigned int* walkersDone;
-    unsigned int* abortFlag;       // set by a watchdog: everybody leaves, the host reports an error
-    int numShaders, numWalkers;
-    int treeletMesh;               // the mesh whose top-of-tree the walkers stage in shared memory (pairs in BFS order)
-    int treeletPairs;              // its number of pairs
-};
 
 struct LaunchParams {
     DScene scene;
@@ -52,7 +36,6 @@ struct LaunchParams {
     volatile unsigned int* bandFlags; // device pointer to pinned, mapped host memory
     unsigned int bandSamples;
     unsigned int bandTag;
-    WalkParams walk;
     // cold half of the wavefront's slot state: 8 x float4 per slot, TB_WF2_PATHS slots per CTA of the launch
     float4* cold;
     int treeletBytes;     // shared memory behind the slot arrays that the prologue fills with the top of DScene::treeletMesh's BVH

@@ -136,9 +136,6 @@ struct DScene {
     // the mesh or none does.
     int splitValid;
     V3 splitLo, splitHi;
-    // Offload mode of the wavefront kernel (wavefront_walk.cuh): bit i set = primitive i is a big mesh
-    // whose BVH walk runs on the walker CTAs; trace_partial() skips it and reports the rays that reach it.
-    uint32_t deferMask;
     // Treelet: the first `treeletPairs` pair records (breadth-first = the top levels) of mesh `treeletMesh`'s BVH,
     // staged in shared memory by the wavefront kernel's prologue (a TMA bulk copy); ray_mesh() reads records
     // below that index from there.  The host sets treeletMesh and the mesh's total pair count; the kernel clips
@@ -235,23 +232,9 @@ struct MeshHit {
     V3 n;   // closestNormal = n*sign, unnormalised (intersection.h:658)
 };
 
-// IntersectRayMesh + MeshQuery, intersection.h:629-749
-//
-// The lanes of a warp that walk a mesh together do it in PHASES, chosen by vote among them (TB_MESH_PHASES):
-//   BOX  interior-node steps, repeated while most of the lanes have one.  A lane that reaches a triangle parks
-//        it in `pend` and keeps descending -- speculatively: its later box tests use a stale, larger tmax, so it
-//        visits a superset of the reference's nodes; everything in the extra nodes lies at t >= the closest hit
-//        and fails the strict `t < closestT`, and triangles are still tested in the reference's order, so the
-//        result is the reference's bit for bit (the walker CTAs of wavefront_walk.cuh run the same scheme);
-//   TRI  the parked triangles are tested.
-// A data-dependent `if (leaf) ... else ...` per lane makes the warp execute both bodies in almost every
-// iteration; this way each pass runs one body with the lanes that are ready for it.  Measured in round 2:
-// bit-exact, but the votes cost more than the divergence they remove (ajax, table and cornell all ran slower),
-// so the plain loop below is the default (-DTB_MESH_PHASES=1 builds
-// the voted one; the walker CTAs of the offload mode, which have nothing else to do, keep theirs).
-#ifndef TB_MESH_PHASES
-#define TB_MESH_PHASES 0
-#endif
+// IntersectRayMesh + MeshQuery, intersection.h:629-749: the reference's stack walk, one triangle or interior
+// pair per iteration in the reference's order.  Pair records below `topCount` are read from `top` (the staged
+// treelet), the rest from the mesh's own array.
 // Returns the closest hit; tri == -1 (and t == FLT_MAX) when the ray misses the mesh.
 static __device__ __noinline__ MeshHit ray_mesh(const DMesh& m, const unsigned char* top, uint32_t topCount, V3 origin, V3 dir)
 {
@@ -267,85 +250,6 @@ static __device__ __noinline__ MeshHit ray_mesh(const DMesh& m, const unsigned c
     out.tri = -1;
     out.u = out.v = out.w = 0.0f;
     out.n = v3s(0.0f);
-#if TB_MESH_PHASES
-    const uint32_t EMPTY = 0xffffffffu;
-    const unsigned mask = __activemask();   // the lanes that entered together; every vote below is among them
-    const int group = __popc(mask);
-    const int boxMin = (group * 5 + 7) / 8, triMin = (group + 3) / 4;
-    int sp = 0;
-    uint32_t cur = m.rootRef, pend = EMPTY;
-    if (cur & TB_LEAF) {   // a one-triangle mesh
-        pend = cur;
-        cur = EMPTY;
-    }
-    for (;;) {
-        // ---- BOX ---------------------------------------------------------------------------------------------
-        int nBox;
-        for (;;) {
-            const bool wBox = cur != EMPTY && (cur & TB_LEAF) == 0u;
-            nBox = __popc(__ballot_sync(mask, wBox));
-            if (nBox == 0) break;
-            if (wBox) {
-                // IntersectRayMesh interior step, intersection.h:702-727; top of the tree from the staged treelet
-                // (shared memory) when there is one, the rest from global memory: one generic load path for both
-                const unsigned char* base = cur < topCount ? top : reinterpret_cast<const unsigned char*>(m.pairs);
-                const BvhPair* pr = reinterpret_cast<const BvhPair*>(base + (size_t)cur * sizeof(BvhPair));
-                const float4 a = pr->a, b = pr->b, c = pr->c;
-                const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
-                float tLeft, tRight;
-                const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < tmax;
-                const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < tmax;
-                // "traverse closest first": the reference pushes the far child, then the near one, and pops the near
-                // one at once (intersection.h:716-727) -- the near child is next, the far one goes on the stack
-                const bool both = hitLeft && hitRight;
-                const bool swap = both && (tLeft < tRight);
-                const uint32_t far = swap ? kids.y : kids.x;
-                uint32_t nxt = both ? (swap ? kids.x : kids.y) : (hitLeft ? kids.x : kids.y);
-                if (both) stack[sp++] = far;
-                if (!(hitLeft || hitRight)) nxt = sp > 0 ? stack[--sp] : EMPTY;
-                if (nxt != EMPTY && (nxt & TB_LEAF) != 0u && pend == EMPTY) {
-                    // park the triangle, go on with what the reference would pop after testing it
-                    pend = nxt;
-                    nxt = sp > 0 ? stack[--sp] : EMPTY;
-                }
-                cur = nxt;
-            }
-            if (nBox < boxMin) break;   // give the triangle phase a turn (one step per turn keeps every lane progressing)
-        }
-        // ---- TRI ---------------------------------------------------------------------------------------------
-        const bool wTri = pend != EMPTY;
-        const int nPend = __popc(__ballot_sync(mask, wTri));
-        if (nPend > 0 && (nPend >= triMin || nBox < boxMin)) {
-            if (wTri) {
-                // MeshQuery, intersection.h:629-674
-                const uint32_t i = pend & ~TB_LEAF;
-                const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
-                const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
-                const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
-                float t, u, v, w, sign;
-                V3 n;
-                if (ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n)) {
-                    if (t > 0.0f && t < closestT) {
-                        closestT = t;
-                        out.u = u;
-                        out.v = v;
-                        out.w = w;
-                        out.tri = (int)i;
-                        out.n = n * sign;
-                    }
-                }
-                tmax = closestT;   // "truncate ray", intersection.h:700
-                pend = EMPTY;
-                if (cur != EMPTY && (cur & TB_LEAF) != 0u) {
-                    // a second triangle was waiting behind the first
-                    pend = cur;
-                    cur = sp > 0 ? stack[--sp] : EMPTY;
-                }
-            }
-        }
-        if (__ballot_sync(mask, cur != EMPTY || pend != EMPTY) == 0u) break;   // every lane of the group is done
-    }
-#else
     stack[0] = m.rootRef;
     int count = 1;
     while (count) {
@@ -387,7 +291,6 @@ static __device__ __noinline__ MeshHit ray_mesh(const DMesh& m, const unsigned c
             if (hitRight) stack[count++] = right;
         }
     }
-#endif
     out.t = closestT;
     return out;
 }
@@ -671,92 +574,6 @@ TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNorm
     if (wantNormal && closest >= 0) {
         rec[ri].t = minT;
         nrm = prim_normal<FEAT>(sc, sc.prims[closest], o, d, time, rec[ri]);
-    }
-    h.n = face_forward(nrm, -d);
-    return h;
-}
-
-
-// trace_closest() for the offload mode of the wavefront kernel: the primitives of sc.deferMask (big
-// meshes) are not intersected here -- a ray that reaches one (its box test passed, or it sits behind
-// infinite boxes) gets that primitive's bit in `pending` and the caller posts it to the walker CTAs.
-// The hit returned covers all other primitives; merging it with the walkers' answer gives exactly
-// trace_closest()'s result, because the closest hit over a set of primitives does not depend on the
-// order they are tested in, EXCEPT for exact ties in t -- which the scene program detects among its
-// own primitives (below), the walkers among theirs, and the merge between the two; every tie is redone
-// with the reference-order walk.  Falls back to the complete trace_ordered() (pending == 0) for the
-// same rays trace_closest() does.
-TB_DEV Hit trace_partial(const DScene& sc, V3 o, V3 d, float time, bool wantNormal, uint32_t& pending)
-{
-    pending = 0u;
-    const int n = sc.numFlat;
-    const bool guard = (fabsf(o.x) < 1.0e7f) & (fabsf(o.y) < 1.0e7f) & (fabsf(o.z) < 1.0e7f) & (d.x == d.x) & (d.y == d.y) &
-                       (d.z == d.z);
-    if (n == 0 || !guard) return trace_ordered(sc, o, d, time, wantNormal);
-
-    V3 rcp;
-    rcp.x = 1.0f / d.x;
-    rcp.y = 1.0f / d.y;
-    rcp.z = 1.0f / d.z;
-
-    float minT = FLT_MAX;
-    int closest = -1;
-    bool tie = false;
-    PrimHit rec[2];
-    int ri = 0;
-    rec[0].t = 0.0f; rec[0].tri = 0; rec[0].u = rec[0].v = rec[0].w = 0.0f; rec[0].gn = v3s(0.0f);
-    uint32_t visited = 0u;
-    uint32_t wait = 0u;
-
-    for (int i = 0; i < n; ++i) {
-        const float4 a = *reinterpret_cast<const float4*>(sc.flat[i].a);
-        const float4 bk = *reinterpret_cast<const float4*>(sc.flat[i].b);   // b[0], b[1], kindPrim, bits
-        const int kindPrim = __float_as_int(bk.z), bits = __float_as_int(bk.w);
-        const int gbit = bits & 0xff;
-        if (gbit != TB_BIT_ALWAYS && !((visited >> gbit) & 1u)) continue;
-        const int kind = kindPrim & 0xff;
-        float t;
-        if (kind == TB_OP_PLANE) {
-            const float dd = a.x * d.x + a.y * d.y + a.z * d.z + a.w * 0.0f;
-            if (dd == 0.0f) continue;
-            t = -(a.x * o.x + a.y * o.y + a.z * o.z + a.w * 1.0f) / dd;
-        } else {
-            if (kind != TB_OP_LEAF) {
-                float tbox;
-                if (!ray_aabb(o, rcp, a.x, a.y, a.z, a.w, bk.x, bk.y, tbox)) continue;
-                if (kind == TB_OP_BOX) {
-                    visited |= 1u << ((bits >> 8) & 0xff);
-                    continue;
-                }
-            }
-            const int prim = kindPrim >> 8;
-            if ((sc.deferMask >> prim) & 1u) {
-                wait |= 1u << prim;
-                continue;
-            }
-            PrimHit* ph = &rec[ri ^ 1];
-            if (!prim_test(sc, sc.prims[prim], o, d, time, *ph)) continue;
-            t = ph->t;
-            if (t > 0.0f && t < minT) ri ^= 1;
-        }
-        if (t > 0.0f) {
-            if (t < minT) {
-                minT = t;
-                closest = kindPrim >> 8;
-            } else if (t == minT) {
-                tie = true;
-            }
-        }
-    }
-    if (tie) return trace_ordered(sc, o, d, time, wantNormal);
-    pending = wait;
-    Hit h;
-    h.t = minT;
-    h.prim = closest;
-    V3 nrm = v3s(0.0f);
-    if (wantNormal && closest >= 0) {
-        rec[ri].t = minT;
-        nrm = prim_normal(sc, sc.prims[closest], o, d, time, rec[ri]);
     }
     h.n = face_forward(nrm, -d);
     return h;

@@ -44,8 +44,8 @@
 //   wf2_lq    the same state with LANE-OWNED slots and bit-set queues (see wf2_push) -- scenes held on chip
 //             under the free-running scheduler: no bank conflicts, cheap queue operations, no FIFO order
 //   wf2_l2    2048 slots per CTA, the cold half of the state in global memory (L2), ring queues -- scenes with
-//             deep mesh BVHs (768-thread CTAs, and the offload mode), which gain from more paths in flight
-//             and from the rings' FIFO order (rays pushed together are traced together)
+//             deep mesh BVHs (768-thread CTAs), which gain from more paths in flight and from the rings' FIFO
+//             order (rays pushed together are traced together)
 // so it has no include guard, and only defines macros whose text is the same every time.
 
 #ifndef TB_WF2_THREADS
@@ -57,7 +57,7 @@
 #ifndef TB_WF2_CTAS_PER_SM
 #define TB_WF2_CTAS_PER_SM 1
 #endif
-static_assert(TB_WF2_PATHS <= TB_WF2_SLOTS, "the host sizes the cold slot state and the offload queues with TB_WF2_SLOTS");
+static_assert(TB_WF2_PATHS <= TB_WF2_SLOTS, "the host sizes the cold slot state with TB_WF2_SLOTS");
 #define TB_WF2_MAX_PRIMS 40     // scene tables up to this size are staged in shared memory (the flat program: up to 16 primitives)
 #define TB_WF2_MAX_PAIRS 40
 
@@ -130,11 +130,6 @@ struct Wf2Shared {
     int pref;                         // stage the warps currently prefer (soft phases, see the main loop)
     int live;                         // slots that still hold (or may still receive) a path
     int exhausted;
-    // offload mode: heads of this CTA's two answer rings (extension / shadow), answers still owed to it,
-    // and whether the CTA has told the walkers that it is done
-    unsigned int ansHead[2];
-    int ansPending[2];
-    int exitSignaled;
     // the scene descriptor every stage reads, pointing at the staged tables below: one copy per CTA, filled by
     // thread 0 in the prologue.  A per-thread copy would live in local memory (the stages take it by reference),
     // where every field read is a dependent L1 / L2 round trip at the head of a stage.
@@ -146,13 +141,8 @@ struct Wf2Shared {
     alignas(8) unsigned long long stageBar;
 };
 
-// dynamic shared memory of a CTA: the slot arrays; a build with fewer slots (experiments) still claims
-// a whole SM, so that the slot count per SM is what changes
-#ifdef TB_WF2_PAD_SMEM
-#define TB_WF2_SMEM_BYTES (sizeof(Wf2Shared) > 204000 ? sizeof(Wf2Shared) : (size_t)204000)
-#else
+// dynamic shared memory of a CTA: the slot arrays
 #define TB_WF2_SMEM_BYTES sizeof(Wf2Shared)
-#endif
 
 // stage queues.  T, A, B, R in the cyclic order of the free-running sweep; F0/F1 hold the freshly
 // regenerated camera rays in hard-phase mode (double-buffered: R fills one while T drains the other)
@@ -469,95 +459,6 @@ TB_DEV bool wf2_scatter(Wf2Shared& S, float4* rec, const DScene& sc, int s, cons
     return true;
 }
 
-#include "wavefront_walk.cuh"
-
-// Claim up to 32 answers of the walkers for this CTA (offload mode): lane i < n receives the three
-// chunks of its answer.  Cells are validated by their lap tags, ownership is taken with a CAS on the
-// ring's head in shared memory (only this CTA's warps consume the ring).
-TB_DEV int wf2_claim_answers(Wf2Shared& S, const WalkParams& W, int kind, int minCount, uint4& c0, uint4& c1, uint4& c2)
-{
-    const int lane = threadIdx.x & 31;
-    unsigned int h = 0;
-    int owed = 0;
-    if (lane == 0) {
-        owed = *(volatile int*)&S.ansPending[kind];
-        h = *(volatile unsigned int*)&S.ansHead[kind];
-    }
-    owed = __shfl_sync(0xffffffffu, owed, 0);
-    if (owed < minCount) return 0;   // nothing (or not enough) can have arrived: skip the round trip to L2
-    h = __shfl_sync(0xffffffffu, h, 0);
-    const unsigned int idx = h + (unsigned)lane;
-    const unsigned int tag = (idx >> WF2_LOG2_PATHS) + 1u;
-    const uint4* cell = W.ansRing + ((size_t)(blockIdx.x * 2 + kind) * TB_WF2_PATHS + (idx & WF2_MASK)) * 3;
-    c0 = walk_ld(cell + 0);
-    c1 = walk_ld(cell + 1);
-    c2 = walk_ld(cell + 2);
-    const bool ok = c0.w == tag && c1.w == tag && c2.w == tag;
-    const unsigned good = __ballot_sync(0xffffffffu, ok);
-    const int n = (good == 0xffffffffu) ? 32 : __ffs(~good) - 1;
-    if (n <= 0 || n < minCount) return 0;
-    unsigned int got = 0;
-    if (lane == 0) got = atomicCAS(&S.ansHead[kind], h, h + (unsigned)n);
-    got = __shfl_sync(0xffffffffu, got, 0);
-    if (got != h) return 0;   // another warp of the CTA took them
-    if (lane == 0) atomicSub(&S.ansPending[kind], n);
-    return n;
-}
-
-#ifndef TB_WF2_LANEQ
-// Fold a walker's answer into the partial hit stage T left in the slot (offload mode).  Afterwards
-// the slot holds exactly what trace_closest() would have produced for the pending ray.
-TB_DEV void wf2_merge_answer(Wf2Shared& S, const DScene& sc, int s, bool isExt, uint4 c0, uint4 c1, uint4 c2)
-{
-    const uint32_t info = c2.z;
-    const bool hit = ((info >> (WF2_SLOT_BITS + 8)) & 1u) != 0u, tie = ((info >> (WF2_SLOT_BITS + 9)) & 1u) != 0u;
-    const int primM = (int)((info >> WF2_SLOT_BITS) & 0xffu);
-    const float tM = __uint_as_float(c0.x);
-    const float partialT = isExt ? S.ht[s] : S.st[s];
-    const int partialPrim = isExt ? S.hprim[s] : S.sprim[s];
-    V3 o = v3(S.ox[s], S.oy[s], S.oz[s]);
-    V3 d = v3(S.dx[s], S.dy[s], S.dz[s]);
-    const float time = S.time[s];
-    if (!isExt) {
-        // the shadow ray, as stage T built it (render.cpp:121,170)
-        const V3 p = o + d * S.ht[s];
-        const V3 nn = v3(S.hnx[s], S.hny[s], S.hnz[s]);
-        d = v3(S.sdx[s], S.sdy[s], S.sdz[s]);
-        o = p + face_forward(nn, d) * TB_RAY_EPS;
-    }
-    if (tie || (hit && partialPrim >= 0 && tM == partialT)) {
-        // two primitives at exactly the same t: the reference's visit order decides -- redo in that order
-        const Hit h = trace_ordered(sc, o, d, time, isExt);
-        if (isExt) {
-            S.ht[s] = h.t;
-            S.hnx[s] = h.n.x; S.hny[s] = h.n.y; S.hnz[s] = h.n.z;
-            S.hprim[s] = h.prim;
-        } else {
-            S.st[s] = h.t;
-            S.sprim[s] = h.prim;
-        }
-        return;
-    }
-    if (!hit || !(tM < partialT)) return;   // the partial hit stands
-    if (isExt) {
-        PrimHit ph;
-        ph.t = tM;
-        ph.u = __uint_as_float(c0.y);
-        ph.v = __uint_as_float(c0.z);
-        ph.w = __uint_as_float(c1.x);
-        ph.gn = v3(__uint_as_float(c1.y), __uint_as_float(c1.z), __uint_as_float(c2.x));
-        ph.tri = (int)c2.y;
-        const V3 n = face_forward(prim_normal(sc, sc.prims[primM], o, d, time, ph), -d);
-        S.ht[s] = tM;
-        S.hnx[s] = n.x; S.hny[s] = n.y; S.hnz[s] = n.z;
-        S.hprim[s] = primM;
-    } else {
-        S.st[s] = tM;
-        S.sprim[s] = primM;
-    }
-}
-#endif
-
 // THREADS: 512 (16 warps, up to 128 registers) for scenes held in shared memory, where more warps
 // only add instruction-cache pressure; 768 (24 warps, 80 registers) for scenes with deep mesh BVHs,
 // whose traversal is latency bound on L2 and pays for the extra warps (LaunchParams::wideCta).
@@ -568,8 +469,7 @@ TB_DEV void wf2_merge_answer(Wf2Shared& S, const DScene& sc, int s, bool isExt, 
 //                     its own specialisation measured slower on cornell)
 //   WF2_MODE_HARD     hard phases only (faster on veach)
 //   WF2_MODE_SPLIT    free-running with the split trace queue TM (scenes with a big mesh)
-//   WF2_MODE_OFFLOAD  free-running shader CTAs + walker CTAs that do the big meshes' BVH walks (wavefront_walk.cuh)
-enum { WF2_MODE_GENERIC = 0, WF2_MODE_HARD = 1, WF2_MODE_SPLIT = 2, WF2_MODE_OFFLOAD = 3 };
+enum { WF2_MODE_GENERIC = 0, WF2_MODE_HARD = 1, WF2_MODE_SPLIT = 2 };
 
 #if defined(TB_WF2_STAGE_CLOCKS) && defined(TB_WF2_LANEQ)
 // Per-stage cycle accounting of the lane-owned layout (development builds with -DTB_WF2_STAGE_CLOCKS, read by
@@ -625,6 +525,17 @@ void wf2_stage_clocks(unsigned long long* out, bool reset)
 }
 #endif
 
+TB_DEV uint32_t wf2_smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// a generic address the compiler cannot trace back to shared memory: loads through it are generic loads
+// (LD), so one instruction serves lanes that read the staged treelet and lanes that read global memory
+TB_DEV const unsigned char* wf2_opaque(const void* p)
+{
+    unsigned long long a = (unsigned long long)p;
+    asm volatile("" : "+l"(a));
+    return reinterpret_cast<const unsigned char*>(a);
+}
+
 // FEAT: the scene features (TB_FEAT_*) compiled in.  The lane-owned layout has a second instantiation without any
 // of them, for scenes that have none (wf2_lq::launch_layout); every other instantiation has them all.
 template <int THREADS, int MODE, uint32_t FEAT = TB_FEAT_ALL>
@@ -633,22 +544,16 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
     extern __shared__ __align__(16) unsigned char wf_smem_raw[];
     Wf2Shared& S = *reinterpret_cast<Wf2Shared*>(wf_smem_raw);
     const int tid = threadIdx.x;
-    constexpr bool offload = MODE == WF2_MODE_OFFLOAD;
-    if (offload && (int)blockIdx.x >= P.walk.numShaders) {
-        wf2_walker_role<THREADS>(P, wf_smem_raw, (int)TB_WF2_SMEM_BYTES);
-        return;
-    }
 
     // ---- prologue: stage the scene tables on chip ---------------------------------------------
     // Primitive records, the scene-level BVH (child-pair records) and the flat scene program go from
     // global to shared memory as TMA bulk copies (cp.async.bulk -> UBLKCP): thread 0 arms an mbarrier
-    // with the byte count and issues up to three copies, everybody waits on the barrier's phase.  (The
-    // walker CTAs of the offload mode stage the top of the big mesh's BVH the same way.)
+    // with the byte count and issues up to three copies, everybody waits on the barrier's phase.
     const bool stagePrims = P.scene.numPrims <= TB_WF2_MAX_PRIMS;
     const bool stagePairs = P.scene.numPairs > 0 && P.scene.numPairs <= TB_WF2_MAX_PAIRS;
     const bool stageFlat = P.scene.numFlat > 0 && P.scene.numFlat <= 32;
     if (tid == 0) {
-        const uint32_t bar = walk_smem_addr(&S.stageBar);
+        const uint32_t bar = wf2_smem_addr(&S.stageBar);
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         // device arrays are padded by one element (api.cu: upload_image), so rounding up stays inside them
@@ -663,21 +568,21 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
             const unsigned char* src = reinterpret_cast<const unsigned char*>(P.scene.meshes[P.scene.treeletMesh].pairs);
             for (uint32_t off = 0; off < treeBytes; off += 32768u) {
                 const uint32_t n = min(32768u, treeBytes - off);
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(walk_smem_addr(tl + off)),
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(wf2_smem_addr(tl + off)),
                              "l"(src + off), "r"(n), "r"(bar)
                              : "memory");
             }
         }
         if (primBytes)
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(walk_smem_addr(S.prims)),
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(wf2_smem_addr(S.prims)),
                          "l"(P.scene.prims), "r"(primBytes), "r"(bar)
                          : "memory");
         if (pairBytes)
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(walk_smem_addr(S.pairs)),
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(wf2_smem_addr(S.pairs)),
                          "l"(P.scene.pairs), "r"(pairBytes), "r"(bar)
                          : "memory");
         if (flatBytes)
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(walk_smem_addr(S.flat)),
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(wf2_smem_addr(S.flat)),
                          "l"(P.scene.flat), "r"(flatBytes), "r"(bar)
                          : "memory");
         // the CTA's scene descriptor (Wf2Shared::scene), published by the barrier below
@@ -692,7 +597,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
         if (P.treeletBytes >= (int)sizeof(BvhPair) && d.treeletMesh >= 0) {
             unsigned char* tl = wf_smem_raw + ((sizeof(Wf2Shared) + 127) & ~size_t(127));
             d.treeletPairs = min(d.treeletPairs, P.treeletBytes / (int)sizeof(BvhPair));
-            d.treelet = walk_opaque(tl);
+            d.treelet = wf2_opaque(tl);
         } else {
             d.treeletPairs = 0;
         }
@@ -735,13 +640,6 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
         S.pref = WF2_Q_R;
         S.live = TB_WF2_PATHS;
         S.exhausted = 0;
-        S.ansPending[0] = S.ansPending[1] = 0;
-        S.exitSignaled = 0;
-        if (offload) {
-            // everything the walkers ever answered has been consumed: the rings' heads are their tails
-            S.ansHead[0] = walk_ld1(P.walk.ansTail + blockIdx.x * 2 + 0);
-            S.ansHead[1] = walk_ld1(P.walk.ansTail + blockIdx.x * 2 + 1);
-        }
     }
     __syncthreads();   // the barrier word and S.scene are initialised (thread 0, above) before anybody reads them
     {
@@ -749,7 +647,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
         while (!landed)
             asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
                          : "=r"(landed)
-                         : "r"(walk_smem_addr(&S.stageBar)), "r"(0u)
+                         : "r"(wf2_smem_addr(&S.stageBar)), "r"(0u)
                          : "memory");
     }
 
@@ -759,11 +657,6 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
     float4* const coldBase = S.cold;
 #else
     float4* const coldBase = P.cold + (size_t)blockIdx.x * TB_WF2_PATHS * CC_CHUNKS;
-#endif
-#ifdef WALK_SHADER_WARPS
-    // offload mode: with most slots parked at the walkers, fewer warps per shader CTA keep fuller chunks and
-    // fewer distinct stages in flight (experiment knob)
-    if (offload && (tid >> 5) >= WALK_SHADER_WARPS) return;
 #endif
 
     // Two scheduling modes share the stage code below (P.hardPhases, uniform for the launch):
@@ -807,7 +700,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
         clk.claim += t1 - t0;
 #endif
 #else
-    const bool hard = MODE == WF2_MODE_HARD ? true : (MODE == WF2_MODE_SPLIT || offload) ? false : (P.hardPhases != 0);
+    const bool hard = MODE == WF2_MODE_HARD ? true : MODE == WF2_MODE_SPLIT ? false : (P.hardPhases != 0);
     constexpr bool split = MODE == WF2_MODE_SPLIT;
     // hard-phase schedule: each cycle is two block-synchronous phases,
     //   phase 0:  R (finished slots -> fresh camera rays into F[cycle&1]),  T,  F[~cycle&1]
@@ -819,11 +712,8 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
     unsigned int stepTail = TB_WF2_PATHS;   // every slot starts in the R queue
     int stepQueue = WF2_Q_R;
 
-    unsigned int idleSpins = 0;
     for (;;) {
         int s = 0, n = 0, stage = -1;
-        bool fromAnswer = false;      // offload mode: the chunk are walkers' answers, merged at the head of stage A / B
-        uint4 ans0 = make_uint4(0u, 0u, 0u, 0u), ans1 = ans0, ans2 = ans0;
         if (hard) {
             n = wf2_claim_ticket(S, stepQueue, stepTail, s);
             if (n > 0) {
@@ -870,32 +760,9 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
             // Once the sample counter has run dry the CTA is draining: nothing refills the queues any more, so
             // waiting for full 32-entry chunks only adds latency -- take whatever is there.  (A 1-spp Render() on
             // one of N GPUs is ALL drain: a single partial fill of the slot arrays.)
-#ifdef TB_WF2_NO_DRAIN
-            const int full = 32;
-#else
             const int full = (p >> 8) ? 1 : 32;
-#endif
             p &= 0xff;
-            if (offload) {
-                // sweep over six sources: T, answers(ext), A, answers(shadow), B, R
-                for (int k = 0; k < WALK_SWEEP_PASSES * 6 && stage < 0; ++k) {
-                    const int pos = (p + k) % 6;
-                    const int minCount = k < 6 ? full : (k < 12 ? WALK_PARTIAL_MIN : 1);
-                    if (pos == 1 || pos == 3) {
-                        n = wf2_claim_answers(S, P.walk, pos == 1 ? WALK_KIND_EXT : WALK_KIND_SHADOW, minCount, ans0, ans1, ans2);
-                        if (n > 0) {
-                            stage = pos == 1 ? WF2_Q_A : WF2_Q_B;
-                            fromAnswer = true;
-                            s = (int)(ans2.z & WF2_SLOT_MASK);
-                        }
-                    } else {
-                        const int q = pos == 0 ? WF2_Q_T : pos == 2 ? WF2_Q_A : pos == 4 ? WF2_Q_B : WF2_Q_R;
-                        n = wf2_claim(S, q, minCount, s);
-                        if (n > 0) stage = q;
-                    }
-                    if (n > 0 && pos != p && lane == 0) *(volatile int*)&S.pref = pos;
-                }
-            } else if (!split) {
+            if (!split) {
                 for (int k = 0; k < 8 && stage < 0; ++k) {
                     // k = 0..3: full chunks only; k = 4..7: whatever is left
                     const int q = (p + k) & 3;
@@ -914,25 +781,12 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                     }
                 }
             }
-            if (!split && !offload && stage >= 0 && stage != p && lane == 0) *(volatile int*)&S.pref = stage;
+            if (!split && stage >= 0 && stage != p && lane == 0) *(volatile int*)&S.pref = stage;
             if (stage < 0) {
                 if (*(volatile int*)&S.live <= 0) break;
-                if (offload) {
-                    // parked slots wait for the walkers: a watchdog instead of an endless spin if they never answer
-                    if ((++idleSpins & 255u) == 0u) {
-                        unsigned int bad = 0;
-                        if (lane == 0) bad = walk_ld1(P.walk.abortFlag);
-                        if (__shfl_sync(0xffffffffu, bad, 0)) break;
-                        if (idleSpins > WALK_WATCHDOG_SPINS) {
-                            if (lane == 0) atomicExch(P.walk.abortFlag, 1u);
-                            break;
-                        }
-                    }
-                }
                 __nanosleep(200);
                 continue;
             }
-            idleSpins = 0;
         }
         const bool active = lane < n;
 #endif
@@ -1026,9 +880,6 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
         } else if (stage == WF2_Q_T || stage >= WF2_Q_F0) {
             // ===================== T: trace the pending ray =======================================
             bool isExt = false, isNee = false;
-            uint32_t parkMask = 0u;       // offload mode: big meshes the ray still has to be walked through
-            V3 postO = v3s(0.0f), postD = v3s(0.0f);
-            float postTime = 0.0f;
             if (active) {
                 const uint32_t fl = S.flags[s];
                 V3 o = v3(S.ox[s], S.oy[s], S.oz[s]);
@@ -1045,12 +896,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                 }
                 if (isNee || maxDepth > 0) {
                     // one traversal instance serves both ray kinds (normals only for extension rays)
-                    const Hit h = offload ? trace_partial(sc, o, d, time, isExt, parkMask) : trace_closest(sc, o, d, time, isExt);
-                    if (offload) {
-                        postO = o;
-                        postD = d;
-                        postTime = time;
-                    }
+                    const Hit h = trace_closest(sc, o, d, time, isExt);
                     if (isExt) {
                         S.ht[s] = h.t;
                         S.hnx[s] = h.n.x; S.hny[s] = h.n.y; S.hnz[s] = h.n.z;
@@ -1064,28 +910,12 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                 }
             }
             __threadfence_block();
-            if (offload) {
-                // rays that reach a big mesh park in their slot; the walkers' answer re-enters at stage A / B
-                const bool park = parkMask != 0u;
-                const unsigned pe = __ballot_sync(0xffffffffu, park && isExt), pn = __ballot_sync(0xffffffffu, park && isNee);
-                if (lane == 0) {
-                    if (pe) atomicAdd(&S.ansPending[WALK_KIND_EXT], __popc(pe));
-                    if (pn) atomicAdd(&S.ansPending[WALK_KIND_SHADOW], __popc(pn));
-                }
-                walk_post(P.walk, park, postO, postD, postTime, parkMask,
-                          (uint32_t)s | ((isExt ? WALK_KIND_EXT : WALK_KIND_SHADOW) << WF2_SLOT_BITS) | ((uint32_t)blockIdx.x << (WF2_SLOT_BITS + 1)));
-                isExt = isExt && !park;
-                isNee = isNee && !park;
-            }
             wf2_push(S, WF2_Q_A, isExt, s);
             wf2_push(S, WF2_Q_B, isNee, s);
 #endif
         } else if (stage == WF2_Q_A) {
             // ===================== A: extension-ray results =======================================
             bool cont = false, fin = false;
-#ifndef TB_WF2_LANEQ
-            if (offload && fromAnswer && active) wf2_merge_answer(S, sc, s, true, ans0, ans1, ans2);
-#endif
             if (active) {
                 float4* rec = coldBase + (size_t)s * CC_CHUNKS;
                 const float4 ct = cold_ld(rec, CC_T), cl = cold_ld(rec, CC_L);
@@ -1177,7 +1007,6 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
         else {
             // ===================== B: shadow-ray results ==========================================
             bool cont = false, fin = false;
-            if (offload && fromAnswer && active) wf2_merge_answer(S, sc, s, false, ans0, ans1, ans2);
             if (active) {
                 float4* rec = coldBase + (size_t)s * CC_CHUNKS;
                 const float4 ct = cold_ld(rec, CC_T), cl = cold_ld(rec, CC_L), ca = cold_ld(rec, CC_A), cr = cold_ld(rec, CC_RNG);
@@ -1230,13 +1059,6 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
 #if defined(TB_WF2_STAGE_CLOCKS) && defined(TB_WF2_LANEQ)
     clk.flush();
 #endif
-    if (offload) {
-        // this CTA posts no more requests: tell the walkers (once)
-        if (lane == 0 && atomicExch(&S.exitSignaled, 1) == 0) {
-            __threadfence();
-            atomicAdd(P.walk.shadersDone, 1u);
-        }
-    }
 }
 
 // The opt-in to > 48 KB of dynamic shared memory and the occupancy answer are PER DEVICE (and the
@@ -1267,11 +1089,11 @@ template <int THREADS, int MODE, uint32_t FEAT = TB_FEAT_ALL>
 static void launch_wavefront2_t(const LaunchParams& p0, int numSMs, cudaStream_t stream, unsigned long long total)
 {
     const int ctasPerSM = wavefront2_ctas_per_sm<THREADS, MODE, FEAT>();
-    // shared memory beyond the slot arrays holds the treelet (the shader role; walker CTAs lay out their own)
+    // shared memory beyond the slot arrays holds the treelet
     LaunchParams p = p0;
     const size_t slotBytes = (TB_WF2_SMEM_BYTES + 127) & ~size_t(127);
     p.treeletBytes = 0;
-    if (p.scene.treeletMesh >= 0 && p.scene.treeletPairs > 0 && MODE != WF2_MODE_OFFLOAD && wavefront2_smem_limit() > slotBytes) {
+    if (p.scene.treeletMesh >= 0 && p.scene.treeletPairs > 0 && wavefront2_smem_limit() > slotBytes) {
         const size_t room = (wavefront2_smem_limit() - slotBytes) / sizeof(BvhPair) * sizeof(BvhPair);
         p.treeletBytes = (int)std::min(room, (size_t)p.scene.treeletPairs * sizeof(BvhPair));
     }
@@ -1279,17 +1101,6 @@ static void launch_wavefront2_t(const LaunchParams& p0, int numSMs, cudaStream_t
     // TB_WF2_CTAS_PER_SM resident CTAs per SM; small jobs use fewer so that every CTA has a full slot array
     const unsigned long long want = (total + TB_WF2_PATHS - 1) / TB_WF2_PATHS;
     int grid = (numSMs > 0 ? numSMs : 132) * ctasPerSM;
-    if (MODE == WF2_MODE_OFFLOAD) {
-        // shader CTAs [0, numShaders) + walker CTAs behind them, all resident at once (they wait for each other)
-        LaunchParams q = p;
-        int walkers = std::max(1, std::min(q.walk.numWalkers, grid - 1));
-        int shaders = grid - walkers;
-        if (want < (unsigned long long)shaders) shaders = (int)std::max<unsigned long long>(1ull, want);
-        q.walk.numShaders = shaders;
-        q.walk.numWalkers = walkers;
-        k_wavefront2<THREADS, MODE><<<shaders + walkers, THREADS, smemBytes, stream>>>(q, total);
-        return;
-    }
     if (want < (unsigned long long)grid) grid = (int)want;
     if (grid < 1) grid = 1;
     k_wavefront2<THREADS, MODE, FEAT><<<grid, THREADS, smemBytes, stream>>>(p, total);
@@ -1322,10 +1133,7 @@ const char* launch_layout(const LaunchParams& p, int numSMs, cudaStream_t stream
     else launch_wavefront2_t<TB_WF2_THREADS, WF2_MODE_GENERIC>(p, numSMs, stream, total);
     name = "wf2_smem";
 #else
-    if (wavefront2_wants_offload(p)) {
-        if (p.wideCta) launch_wavefront2_t<TB_WF2_THREADS_WIDE, WF2_MODE_OFFLOAD>(p, numSMs, stream, total);
-        else launch_wavefront2_t<TB_WF2_THREADS, WF2_MODE_OFFLOAD>(p, numSMs, stream, total);
-    } else if (split) {
+    if (split) {
         launch_wavefront2_t<TB_WF2_THREADS_WIDE, WF2_MODE_SPLIT>(p, numSMs, stream, total);
     } else {
         launch_wavefront2_t<TB_WF2_THREADS_WIDE, WF2_MODE_GENERIC>(p, numSMs, stream, total);   // hard phases too (run-time flag)

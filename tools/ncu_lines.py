@@ -142,7 +142,7 @@ def main():
     print("\nby line: %inst lanes %samples")
     for k, v in sorted(by_line.items(), key=lambda x: -x[1][2])[:30]:
         print("  %-34s %5.1f %5.1f %5.1f" % ("%s:%s" % k if k else "?", 100.0 * v[0] / tot[0], v[1] / max(1, v[0]), 100.0 * v[2] / max(1, tot[2])))
-    only = os.environ.get("NCU_LINES_FILE")   # e.g. wavefront_walk.cuh: every line of that file, in line order
+    only = os.environ.get("NCU_LINES_FILE")   # e.g. wavefront2.cuh: every line of that file, in line order
     if only:
         print("\nevery line of %s: %%inst lanes %%samples" % only)
         for k, v in sorted((kv for kv in by_line.items() if kv[0] and kv[0][0] == only), key=lambda x: x[0][1]):

@@ -17,9 +17,7 @@ run() {  # name, env..., scene w h spp
 SCENE="cornell 64 48 1 1";   run "free 512 (wf2_smem generic)" TINSEL_B200_SCHED=free TINSEL_B200_CTA=512
 SCENE="cornell 64 48 1 1";   run "lanes 512 (wf2_lq generic)" TINSEL_B200_SCHED=free TINSEL_B200_QUEUES=lanes TINSEL_B200_CTA=512
 SCENE="veach 64 48 1 1";     run "hard 512 (wf2_smem hard)" TINSEL_B200_SCHED=hard TINSEL_B200_CTA=512
-SCENE="meshlight 64 48 1 1"; run "split 512 (wf2_smem split)" TINSEL_B200_SCHED=free TINSEL_B200_SPLIT=1 TINSEL_B200_OFFLOAD=0 TINSEL_B200_CTA=512
-SCENE="meshlight 64 48 1 1"; run "free 768 (wf2_l2 generic)" TINSEL_B200_SCHED=free TINSEL_B200_SPLIT=0 TINSEL_B200_OFFLOAD=0 TINSEL_B200_CTA=768
+SCENE="meshlight 64 48 1 1"; run "split 512 (wf2_smem split)" TINSEL_B200_SCHED=free TINSEL_B200_SPLIT=1 TINSEL_B200_CTA=512
+SCENE="meshlight 64 48 1 1"; run "free 768 (wf2_l2 generic)" TINSEL_B200_SCHED=free TINSEL_B200_SPLIT=0 TINSEL_B200_CTA=768
 SCENE="veach 64 48 1 1";     run "hard 768 (wf2_l2 generic, hard flag)" TINSEL_B200_SCHED=hard TINSEL_B200_CTA=768
-SCENE="meshlight 64 48 1 1"; run "split 768 (wf2_l2 split)" TINSEL_B200_SCHED=free TINSEL_B200_SPLIT=1 TINSEL_B200_OFFLOAD=0 TINSEL_B200_CTA=768
-SCENE="meshlight 64 48 1 1"; run "offload 512 (wf2_l2 offload)" TINSEL_B200_OFFLOAD=1 TINSEL_B200_WALKERS=2 TINSEL_B200_CTA=512
-SCENE="meshlight 64 48 1 1"; run "offload 768 (wf2_l2 offload)" TINSEL_B200_OFFLOAD=1 TINSEL_B200_WALKERS=2 TINSEL_B200_CTA=768
+SCENE="meshlight 64 48 1 1"; run "split 768 (wf2_l2 split)" TINSEL_B200_SCHED=free TINSEL_B200_SPLIT=1 TINSEL_B200_CTA=768
