@@ -84,6 +84,12 @@ typedef struct tb200_bvh_node {
  * tb200_create_cached refuse a scene that breaks either rule; tb200_bvh_build never returns one. */
 #define TB200_MAX_BVH_LEVELS 31
 
+/* The most primitives a scene may have, and the most lightSamples one primitive may take: the wavefront
+ * kernel keeps a hit's next-event-estimation position (a primitive index, and a sample index within that
+ * light) in two 12-bit fields.  tb200_create, tb200_scene_cache_save and tb200_create_cached refuse more. */
+#define TB200_MAX_PRIMITIVES 4095
+#define TB200_MAX_LIGHT_SAMPLES 4095
+
 /* MeshGeometry (src/scene.h:121-139).  All pointers are borrowed host memory. */
 typedef struct tb200_mesh {
     const float* positions;      /* numVertices * 3 */

@@ -121,7 +121,7 @@ def _nodes(tree):
     return nodes
 
 
-def _save(rng, path, prims, tree, meshes, width, height, probe=None, camera=None):
+def _save(rng, path, prims, tree, meshes, width, height, probe=None, camera=None, max_depth=None):
     """Sky, camera and options drawn from `rng`, then the snapshot.  meshes: list of MeshData."""
     scene, keep = make_scene_struct(prims, tree, meshes)
     scene.sky.horizon[:] = [float(x) for x in rng.uniform(0.0, 1.0, 3)]
@@ -141,6 +141,8 @@ def _save(rng, path, prims, tree, meshes, width, height, probe=None, camera=None
         cam.position[:] = camera
     opt.width, opt.height = width, height
     opt.maxDepth = int(rng.randint(2, 6))
+    if max_depth is not None:
+        opt.maxDepth = max_depth
     opt.filterType, opt.filterWidth, opt.filterFalloff, opt.filterOffset = abi.FILTER_GAUSSIAN, 0.75, 1.0, 0.5697828531265259
     if tb.load_library().tb200_snapshot_save(str(path).encode(), C.byref(scene), C.byref(cam), C.byref(opt)) != 0:
         raise RuntimeError(tb.last_error())
@@ -478,4 +480,105 @@ def make_mesh_scene(seed, path, family, width=40, height=30, swap_ties=False, le
                 moving_scale=sum(1 for q in prims if q.type == abi.MESH and q.start.s != q.end.s),
                 mesh_lights=sum(1 for q in prims if q.type == abi.MESH and q.lightSamples > 0),
                 zero_area=sum(m.zero_area for m in meshes), probe=probe is not None)
+    return info
+
+
+# ---- the limits tb200_create accepts -------------------------------------------------------------
+
+MAX_PRIMS = 4095            # TB200_MAX_PRIMITIVES
+MAX_LIGHT_SAMPLES = 4095    # TB200_MAX_LIGHT_SAMPLES
+LIMIT_CASES = ("prims40", "prims41", "prims42", "prims600", "prims4095", "nee255", "nee256", "nee257", "nee300",
+               "nee300_odd", "probe255", "meshlight300")
+
+
+def _wall(p, rng):
+    """A plane at z = -3 behind everything: with the floor, every camera ray hits a surface."""
+    p.type = abi.PLANE
+    p.plane[:] = [0.0, 0.0, 1.0, 3.0]
+    _xf(p.start, (0, 0, 0), (0, 0, 0, 1), 1.0)
+    _xf(p.end, (0, 0, 0), (0, 0, 0, 1), 1.0)
+    p.mesh = -1
+    p.material = _material(rng, False)
+    p.material.transmission = 0.0
+    return (np.full(3, -1.0e8, np.float32), np.full(3, 1.0e8, np.float32))
+
+
+def nee_order(light_samples):
+    """(primitive, sample) of every shadow ray a surface hit draws, in order, after the probe sample if there is one."""
+    return [(i, k) for i, n in enumerate(light_samples) for k in range(n)]
+
+
+def make_limit_scene(case, path, width=48, height=32):
+    """Writes one of LIMIT_CASES to `path` and returns a dict describing what it holds.  Floor and back wall
+    first (every camera ray hits a surface, and every surface hit draws all numNee shadow rays), then:
+      prims40/41/42  spheres, about a quarter of them lights with 1-2 samples: 40 primitives stage their
+                     records and the 39 BVH pairs on chip, 41 stage the 40 pairs only, 42 neither
+      prims600       lights at even and odd indices with 1-12 samples each; the 256th shadow ray is a sample
+                     of a light at an even index that is not that light's last one
+      prims4095      the most primitives tb200_create accepts; the last one is a light with the most lightSamples
+                     it accepts
+      neeN           8 primitives, one sphere light with N samples at index 2
+      nee300_odd     the light at index 3
+      probe255       an HDR probe (no black rows) and a 255-sample light at index 3: 256 shadow rays per hit
+      meshlight300   an icosphere mesh light at index 2 with 300 samples"""
+    rng = np.random.RandomState(7919 * (LIMIT_CASES.index(case) + 1))
+    counts = {"prims40": 40, "prims41": 41, "prims42": 42, "prims600": 600, "prims4095": MAX_PRIMS}
+    n = counts.get(case, 8)
+    P = (abi.Primitive * n)()
+    bounds = [_floor(P[0], rng), _wall(P[1], rng)]
+    meshes, probe, max_depth = [], None, None
+    if case in counts:
+        r_lo, r_hi = {40: (0.15, 0.35), 41: (0.15, 0.35), 42: (0.15, 0.35), 600: (0.05, 0.14), MAX_PRIMS: (0.02, 0.05)}[n]
+        if case == "prims600":
+            while True:       # lights at random indices until the 256th shadow ray falls inside an even-index light
+                lights = set(int(i) for i in rng.choice(np.arange(2, n), 60, replace=False))
+                samples = [int(rng.randint(1, 13)) if i in lights else 0 for i in range(n)]
+                prim, k = nee_order(samples)[255]
+                if prim % 2 == 0 and k + 1 < samples[prim] and any(i % 2 for i in lights) and max(lights) > prim:
+                    break
+        elif case == "prims4095":
+            samples = [0] * n
+            samples[n - 1] = MAX_LIGHT_SAMPLES
+            max_depth = 2
+        else:
+            samples = [int(rng.randint(1, 3)) if rng.uniform() < 0.25 else 0 for i in range(n)]
+            samples[0] = samples[1] = 0
+            samples[2] = max(samples[2], 1)
+        for i in range(2, n):
+            light = samples[i] > 0
+            if case == "prims4095" and light:
+                bounds.append(_sphere(P[i], (0.0, 3.2, 1.0), 0.3, _material(rng, True), samples[i]))
+                continue
+            pos = rng.uniform(-2.8, 2.8, 3) * (1, 0.4, 1) + (0, 2.5 if light else 1.0, -0.2)
+            bounds.append(_sphere(P[i], pos, rng.uniform(r_lo, r_hi), _material(rng, light), samples[i]))
+    else:
+        spp = int("".join(ch for ch in case if ch.isdigit()))
+        at = 3 if case in ("nee300_odd", "probe255") else 2
+        samples = [0] * n
+        samples[at] = spp
+        if case == "meshlight300":
+            p, nrm, f = _icosphere(2)
+            meshes.append(MeshData(p, nrm, f))
+        for i in range(2, n):
+            if i == at and meshes:
+                P[i].material = _material(rng, True)
+                P[i].lightSamples = spp
+                bounds.append(_instance(P[i], 0, meshes[0], (0.3, 2.6, 0.5), _quat(rng), 0.35))
+            elif i == at:
+                bounds.append(_sphere(P[i], (0.3, 2.6, 0.5), 0.3, _material(rng, True), spp))
+            else:
+                pos = rng.uniform(-1.8, 1.8, 3) * (1, 0.3, 1) + (0, 0.8, 0)
+                bounds.append(_sphere(P[i], pos, rng.uniform(0.25, 0.5), _material(rng, False)))
+        if case == "probe255":
+            probe = _probe(rng)
+            probe[..., :3] = np.maximum(probe[..., :3], np.float32(0.05))     # black rows would give NaN samples
+    opt = _save(rng, path, P, _build_bvh(bounds), meshes, width, height, probe=probe, max_depth=max_depth)
+    samples = [int(q.lightSamples) for q in P]
+    lights = [i for i, s in enumerate(samples) if s > 0]
+    order = [(-1, 0)] * int(probe is not None) + nee_order(samples)      # (-1, 0): the probe sample
+    info = {"case": case, "prims": n, "meshes": len(meshes), "tris": [len(m.idx) for m in meshes], "probe": probe is not None,
+            "lights": lights, "light_samples": {i: samples[i] for i in lights}, "maxDepth": opt.maxDepth,
+            "numNee": len(order), "lightBegin": lights[0], "lightEnd": lights[-1] + 1}
+    if len(order) >= 256:
+        info["ray256"] = order[255]       # (primitive, sample) of the 256th shadow ray
     return info

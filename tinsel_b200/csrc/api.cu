@@ -805,7 +805,7 @@ int pair_levels(const std::vector<BvhPair>& pairs, uint32_t root)
 bool validate_image(const SceneImage& img, std::string* why)
 {
     const size_t np = img.prims.size();
-    if (np == 0 || np > 4095) return *why = "bad primitive count", false;
+    if (np == 0 || np > TB200_MAX_PRIMITIVES) return *why = "bad primitive count", false;
     auto ref_ok = [](uint32_t ref, size_t pairs, size_t items) { return (ref & TB_LEAF) ? (ref & ~TB_LEAF) < items : ref < pairs; };
     if (!ref_ok(img.sceneRoot, img.scenePairs.size(), np)) return *why = "scene root reference out of range", false;
     for (const BvhPair& p : img.scenePairs)
@@ -828,7 +828,7 @@ bool validate_image(const SceneImage& img, std::string* why)
     for (const DPrim& p : img.prims) {
         if (p.type != TB200_SPHERE && p.type != TB200_PLANE && p.type != TB200_MESH) return *why = "unknown primitive type", false;
         if (p.type == TB200_MESH && (p.mesh < 0 || (size_t)p.mesh >= img.meshes.size())) return *why = "primitive references a missing mesh", false;
-        if (p.lightSamples < 0 || p.lightSamples > 4095) return *why = "lightSamples out of range", false;
+        if (p.lightSamples < 0 || p.lightSamples > TB200_MAX_LIGHT_SAMPLES) return *why = "lightSamples out of range", false;
     }
     for (const ProgOp& op : img.flat)
         if ((size_t)(op.kindPrim >> 8) >= np && (op.kindPrim & 0xff) != TB_OP_BOX) return *why = "scene program references a missing primitive", false;
@@ -1185,7 +1185,8 @@ static bool validate_bvh(const tb200_bvh_node* nodes, int numNodes, int numItems
 static bool validate_scene(const tb200_scene* s, std::string* why)
 {
     if (s->numPrimitives <= 0 || !s->primitives) return *why = "scene has no primitives", false;
-    if (s->numPrimitives > 4095) return *why = "more than 4095 primitives (the wavefront's NEE cursor holds 12-bit primitive indices)", false;
+    if (s->numPrimitives > TB200_MAX_PRIMITIVES)
+        return *why = "more than " + std::to_string(TB200_MAX_PRIMITIVES) + " primitives (the wavefront's NEE cursor holds 12-bit primitive indices)", false;
     if (s->numMeshes < 0 || (s->numMeshes > 0 && !s->meshes)) return *why = "bad mesh array", false;
     if (!validate_bvh(s->bvhNodes, s->numBvhNodes, s->numPrimitives, "scene", why)) return false;
     for (int m = 0; m < s->numMeshes; ++m) {
@@ -1205,7 +1206,8 @@ static bool validate_scene(const tb200_scene* s, std::string* why)
             return *why = "primitive " + std::to_string(i) + ": mesh index out of range", false;
         if (p.type == TB200_MESH && p.lightSamples > 0 && !s->meshes[p.mesh].cdf)
             return *why = "primitive " + std::to_string(i) + ": mesh light without a sampling CDF", false;
-        if (p.lightSamples < 0 || p.lightSamples > 4095) return *why = "primitive " + std::to_string(i) + ": lightSamples out of range", false;
+        if (p.lightSamples < 0 || p.lightSamples > TB200_MAX_LIGHT_SAMPLES)
+            return *why = "primitive " + std::to_string(i) + ": lightSamples out of range", false;
     }
     if (s->sky.probeValid) {
         const tb200_sky& k = s->sky;

@@ -483,7 +483,7 @@ TB_DEV void path_hit(const DScene& sc, PathState& ps, const Hit& h, int bounce, 
 // (if the sky has a probe), then for every primitive with lightSamples>0, in scene order, one
 // slot per sample (render.cpp:107-224).  nee_slot_light() maps a slot to its primitive.
 struct NeeCursor {
-    int slot;        // next slot
+    int slot;        // next slot (only compared with 0: the ring wavefront stores it as one bit)
     int prim;        // primitive scan position
     int sample;      // sample index within the current light
     V3 sum;          // running `sum`

@@ -70,6 +70,9 @@ enum { WF2_PH_EXT = 0, WF2_PH_NEE = 1 };
 //   0: T.xyz, eta        1: L.xyz, bsdfPdf     2: absorption.xyz, sample index
 //   3: rng1, rng2, NEE cursor, sampled light   4: shadow dist, light normal.xyz
 //   5: sky pdf, NEE sum.xyz                     6: NEE radiance accumulator.xyz
+// The NEE cursor word (wf2_store_shadow): bit 0 "a shadow ray has been drawn at this hit" (NeeCursor::slot is only
+// ever compared with 0, and a hit draws up to 1 + 4095 * 4095 of them), the primitive scan position in bits
+// 8..19, the sample index within that light in bits 20..31.
 // TB_WF2_COLD_SMEM: the same records in SHARED memory instead (stride 7 chunks), for builds with few enough
 // slots per CTA: the cold half then costs 7 128-bit accesses per stage instead of 27 32-bit ones.
 // TB_WF2_LANEQ: no shadow ray ever waits in a slot (stage A traces them in place), so only chunks 0-3 exist
@@ -411,11 +414,15 @@ static __device__ __noinline__ void wf2_band_pad(unsigned int* bandCount, volati
 }
 
 #ifndef TB_WF2_LANEQ
+// The stored primitive position runs up to numPrims (past the last light, after the probe sample of a scene
+// without lights), the stored sample index up to lightSamples - 1: both fit the cursor's 12-bit fields.
+static_assert(TB200_MAX_PRIMITIVES <= 0xfff && TB200_MAX_LIGHT_SAMPLES <= 0xfff, "the NEE cursor holds 12-bit primitive and sample indices");
+
 // the pending shadow ray and the NEE bookkeeping that waits for its result
 TB_DEV void wf2_store_shadow(Wf2Shared& S, float4* rec, int s, const ShadowRay& sr, const NeeCursor& c, Rng rng)
 {
     S.sdx[s] = sr.d.x; S.sdy[s] = sr.d.y; S.sdz[s] = sr.d.z;
-    const uint32_t cursor = (uint32_t)c.slot | ((uint32_t)c.prim << 8) | ((uint32_t)c.sample << 20);
+    const uint32_t cursor = (c.slot != 0 ? 1u : 0u) | ((uint32_t)c.prim << 8) | ((uint32_t)c.sample << 20);
     cold_st(rec, CC_RNG, u2f(rng.s1), u2f(rng.s2), u2f(cursor), __int_as_float(sr.light));
     cold_st(rec, CC_SH, sr.dist, sr.lightN.x, sr.lightN.y, sr.lightN.z);
     cold_st(rec, CC_SUM, sr.skyPdf, c.sum.x, c.sum.y, c.sum.z);
@@ -1023,7 +1030,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                 sr.light = __float_as_int(cr.w);
                 NeeCursor c;
                 const uint32_t cw = f2u(cr.z);
-                c.slot = (int)(cw & 0xffu);
+                c.slot = (int)(cw & 1u);
                 c.prim = (int)((cw >> 8) & 0xfffu);
                 c.sample = (int)(cw >> 20);
                 c.sum = v3(csum.y, csum.z, csum.w);
