@@ -1,4 +1,4 @@
-"""The lane-owned wavefront kernel has two instantiations (wavefront2.cuh, wf2_lq::launch_layout): one with every
+"""The lane-owned wavefront kernel has two instantiations (wf2_lanes.cuh; kernels.cu: launch_wavefront2): one with every
 scene feature (probe, motion, transmission, subsurface, clearcoat, absorption) and one compiled without them, which
 scenes that have none of them run (api.cu: scene_features).  Routing to the right one, and the same bits from both."""
 import ctypes as C

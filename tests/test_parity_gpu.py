@@ -342,7 +342,7 @@ def test_rotated_camera_and_fov():
 ])
 def test_streamed_readback_delivers_final_rows(case):
     """tb200_render copies finished pixel rows to the host while the kernel is still running
-    (api.cu render_streamed / wavefront2.cuh wf2_band_report).  Whatever the timing, the host
+    (api.cu render_streamed / wf2_common.cuh wf2_band_report).  Whatever the timing, the host
     buffer must equal the device accumulator bit for bit after every call, and must equal what
     the plain launch-then-copy path delivers up to the accumulation order."""
     name, size, shards, boxw = case

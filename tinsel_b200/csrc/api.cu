@@ -307,7 +307,7 @@ struct tb200_renderer {
     float* dRadiance = nullptr;   // tb200_trace_frame scratch
     float* dRaster = nullptr;
     unsigned long long* dCounter = nullptr;
-    float4* dCold = nullptr;      // cold half of the wavefront's slot state (wavefront2.cuh): 128 B per slot
+    float4* dCold = nullptr;      // cold half of the wavefront's slot state (wf2_common.cuh): 128 B per slot
     int frame = 0;
 
     // display/finish step (tb200_finish)
@@ -344,9 +344,9 @@ struct tb200_renderer {
     bool peerAccess = false;
 
     int pipeline = 2;             // 0 = mega (validation), 2 = wavefront (product)
-    int hardPhases = 1;           // wavefront scheduling mode (see wavefront2.cuh)
-    int wideCta = 0;              // 768-thread CTAs for deep mesh BVHs (see wavefront2.cuh)
-    int laneQueues = 0;           // lane-owned slots + bit-set queues (see wavefront2.cuh)
+    int hardPhases = 1;           // wavefront scheduling mode (see wf2_rings.cuh)
+    int wideCta = 0;              // 768-thread CTAs for deep mesh BVHs (see wf2_common.cuh)
+    int laneQueues = 0;           // lane-owned slots + bit-set queues (see wf2_lanes.cuh)
     uint32_t features = TB_FEAT_ALL;   // the scene's TB_FEAT_* features (scene_features)
     int specialize = 1;           // scenes without any feature run the specialised lane-owned kernel (TINSEL_B200_SPECIALIZE=0: never)
     const char* lastKernel = "";  // the kernel the last path-tracing launch ran (tb200_last_kernel)
@@ -548,7 +548,7 @@ bool image_from_scene(const tb200_scene* s, SceneImage* img)
 }
 
 // The scene's features (tb_scene.cuh: TB_FEAT_*).  A scene without any of them runs the lane-owned kernel compiled
-// without them (wavefront2.cuh: wf2_lq::launch_layout); a NaN parameter counts as present.
+// without them (kernels.cu: launch_wavefront2); a NaN parameter counts as present.
 uint32_t scene_features(const SceneImage& img)
 {
     uint32_t f = img.probeValid ? TB_FEAT_PROBE : TB_FEAT_NONE;
@@ -985,7 +985,7 @@ bool read_back(tb200_renderer* r, float* output)
 
 // One frame of the wavefront kernel with the read-back streamed underneath it: samples are handed
 // out in tile-row order, the kernel flags each band of tile rows as its last sample retires
-// (wavefront2.cuh, wf2_band_report), and this thread copies every owned pixel row that no
+// (wf2_common.cuh, wf2_band_report), and this thread copies every owned pixel row that no
 // unfinished sample can still touch while the kernel is tracing the rest.  What is left when the
 // kernel ends is the last band or two instead of the whole slab.
 bool render_streamed(tb200_renderer* r, LaunchParams& P, float* output, bool recordStart = true)
@@ -2004,7 +2004,7 @@ int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, 
 
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds only (-DTB_WF2_STAGE_CLOCKS, tools/stage_clocks.py): copies the lane-owned wavefront
-// layout's per-stage cycle counters of the current device into out[0..n) (n >= 15 words, see wavefront2.cuh:
+// layout's per-stage cycle counters of the current device into out[0..n) (n >= 15 words, see wf2_lanes.cuh:
 // Wf2Clocks) after the work queued so far has finished, and zeroes them when `reset` is set
 int tb200_stage_clocks(unsigned long long* out, int n, int reset)
 {

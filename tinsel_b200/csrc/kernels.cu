@@ -152,7 +152,7 @@ void launch_normals(const LaunchParams& p, cudaStream_t stream, unsigned long lo
 }
 
 // ------------------------------------------------------------------------------------------------
-// Wavefront pipeline: see wavefront2.cuh
+// Wavefront pipeline: see wf2_common.cuh and launch_wavefront2 below
 // ------------------------------------------------------------------------------------------------
 // ------------------------------------------------------------------------------------------------
 // Display/finish step: exposure / weight normalisation, filmic tone map, sRGB, 8-bit with the PNG
@@ -302,34 +302,35 @@ static size_t wavefront2_smem_limit()
     return (size_t)v;
 }
 
-// Three layouts of the wavefront's slot state and queues, one compilation of wavefront2.cuh each:
-//  * wf2_smem: 1024 slots per CTA, hot + cold state in shared memory.  Scenes held on chip (cornell, veach):
-//    they are issue-bound, and fetching the cold half from L2 slows them down.
-//  * wf2_l2: 2048 slots per CTA, the cold half (27 of 45 words) in a 128-byte record per slot in global
+// Three layouts of the wavefront's slot state and queues, each in its own namespace (see wf2_common.cuh):
+//  * wf2_smem: the ring-queue kernel with 1024 slots per CTA, hot + cold state in shared memory.  Scenes held on
+//    chip (cornell, veach): they are issue-bound, and fetching the cold half from L2 slows them down.
+//  * wf2_l2: the ring-queue kernel with 2048 slots per CTA, the cold half in a 128-byte record per slot in global
 //    memory, L2-resident.  Scenes with deep mesh BVHs (ajax, env): their rays take long, and twice the
 //    paths in flight hide it.
-//  * wf2_lq: wf2_smem's state with LANE-OWNED slots and bit-set stage queues instead of rings, free-running
-//    scheduler only: no shared-memory bank conflicts and far cheaper queue operations, at the price of the
-//    rings' FIFO order (scenes held on chip do not care; deep BVHs such as ajax do).
+//  * wf2_lq: the lane-owned kernel, 1024 slots per CTA in shared memory with LANE-OWNED slots and bit-set stage
+//    queues instead of rings, free-running scheduler only: no shared-memory bank conflicts and far cheaper queue
+//    operations, at the price of the rings' FIFO order (scenes held on chip do not care; deep BVHs such as ajax do).
 namespace wf2_smem {
 #undef TB_WF2_PATHS
 #define TB_WF2_PATHS 1024
 #define TB_WF2_COLD_SMEM 1
-#include "wavefront2.cuh"
+#include "wf2_common.cuh"
+#include "wf2_rings.cuh"
 #undef TB_WF2_COLD_SMEM
 }  // namespace wf2_smem
 namespace wf2_l2 {
 #undef TB_WF2_PATHS
 #define TB_WF2_PATHS 2048
-#include "wavefront2.cuh"
+#include "wf2_common.cuh"
+#include "wf2_rings.cuh"
 }  // namespace wf2_l2
 namespace wf2_lq {
 #undef TB_WF2_PATHS
 #define TB_WF2_PATHS 1024
 #define TB_WF2_COLD_SMEM 1
-#define TB_WF2_LANEQ 1
-#include "wavefront2.cuh"
-#undef TB_WF2_LANEQ
+#include "wf2_common.cuh"
+#include "wf2_lanes.cuh"
 #undef TB_WF2_COLD_SMEM
 }  // namespace wf2_lq
 
@@ -337,18 +338,50 @@ namespace wf2_lq {
 void read_stage_clocks(unsigned long long* out, bool reset) { wf2_lq::wf2_stage_clocks(out, reset); }
 #endif
 
+// The seven wavefront kernels, in the order launch_wavefront2 chooses between them.
+using Wf2Launcher = void (*)(const LaunchParams&, int, cudaStream_t, unsigned long long);
+static const struct {
+    Wf2Launcher launch;
+    const char* name;   // reported by tb200_last_kernel
+} kWavefront2[] = {
+    {wf2_l2::launch_wavefront2_t<TB_WF2_THREADS_WIDE, wf2_l2::WF2_MODE_SPLIT>, "wf2_l2"},
+    {wf2_l2::launch_wavefront2_t<TB_WF2_THREADS_WIDE, wf2_l2::WF2_MODE_GENERIC>, "wf2_l2"},
+    {wf2_lq::launch_wavefront2_t<TB_WF2_THREADS, wf2_lq::WF2_MODE_GENERIC, TB_FEAT_NONE>, "wf2_lq.specialized"},
+    {wf2_lq::launch_wavefront2_t<TB_WF2_THREADS, wf2_lq::WF2_MODE_GENERIC>, "wf2_lq.generic"},
+    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_HARD>, "wf2_smem"},
+    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_SPLIT>, "wf2_smem"},
+    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_GENERIC>, "wf2_smem"},
+};
+enum { WF2_L2_SPLIT, WF2_L2_GENERIC, WF2_LQ_NONE, WF2_LQ_ALL, WF2_SMEM_HARD, WF2_SMEM_SPLIT, WF2_SMEM_GENERIC };
+
+// Launches the wavefront kernel the launch parameters call for; returns its name (nullptr: nothing to do).  With
+// split = the free-running scheduler with the split trace queue, the first rule that applies chooses:
+//  1. wideCta (768-thread CTAs, scenes with deep mesh BVHs): wf2_l2, SPLIT when split, else GENERIC, which runs
+//     hard phases too (P.hardPhases stays a run-time flag there).
+//  2. The free-running scheduler without the split trace queue, lane queues forced (laneQueues 2) or chosen
+//     (laneQueues 1) and a launch that is not small: wf2_lq, without the scene-feature code when p.specialized.
+//     The lane-owned layout wins in the steady state (cornell 32 spp on an H100: 1131 vs 893 Msamples/s) and loses
+//     while the slots fill and drain (1-spp frames, slabs of a multi-GPU render; measured in round 2): launches of
+//     fewer than six samples per slot are small and keep the rings.  The specialised kernel has 512-thread CTAs
+//     too: at 640 (20 warps, 96 registers) it spills 128 bytes and measured no faster on cornell.
+//  3. Otherwise wf2_smem: HARD when hardPhases, else SPLIT when split, else GENERIC.
 const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
-    // The lane-owned layout wins in the steady state (cornell 32 spp on an H100: 1131 vs 893 Msamples/s) and loses
-    // while the slots fill and drain (1-spp frames, slabs of a multi-GPU render; measured in round 2): launches of
-    // fewer than six samples per slot keep the rings.
     const unsigned long long total = p.samplesPerFrame * (unsigned long long)p.numFrames;
+    if (total == 0ull) return nullptr;
     const bool small = total < 6ull * (unsigned long long)(numSMs > 0 ? numSMs : 132) * 1024ull;
+    const bool split = !p.hardPhases && p.scene.splitValid;
+    int k;
     if (p.wideCta)
-        return wf2_l2::launch_layout(p, numSMs, stream, launchCount);
-    if (!p.hardPhases && !p.scene.splitValid && (p.laneQueues == 2 || (p.laneQueues == 1 && !small)))
-        return wf2_lq::launch_layout(p, numSMs, stream, launchCount);
-    return wf2_smem::launch_layout(p, numSMs, stream, launchCount);
+        k = split ? WF2_L2_SPLIT : WF2_L2_GENERIC;
+    else if (!p.hardPhases && !p.scene.splitValid && (p.laneQueues == 2 || (p.laneQueues == 1 && !small)))
+        k = p.specialized ? WF2_LQ_NONE : WF2_LQ_ALL;
+    else
+        k = p.hardPhases ? WF2_SMEM_HARD : split ? WF2_SMEM_SPLIT : WF2_SMEM_GENERIC;
+    cudaMemsetAsync(p.sampleCounter, 0, sizeof(unsigned long long), stream);
+    kWavefront2[k].launch(p, numSMs, stream, total);
+    if (launchCount) ++*launchCount;
+    return kWavefront2[k].name;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -53,7 +53,7 @@ const char* launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned lon
 // persistent CTA-resident wavefront pipeline with a dedicated traversal stage (the product path)
 const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
 #ifdef TB_WF2_STAGE_CLOCKS
-// development builds: the per-stage cycle counters of the lane-owned wavefront layout (wavefront2.cuh), summed
+// development builds: the per-stage cycle counters of the lane-owned wavefront layout (wf2_lanes.cuh), summed
 // over every launch since the last reset
 #define TB_WF2_STAGE_CLOCK_WORDS 15
 void read_stage_clocks(unsigned long long* out, bool reset);

@@ -78,7 +78,7 @@ def function_of_line():
 def mangled_fragment(rep, kernel):
     """The mangled name of the profiled kernel (`_ZN6wf2_lq12k_wavefront2ILi512ELi0EEEv12LaunchParamsy`), so that
     the line table of exactly that instantiation is used: the library holds the same template in several
-    namespaces (the layouts of wavefront2.cuh) and with several arguments."""
+    namespaces (the layouts of wf2_common.cuh) and with several arguments."""
     raw = subprocess.check_output(["ncu", "-i", rep, "--page", "raw", "--csv", "--print-kernel-base", "mangled"], text=True, stderr=subprocess.DEVNULL)
     rows = list(csv.reader(io.StringIO(raw)))
     name = rows[2][rows[0].index("Kernel Name")]
@@ -142,7 +142,7 @@ def main():
     print("\nby line: %inst lanes %samples")
     for k, v in sorted(by_line.items(), key=lambda x: -x[1][2])[:30]:
         print("  %-34s %5.1f %5.1f %5.1f" % ("%s:%s" % k if k else "?", 100.0 * v[0] / tot[0], v[1] / max(1, v[0]), 100.0 * v[2] / max(1, tot[2])))
-    only = os.environ.get("NCU_LINES_FILE")   # e.g. wavefront2.cuh: every line of that file, in line order
+    only = os.environ.get("NCU_LINES_FILE")   # e.g. wf2_lanes.cuh: every line of that file, in line order
     if only:
         print("\nevery line of %s: %%inst lanes %%samples" % only)
         for k, v in sorted((kv for kv in by_line.items() if kv[0] and kv[0][0] == only), key=lambda x: x[0][1]):

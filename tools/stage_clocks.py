@@ -24,7 +24,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 VARIANT = "libtinsel_b200_clocks.so"
 WORDS = 15                     # tb_kernels.cuh: TB_WF2_STAGE_CLOCK_WORDS
 WARPS_PER_CTA = 512 // 32
-STAGES = ["R", "T", "A", "B"]  # counter order (wavefront2.cuh: Wf2Clocks)
+STAGES = ["R", "T", "A", "B"]  # counter order (wf2_lanes.cuh: Wf2Clocks)
 
 
 def main():
