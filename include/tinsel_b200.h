@@ -195,6 +195,11 @@ int tb200_num_devices(const tb200_renderer* r);
 void tb200_slab_rows(int height, int member, int numMembers, int* firstRow, int* numRows);
 void tb200_slab_traced_rows(int height, int firstRow, int numRows, float filterWidth, int* firstTraced, int* numTraced);
 
+/* The multiplier and shift with which the kernels divide sample indices by a launch's samples per frame and
+ * tile index by its 8-pixel tile columns: for every 32-bit n, n / d == (((n * mul) >> 32) + n) >> shift, the
+ * product and the sum formed in 64 bits.  d = 0 gives 0, 0. */
+void tb200_divisor_magic(unsigned int d, unsigned int* mul, unsigned int* shift);
+
 /* Replaces Renderer::Init (src/render.h:70; semantics of src/render.cu:1070-1075):
  * (re)allocates and zeroes the device accumulator, resets the frame counter. Returns 0 on success. */
 int tb200_init(tb200_renderer* r, int width, int height);

@@ -56,6 +56,8 @@ def load_library():
     lib.tb200_num_devices.argtypes = [C.c_void_p]
     lib.tb200_slab_rows.restype = None
     lib.tb200_slab_rows.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    lib.tb200_divisor_magic.restype = None
+    lib.tb200_divisor_magic.argtypes = [C.c_uint, C.POINTER(C.c_uint), C.POINTER(C.c_uint)]
     lib.tb200_slab_traced_rows.restype = None
     lib.tb200_slab_traced_rows.argtypes = [C.c_int, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.tb200_set_slab.restype = C.c_int

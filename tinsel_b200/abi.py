@@ -173,6 +173,7 @@ EXPORTS = [
     "tb200_get_member_stats",
     "tb200_slab_rows",
     "tb200_slab_traced_rows",
+    "tb200_divisor_magic",
     "tb200_set_slab",
     "tb200_pin_output",
     "tb200_unpin_output",

@@ -1688,6 +1688,14 @@ void tb200_slab_traced_rows(int height, int firstRow, int numRows, float filterW
     if (numTraced) *numTraced = hi > lo ? std::min(height, hi + reach) - t0 : 0;
 }
 
+void tb200_divisor_magic(unsigned int d, unsigned int* mul, unsigned int* shift)
+{
+    uint32_t m = 0, l = 0;
+    divisor_magic(d, &m, &l);
+    if (mul) *mul = m;
+    if (shift) *shift = l;
+}
+
 static int render_n_one(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options, int n, float* output)
 {
     cudaSetDevice(r->device);
@@ -2009,7 +2017,7 @@ int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, 
 int tb200_stage_clocks(unsigned long long* out, int n, int reset)
 {
     if (!out || n < TB_WF2_STAGE_CLOCK_WORDS) {
-        set_error("tb200_stage_clocks: need room for 15 counters");
+        set_error("tb200_stage_clocks: need room for 18 counters");
         return -1;
     }
     if (cudaDeviceSynchronize() != cudaSuccess) {

@@ -17,18 +17,35 @@ void finalize_params(LaunchParams* p)
     // tile rows t in [0, tileRowsAll) with t % numShards == shard
     p->tileRows = tileRowsAll > p->shard ? (tileRowsAll - p->shard + p->numShards - 1) / p->numShards : 0;
     p->samplesPerFrame = (unsigned long long)p->tilesX * (unsigned long long)p->tileRows * 32ull;
+    divisor_magic((uint32_t)p->samplesPerFrame, &p->spfMul, &p->spfShift);
+    divisor_magic((uint32_t)p->tilesX, &p->tilesXMul, &p->tilesXShift);
 }
 
-// (launches are split on the host so that idx and samplesPerFrame fit 31 bits: 32-bit division)
+// Division by an invariant integer (Granlund and Montgomery, "Division by invariant integers using
+// multiplication", 1994, section 4): with l = ceil(log2 d) and m = floor(2^32 (2^l - d) / d) + 1, which fits 32 bits,
+// n / d = (mulhi(n, m) + n) >> l for every 32-bit n, the sum formed in 64 bits.  d = 0 (no samples) gives 0, 0.
+void divisor_magic(uint32_t d, uint32_t* mul, uint32_t* shift)
+{
+    uint32_t l = 0;
+    while (l < 32 && (1ull << l) < d) ++l;
+    *mul = d ? (uint32_t)((((1ull << 32) * ((1ull << l) - d)) / d) + 1ull) : 0u;
+    *shift = l;
+}
+
+TB_DEV uint32_t div_magic(uint32_t n, uint32_t mul, uint32_t shift) { return (uint32_t)(((unsigned long long)__umulhi(n, mul) + n) >> shift); }
+
+// (launches are split on the host so that idx and samplesPerFrame fit 31 bits: 32-bit division, by the
+// multipliers finalize_params computed)
 TB_DEV bool decode_sample(const LaunchParams& P, unsigned long long idx64, int& px, int& py, int& frame)
 {
     const uint32_t idx = (uint32_t)idx64, spf = (uint32_t)P.samplesPerFrame;
-    const uint32_t f = idx / spf;
+    const uint32_t f = div_magic(idx, P.spfMul, P.spfShift);
     frame = P.frame0 + (int)f;
     const uint32_t local = idx - f * spf;
     const uint32_t tile = local >> 5, in = local & 31u;
-    px = (int)((tile % (uint32_t)P.tilesX) * 8u + (in & 7u));
-    const int tileRow = (int)(tile / (uint32_t)P.tilesX) * P.numShards + P.shard;
+    const uint32_t tileY = div_magic(tile, P.tilesXMul, P.tilesXShift);
+    px = (int)((tile - tileY * (uint32_t)P.tilesX) * 8u + (in & 7u));
+    const int tileRow = (int)tileY * P.numShards + P.shard;
     const int ry = tileRow * 4 + (int)(in >> 3);
     py = P.firstRow + ry;
     return px < P.film.width && ry < P.numRows;

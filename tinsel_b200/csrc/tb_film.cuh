@@ -87,3 +87,42 @@ TB_DEV void add_sample(const DFilm& f, float4* accum, float rasterX, float raste
         }
     }
 }
+
+// add_sample with the Gaussian's weights evaluated once per column and once per row: for a finite sample whose
+// footprint is at most 3x3 pixels, the six filter_gaussian values are independent, inline expf chains that run
+// side by side (add_sample makes up to twelve out-of-line calls, one after the other).  Each pixel's weight is
+// still gx * gy, and the pixels whose weight is zero are still skipped, so every reduction carries the same bits.
+// Anything else takes add_sample.
+TB_DEV void add_sample_small(const DFilm& f, float4* accum, float rasterX, float rasterY, V3 sample)
+{
+    const int startX = tb_max(0, int(rasterX - f.filterWidth));
+    const int startY = tb_max(f.rowLo, int(rasterY - f.filterWidth));
+    const int endX = tb_min(int(rasterX + f.filterWidth), f.width - 1);
+    const int endY = tb_min(int(rasterY + f.filterWidth), f.rowHi - 1);
+    V3 c = sample;
+    const float l = length(sample);
+    if (l > f.clamp) c = sample * (f.clamp / l);
+    if (f.filterType != TB200_FILTER_GAUSSIAN || endX - startX > 2 || endY - startY > 2 || !(isfinite(c.x) && isfinite(c.y) && isfinite(c.z))) {
+        add_sample(f, accum, rasterX, rasterY, sample);
+        return;
+    }
+    float gx[3], gy[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        // filter_gaussian, with tbm_expf inline
+        const float dx = (float)(startX + k) - rasterX, dy = (float)(startY + k) - rasterY;
+        const float ax = -f.filterFalloff * dx * dx, ay = -f.filterFalloff * dy * dy;
+        gx[k] = ax < f.filterArgZero ? 0.0f : tb_max(0.0f, tbm_expf(ax) - f.filterOffset);
+        gy[k] = ay < f.filterArgZero ? 0.0f : tb_max(0.0f, tbm_expf(ay) - f.filterOffset);
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        if (startX + i > endX || gx[i] == 0.0f) continue;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            const float w = gx[i] * gy[j];
+            if (startY + j > endY || w == 0.0f) continue;
+            accum_add(accum, (startY + j) * f.width + startX + i, c.x * w, c.y * w, c.z * w, w);
+        }
+    }
+}

@@ -25,6 +25,8 @@ struct LaunchParams {
     int tilesX;           // 8-pixel tile columns
     int tileRows;         // tile rows owned by this shard inside the row range
     unsigned long long samplesPerFrame;   // tilesX * tileRows * 32 (includes padding outside the image)
+    uint32_t spfMul, spfShift;            // division by samplesPerFrame and by tilesX: divisor_magic, set by finalize_params
+    uint32_t tilesXMul, tilesXShift;
     // tb200_trace_frame outputs (nullptr in normal rendering)
     float* outRadiance;   // 3 floats per pixel
     float* outRaster;     // 2 floats per pixel
@@ -44,8 +46,10 @@ struct LaunchParams {
 
 #define TB_MAX_BANDS 64
 
-// fills tilesX / tileRows / samplesPerFrame from the row range and shard
+// fills tilesX / tileRows / samplesPerFrame and their division multipliers from the row range and shard
 void finalize_params(LaunchParams* p);
+// multiplier and shift that divide every 32-bit integer by d exactly (kernels.cu; tb200_divisor_magic)
+void divisor_magic(uint32_t d, uint32_t* mul, uint32_t* shift);
 
 // The launches below return the name of the kernel they ran (nullptr when there was no work), for tb200_last_kernel.
 // one thread per (pixel, frame): the whole path in registers.  Validation / fallback pipeline.
@@ -55,7 +59,7 @@ const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t st
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds: the per-stage cycle counters of the lane-owned wavefront layout (wf2_lanes.cuh), summed
 // over every launch since the last reset
-#define TB_WF2_STAGE_CLOCK_WORDS 15
+#define TB_WF2_STAGE_CLOCK_WORDS 18
 void read_stage_clocks(unsigned long long* out, bool reset);
 #endif
 // eNormals mode (render.cpp:494-515)

@@ -35,16 +35,19 @@ enum { WF2_PH_EXT = 0, WF2_PH_NEE = 1 };
 
 // Cold half of a slot's state: 16-byte chunks, one record per slot, accessed by the one lane that owns the slot at
 // the time (ownership moves through the stage queues, whose pushes are preceded by a block-scope fence).  Chunks 0-3:
-//   0: T.xyz, eta        1: L.xyz, bsdfPdf     2: absorption.xyz, sample index     3: rng1, rng2 (.zw: layout's own)
+//   0: T.xyz, eta        1: L.xyz, bsdfPdf     2: absorption.xyz, sample index     3: rng1, rng2 (.zw: layout's own;
+// the lane-owned layout keeps the sample's raster position there)
 // TB_WF2_COLD_SMEM: the records live in shared memory (Wf2Shared::cold); otherwise in global memory (P.cold),
 // read with ld.global.cg / written with st.global.cg.
 enum { CC_T = 0, CC_L = 1, CC_A = 2, CC_RNG = 3 };
 #ifdef TB_WF2_COLD_SMEM
 TB_DEV float4 cold_ld(const float4* rec, int c) { return rec[c]; }
 TB_DEV void cold_st(float4* rec, int c, float x, float y, float z, float w) { rec[c] = make_float4(x, y, z, w); }
+TB_DEV void cold_st2(float4* rec, int c, float x, float y) { *reinterpret_cast<float2*>(rec + c) = make_float2(x, y); }
 #else
 TB_DEV float4 cold_ld(const float4* rec, int c) { return __ldcg(rec + c); }
 TB_DEV void cold_st(float4* rec, int c, float x, float y, float z, float w) { __stcg(rec + c, make_float4(x, y, z, w)); }
+TB_DEV void cold_st2(float4* rec, int c, float x, float y) { __stcg(reinterpret_cast<float2*>(rec + c), make_float2(x, y)); }
 #endif
 TB_DEV float u2f(uint32_t v) { return __uint_as_float(v); }
 TB_DEV uint32_t f2u(float v) { return __float_as_uint(v); }
@@ -210,7 +213,7 @@ TB_DEV bool wf2_scatter(Wf2SharedBase& S, float4* rec, const DScene& sc, int s, 
     S.dx[s] = ps.d.x; S.dy[s] = ps.d.y; S.dz[s] = ps.d.z;
     cold_st(rec, CC_T, ps.T.x, ps.T.y, ps.T.z, ps.eta);
     cold_st(rec, CC_A, ps.absorb.x, ps.absorb.y, ps.absorb.z, u2f(sample));
-    cold_st(rec, CC_RNG, u2f(ps.rng.s1), u2f(ps.rng.s2), 0.0f, 0.0f);
+    cold_st2(rec, CC_RNG, u2f(ps.rng.s1), u2f(ps.rng.s2));   // .zw: the layout's own
     S.flags[s] = ((uint32_t)ps.rayType << 1) | ((uint32_t)WF2_PH_EXT << 3) | ((uint32_t)(bounce + 1) << 8);
     return true;
 }
@@ -317,6 +320,7 @@ TB_DEV void wf2_await_scene(Shared& S)
 
 // Stage R, by a whole warp (`active` lanes hold slot s, cold record `rec`): splat the finished sample, claim a new one
 // and generate its camera ray.  Returns true where one was; the caller pushes those, then wf2_retire()s the others.
+// The ring kernels' stage R; the lane-owned kernel has its own (wf2_lanes.cuh: wf2_lq_stage_r).
 template <class Shared>
 TB_DEV bool wf2_stage_r(Shared& S, const LaunchParams& P, unsigned long long total, float4* rec, int s, bool active)
 {

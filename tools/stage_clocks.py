@@ -7,6 +7,8 @@ Builds the development variant with the kernel's own clock64() accounting (-DTB_
 product build) as tinsel_b200/libtinsel_b200_clocks.so, renders cornell in the benchmark's shape with it
 (1024x1024, 32 spp per render_device call, TINSEL_B200_LIB pointing at the variant) and prints per stage:
 SM cycles per camera sample, visits (warp chunks) per sample and the mean number of lanes active per chunk.
+Stage R is also split into its parts: the splat of the finished sample, the claim of new sample indices (from
+the vote to the index) and the regeneration (the camera rays).
 
     python tools/stage_clocks.py [--steps N] [--lib PATH | --no-build]
 
@@ -22,9 +24,10 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 VARIANT = "libtinsel_b200_clocks.so"
-WORDS = 15                     # tb_kernels.cuh: TB_WF2_STAGE_CLOCK_WORDS
+WORDS = 18                     # tb_kernels.cuh: TB_WF2_STAGE_CLOCK_WORDS
 WARPS_PER_CTA = 512 // 32
 STAGES = ["R", "T", "A", "B"]  # counter order (wf2_lanes.cuh: Wf2Clocks)
+R_PARTS = ["splat", "claim", "regenerate"]   # wf2_lanes.cuh: WF2_R_*
 
 
 def main():
@@ -90,6 +93,10 @@ def main():
             continue
         print("%-10s %14.1f %7.1f%% %16.3f %12.2f" % (name, cyc[k] / per, 100.0 * cyc[k] / total, lanes[k] / samples,
                                                      lanes[k] / chunks[k]))
+        if name == "R":
+            # stage R's parts; what is left is the bookkeeping between them (flags, the claim loop's vote)
+            for p, part in enumerate(R_PARTS):
+                print("%-10s %14.1f %7.1f%%" % ("  " + part, c[15 + p] / per, 100.0 * c[15 + p] / total))
     print("%-10s %14.1f" % ("total", total / per))
 
 
