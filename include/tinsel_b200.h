@@ -137,7 +137,12 @@ typedef struct tb200_camera {
     float shutterEnd;
 } tb200_camera;
 
-/* Options + Filter (src/render.h:13-63); same field order as the reference. */
+/* Options + Filter (src/render.h:13-63); same field order as the reference.
+ * Every call that takes options refuses them (returns -1, tb200_last_error says why, nothing is launched and
+ * the accumulator is untouched) when filterType is neither TB200_FILTER_BOX nor TB200_FILTER_GAUSSIAN, or when
+ * filterWidth is not finite or is 2^30 or more in magnitude: the splat converts raster +- filterWidth to int,
+ * and only below that bound does the conversion mean the same on every side.  filterFalloff, filterOffset and
+ * clamp only enter arithmetic and are taken as they are, NaN and infinities included. */
 enum { TB200_FILTER_BOX = 0, TB200_FILTER_GAUSSIAN = 1 };
 enum { TB200_MODE_NORMALS = 0, TB200_MODE_COMPLEXITY = 1, TB200_MODE_PATHTRACE = 2 };
 typedef struct tb200_options {

@@ -1111,6 +1111,23 @@ float oracle_filter_eval(int type, float width, float falloff, float offset, flo
     if (type != TB200_FILTER_GAUSSIAN) return 1.0f;
     return filter_gauss(o, x) * filter_gauss(o, y);
 }
+// add_sample (render.cpp:401-445) of n independent samples, sample k into its own caller-zeroed W x H film
+// films + k*H*W*4: filterType[k]; params[4k..4k+3] = width, falloff, offset, clamp; samples[5k..5k+4] =
+// rasterX, rasterY, r, g, b.
+void oracle_add_samples(int n, int W, int H, const int32_t* filterType, const float* params, const float* samples, float* films)
+{
+    tb200_options o;
+    memset(&o, 0, sizeof(o));
+    o.width = W;
+    o.height = H;
+    for (int k = 0; k < n; ++k) {
+        const float* p = params + 4 * (size_t)k;
+        const float* s = samples + 5 * (size_t)k;
+        o.filterType = filterType[k];
+        o.filterWidth = p[0]; o.filterFalloff = p[1]; o.filterOffset = p[2]; o.clamp = p[3];
+        add_sample(o, films + (size_t)k * W * H * 4, W, H, s[0], s[1], mk(s[2], s[3], s[4]));
+    }
+}
 int oracle_trace(void* h, const float* o, const float* d, float time, float* t, float* n)
 {
     hit_t hit = closest_hit(*((Oracle*)h)->scene, from(o), from(d), time);

@@ -242,6 +242,7 @@ def load_port():
     lib.oracle_generate_ray.argtypes = [C.POINTER(abi.Camera), C.c_int, C.c_int, C.c_float, C.c_float, _f32p, _f32p]
     lib.oracle_filter_eval.restype = C.c_float
     lib.oracle_filter_eval.argtypes = [C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float]
+    lib.oracle_add_samples.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32), _f32p, _f32p, _f32p]
     lib.oracle_trace.restype = C.c_int
     lib.oracle_trace.argtypes = [C.c_void_p, _f32p, _f32p, C.c_float, _f32p, _f32p]
     lib.oracle_probe_sample.argtypes = [C.c_void_p, C.c_int, _f32p, _f32p, _f32p]
@@ -326,6 +327,21 @@ class PortScene:
         if self.h:
             self.lib.oracle_destroy(self.h)
             self.h = None
+
+
+def port_add_samples(width, height, filter_type, params, samples):
+    """The restatement's add_sample (render.cpp:401-445) of n samples, each into its own zeroed film.
+    filter_type (n,) int32; params (n, 4) float32: width, falloff, offset, clamp; samples (n, 5) float32:
+    rasterX, rasterY, r, g, b.  Returns (n, height, width, 4) float32."""
+    filter_type = np.ascontiguousarray(filter_type, np.int32)
+    params = np.ascontiguousarray(params, np.float32)
+    samples = np.ascontiguousarray(samples, np.float32)
+    n = filter_type.shape[0]
+    assert params.shape == (n, 4) and samples.shape == (n, 5)
+    films = np.zeros((n, height, width, 4), np.float32)
+    load_port().oracle_add_samples(n, width, height, filter_type.ctypes.data_as(C.POINTER(C.c_int32)), _fp(params),
+                                   _fp(samples), _fp(films))
+    return films
 
 
 # ---- display/finish step (src/main.cpp:262-271, src/png.cpp:329-343) -----------------------------

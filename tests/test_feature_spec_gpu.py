@@ -38,25 +38,30 @@ def _port(path):
 
 
 def _trace(path, frame=2):
-    """Per-sample radiance of one frame on the GPU and the name of the kernel that traced it."""
+    """Per-sample radiance and raster position of one frame on the GPU, and the name of the kernel that traced it.
+    The lane-owned kernel carries each sample's raster position in its slot from the sample's generation to its
+    splat (wf2_lanes.cuh: wf2_lq_stage_r), past every stage that must leave it alone."""
     snap = tb.Snapshot(path)
     cam, opt = snap.camera, snap.options
     opt.width, opt.height = SIZE
     r = tb.Renderer(snap.scene)
     r.Init(*SIZE)
-    rad, _ = r.trace_frame(cam, opt, frame)
+    rad, ras = r.trace_frame(cam, opt, frame)
     kernel = r.last_kernel()
     r.close()
     snap.close()
-    return rad, kernel
+    return (rad, ras), kernel
 
 
-def _assert_matches_port(path, rad, frame=2):
+def _assert_matches_port(path, traced, frame=2):
+    rad, ras = traced
     port = _port(path)
-    prad, _ = port.trace_frame(frame, nthreads=8)
+    prad, pras = port.trace_frame(frame, nthreads=8)
     port.close()
     same = (rad.view(np.uint32) == prad.view(np.uint32)).all(-1) | (np.isnan(rad).any(-1) & np.isnan(prad).any(-1))
     assert same.all(), "%s: %d of %d samples differ from the CPU restatement" % (path, int((~same).sum()), same.size)
+    same = (ras.view(np.uint32) == pras.view(np.uint32)).all(-1)
+    assert same.all(), "%s: %d of %d raster positions differ from the CPU restatement" % (path, int((~same).sum()), same.size)
 
 
 @pytest.mark.parametrize("name,kernel", [("cornell", SPECIALIZED), ("simple", SPECIALIZED), ("gloss", SPECIALIZED),
@@ -81,7 +86,7 @@ def test_specialized_equals_generic_and_restatement(name, monkeypatch):
     monkeypatch.setenv("TINSEL_B200_SPECIALIZE", "0")
     grad, gran = _trace(path)
     assert gran == GENERIC
-    assert (rad.view(np.uint32) == grad.view(np.uint32)).all()
+    assert all((a.view(np.uint32) == b.view(np.uint32)).all() for a, b in zip(rad, grad))
     _assert_matches_port(path, rad)
 
 
@@ -140,5 +145,5 @@ def test_absorption_reaches_the_image(tmp_path):
     path = _cornell_variant(tmp_path, "transmission", "absorption")
     rad, ran = _trace(path)
     assert ran == GENERIC
-    assert not (rad.view(np.uint32) == clear.view(np.uint32)).all()
+    assert not (rad[0].view(np.uint32) == clear[0].view(np.uint32)).all()
     _assert_matches_port(path, rad)

@@ -221,30 +221,54 @@ def test_interleaved_shards(scenes):
     snap.close()
 
 
-@pytest.mark.parametrize("name,size,parts", [("cornell", (200, 150), 3), ("veach", (160, 90), 2), ("cornell", (64, 9), 4)])
-def test_row_slabs(name, size, parts, scenes):
-    """Owner-computes row slabs: set_slab renderers side by side, and a create_multi group whose members share the
-    one device.  The rows each owner delivers must equal the whole image's reference."""
-    snap, cam, opt = setup(scenes[name], size)
-    ref = reference(scenes[name], size, range(4), [opt])[0]
-    out = np.full((size[1], size[0], 4), -7.0, np.float32)
-    with env(TINSEL_B200_PIPELINE=None):
-        for k in range(parts):
-            row0, nrows = sharding.slab_rows(size[1], k, parts)
+SLAB_CASES = [("cornell", (200, 150), 3), ("veach", (160, 90), 2), ("cornell", (64, 9), 4),
+              ("cornell", (64, 37), [(0, 13), (13, 1), (14, 0), (14, 23)])]   # cuts off the 4-row tile grid
+SLAB_FILTERS = [("scene", {}), ("gauss-1.5", {"filterWidth": 1.5}), ("gauss-3.5", {"filterWidth": 3.5}),
+                ("box-0.5", {"filterType": tb.abi.FILTER_BOX, "filterWidth": 0.5})]
+SENTINEL = -7.0
+
+
+@pytest.mark.parametrize("queues", ["rings", "lanes"])
+@pytest.mark.parametrize("filt", SLAB_FILTERS, ids=[f[0] for f in SLAB_FILTERS])
+@pytest.mark.parametrize("name,size,parts", SLAB_CASES)
+def test_row_slabs(name, size, parts, filt, queues, scenes):
+    """Owner-computes row slabs: set_slab renderers side by side, 4 Render() calls and one render_device(4) each, and
+    a create_multi group whose members share the one device.  The rows each owner delivers, into a buffer filled with
+    a sentinel, must equal the whole image's reference.  `parts`: a number of tile-row slabs (sharding.slab_rows),
+    or a list of (first row, rows)."""
+    fname, changes = filt
+    snap, cam, opt = setup(scenes[name], size, changes)
+    ref = reference(scenes[name], size, range(4), [opt], key=("slab", name, size, fname))[0]
+    cuts = [sharding.slab_rows(size[1], k, parts) for k in range(parts)] if isinstance(parts, int) else parts
+    what = "%s %dx%d %s queues=%s" % (name, size[0], size[1], fname, queues)
+    with env(**QUEUES[queues]):
+        render_out = np.full((size[1], size[0], 4), SENTINEL, np.float32)
+        device_out = render_out.copy()
+        for row0, nrows in cuts:
             r = renderer(snap, opt)
             r.set_slab(row0, nrows)
             for _ in range(4):
-                r.Render(cam, opt, out)
+                r.Render(cam, opt, render_out)
+            r.Init(*size)
+            r.render_device(cam, opt, 4)
+            if queues == "lanes" and nrows:
+                assert r.last_kernel().startswith("wf2_lq"), r.last_kernel()
+            r.read_accumulator(device_out)
             r.close()
-        filmref.assert_film_close(out, ref, "%s %dx%d %d set_slab renderers" % (name, size[0], size[1], parts))
+        filmref.assert_film_close(render_out, ref, "%s: %d set_slab renderers, Render() x 4" % (what, len(cuts)))
+        filmref.assert_film_close(device_out, ref, "%s: %d set_slab renderers, render_device(4)" % (what, len(cuts)))
         with env(TINSEL_B200_TEST_DUP_DEVICES="1"):
-            m = tb.Renderer(snap.scene, devices=[0] * parts)
+            m = tb.Renderer(snap.scene, devices=[0] * len(cuts))
         m.Init(*size)
-        out = np.zeros_like(out)
+        out = np.full_like(render_out, SENTINEL)
         for _ in range(4):
             m.Render(cam, opt, out)
         assert m.stats().samples == 4 * size[0] * size[1]
-        filmref.assert_film_close(out, ref, "%s %dx%d create_multi of %d" % (name, size[0], size[1], parts))
+        filmref.assert_film_close(out, ref, "%s: create_multi of %d, Render() x 4" % (what, len(cuts)))
+        m.Init(*size)
+        m.render_device(cam, opt, 4)
+        out = m.read_accumulator(np.full_like(render_out, SENTINEL))
+        filmref.assert_film_close(out, ref, "%s: create_multi of %d, render_device(4)" % (what, len(cuts)))
         m.close()
     snap.close()
 
@@ -266,22 +290,38 @@ def test_ragged_sizes(size, queues, scenes):
     snap.close()
 
 
-# ---- the film's edges: every filter variant in both pipelines ----
+# ---- the film's edges: every filter variant in every kernel ----
 
 FILTER_CASES = [(v[0], v[1], v[2], "cornell") for v in VARIANTS] + [("nan-probe", (40, 30), NAN_FILTER, "nan-probe")]
+# the lane-owned layout whatever the launch size, as in test_feature_spec_gpu.py
+LANES = dict(TINSEL_B200_PIPELINE=None, TINSEL_B200_QUEUES="lanes", TINSEL_B200_SCHED="free", TINSEL_B200_SPLIT="0",
+             TINSEL_B200_CTA="512")
+QUEUES = {"rings": dict(TINSEL_B200_PIPELINE=None, TINSEL_B200_QUEUES="ring"), "lanes": LANES}
+PIPELINES = {"mega": dict(TINSEL_B200_PIPELINE="mega"), "rings": QUEUES["rings"], "lanes": LANES,
+             "lanes-generic": dict(LANES, TINSEL_B200_SPECIALIZE="0")}
+FILTER_RUNS = [(c, p) for c in FILTER_CASES for p in PIPELINES if p != "lanes-generic" or c[3] == "cornell"]
 
 
-@pytest.mark.parametrize("pipeline", ["mega", "wavefront"])
-@pytest.mark.parametrize("case", FILTER_CASES, ids=[c[0] for c in FILTER_CASES])
+def expected_kernel(pipeline, scene):
+    """The kernel each forced pipeline must run (kernels.cu: launch_mega, launch_wavefront2)."""
+    if pipeline == "mega":
+        return "k_mega"
+    if pipeline == "rings":
+        return "wf2_smem"
+    return "wf2_lq.specialized" if pipeline == "lanes" and scene == "cornell" else "wf2_lq.generic"
+
+
+@pytest.mark.parametrize("case,pipeline", FILTER_RUNS, ids=["%s-%s" % (c[0], p) for c, p in FILTER_RUNS])
 def test_filter_variants(case, pipeline, scenes):
     what, size, changes, scene = case
     snap, cam, opt = setup(scenes[scene], size, changes)
     ref = reference(scenes[scene], size, range(4), [opt], key=("filter", what))[0]
     if scene == "nan-probe":
         assert np.isnan(ref.sums).any() and np.isfinite(ref.sums).any()
-    with env(TINSEL_B200_PIPELINE=pipeline):
+    with env(**dict({"TINSEL_B200_SPECIALIZE": None}, **PIPELINES[pipeline])):
         r = renderer(snap, opt)
     r.render_device(cam, opt, 4)
+    assert r.last_kernel() == expected_kernel(pipeline, scene)
     filmref.assert_film_close(r.read_accumulator(), ref, "%s %dx%d %s %s" % (scene, size[0], size[1], what, pipeline))
     r.close()
     snap.close()

@@ -114,6 +114,24 @@ def test_slab_rule_matches_the_c_abi():
     assert sharding.slab_traced_rows(1024, 0, 128, 0.75) == (0, 130)
 
 
+def test_slab_traced_rows_of_unbounded_widths_stay_in_the_image():
+    """tb200_slab_traced_rows takes a width that no fill_params has checked: infinite, NaN and huge widths must give
+    traced rows inside the image (the whole image, or the slab alone for NaN), never an int overflow."""
+    import ctypes as C
+    lib = tb.load_library()
+    for fw in (float("inf"), float("-inf"), float("nan"), 1e30, -1e30, 2.0 ** 30, 3e38):
+        for h, row0, rows in ((1, 0, 1), (70, 0, 68), (70, 32, 20), (1080, 1076, 4), (2048, 512, 512), (64, 13, 0)):
+            t0, tn = C.c_int(), C.c_int()
+            lib.tb200_slab_traced_rows(h, row0, rows, fw, C.byref(t0), C.byref(tn))
+            what = (fw, h, row0, rows, t0.value, tn.value)
+            assert (t0.value, tn.value) == sharding.slab_traced_rows(h, row0, rows, fw), what
+            assert 0 <= t0.value <= h and 0 <= tn.value and t0.value + tn.value <= h, what
+            if rows:
+                assert t0.value <= row0 and t0.value + tn.value >= row0 + rows, what
+            if fw > 1e6:
+                assert (t0.value, tn.value) == ((0, h) if rows else (max(0, row0 - 2 ** 30 - 1), 0)), what
+
+
 def _slab_worker(rank, world, port, w, h, spp, out_path):
     import torch
     import torch.distributed as dist

@@ -842,14 +842,30 @@ bool validate_image(const SceneImage& img, std::string* why)
     return true;
 }
 
-// pixel rows a sample of row y can splat into: y - reach .. y + reach (render.cpp:404-407)
-int filter_reach(float filterWidth) { return (int)ceilf(std::max(0.0f, filterWidth)) + 1; }
+// pixel rows a sample of row y can splat into: y - reach .. y + reach (render.cpp:404-407).  The width is
+// clamped to [0, 2^30] first (NaN counts as 0), the widths fill_params accepts, so that no width -- infinite, NaN
+// or huge -- converts to int out of range; row + reach then stays in range for images of fewer than 2^30 rows.
+int filter_reach(float filterWidth) { return (int)ceilf(std::min(std::max(0.0f, filterWidth), 1073741824.0f)) + 1; }
+
+// add_sample converts raster +- filterWidth to int.  Below 2^30 in magnitude that conversion is defined on the
+// device and the host alike for every image size; a NaN, infinite or larger width saturates on the device and is
+// undefined on the host.  Any filter type but the two known ones is read as Gaussian by the device and as a box
+// by the CPU restatement.
+bool filter_options_ok(const tb200_options* o)
+{
+    if (o->filterType != TB200_FILTER_BOX && o->filterType != TB200_FILTER_GAUSSIAN)
+        return set_error("options.filterType " + std::to_string(o->filterType) + " is neither TB200_FILTER_BOX nor TB200_FILTER_GAUSSIAN");
+    if (!(std::fabs(o->filterWidth) < 1073741824.0f))
+        return set_error("options.filterWidth " + std::to_string(o->filterWidth) + " is not finite or is 2^30 or more in magnitude");
+    return true;
+}
 
 bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_options* o, LaunchParams* P)
 {
     if (!r->dAccum) return set_error("tb200_init has not been called");
     if (o->width != r->width || o->height != r->height)
         return set_error("options.width/height differ from the last tb200_init");
+    if (!filter_options_ok(o)) return false;
     memset(P, 0, sizeof(*P));
     P->scene = r->scene;
     if (r->tunePhase == 2) P->scene.splitValid = 0;
@@ -862,13 +878,7 @@ bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_opti
     P->film.filterOffset = o->filterOffset;
     P->film.clamp = o->clamp;
     P->film.maxDepth = o->maxDepth;
-    // Gaussian() is exactly +0 wherever expf(arg) < offset; keep a 1e-3 relative margin so the
-    // shortcut never depends on the last bits of expf (tb_film.cuh: filter_gaussian)
-    P->film.filterArgZero = -INFINITY;
-    if (o->filterOffset > 0.0f && o->filterOffset < 1.0f) {
-        const float a = (float)log((double)o->filterOffset * (1.0 - 1.0e-3));
-        if (tbm_expf(a) < o->filterOffset) P->film.filterArgZero = a;
-    }
+    P->film.filterArgZero = film_filter_arg_zero(o->filterOffset);
     P->accum = r->boundAccum ? r->boundAccum : r->dAccum;
     P->sampleCounter = r->dCounter;
     P->cold = r->dCold;

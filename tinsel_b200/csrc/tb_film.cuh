@@ -37,6 +37,16 @@ TB_DEV void generate_ray(const DCamera& cam, float rx, float ry, V3& origin, V3&
     dir = normalize(p - origin);
 }
 
+// DFilm::filterArgZero for a filter offset (host).  Gaussian() is exactly +0 wherever expf(arg) < offset; keep a
+// 1e-3 relative margin so the shortcut never depends on the last bits of expf.  -inf (shortcut off) unless the
+// offset lies in (0, 1) and tbm_expf confirms the cut-off.
+inline float film_filter_arg_zero(float filterOffset)
+{
+    if (!(filterOffset > 0.0f && filterOffset < 1.0f)) return -INFINITY;
+    const float a = (float)log((double)filterOffset * (1.0 - 1.0e-3));
+    return tbm_expf(a) < filterOffset ? a : -INFINITY;
+}
+
 // Filter::Gaussian, render.h:29-32 (offset is taken as handed in, never recomputed)
 TB_DEV float filter_gaussian(const DFilm& f, float x)
 {

@@ -34,9 +34,10 @@ def slab_rows(height, member, num_members):
 
 def slab_traced_rows(height, first_row, num_rows, filter_width):
     """(first, count) of the pixel rows whose samples the owner of a slab traces: the slab plus the filter's
-    reach, ceil(width) + 1 rows, on either side (render.cpp:404-407).  Mirrors tb200_slab_traced_rows."""
+    reach, ceil(width) + 1 rows, on either side (render.cpp:404-407), with the width clamped to [0, 2^30] (NaN
+    counts as 0).  Mirrors tb200_slab_traced_rows."""
     import math
-    reach = int(math.ceil(max(0.0, filter_width))) + 1
+    reach = int(math.ceil(min(max(0.0, filter_width), 1073741824.0))) + 1
     lo = max(0, min(first_row, height))
     hi = max(lo, min(first_row + max(0, num_rows), height))
     if hi <= lo:
