@@ -323,9 +323,11 @@ void tb200_set_frame(tb200_renderer* r, int frame);
 
 void tb200_get_stats(tb200_renderer* r, tb200_stats* out);
 
-/* Name of the path-tracing kernel the renderer's last launch ran, e.g. "wf2_lq.specialized" or "wf2_lq.generic"
- * (lane-owned wavefront with or without the scene-feature code), "wf2_smem", "wf2_l2", "k_mega"; "" before the
- * first launch.  A static string.  Multi-device renderers: the head's. */
+/* Name of the path-tracing kernel the renderer's last launch ran, one per kernel: "wf2_lq.specialized" or
+ * "wf2_lq.generic" (lane-owned wavefront with or without the scene-feature code), "wf2_smem.hard",
+ * "wf2_smem.split", "wf2_smem.generic", "wf2_l2.split", "wf2_l2.generic" (ring-queue wavefront: layout before the
+ * dot, scheduling mode after it), "k_mega"; "" before the first launch.  A static string.  Multi-device renderers:
+ * the head's. */
 const char* tb200_last_kernel(tb200_renderer* r);
 
 /* The counters of ONE member of a multi-device renderer (0 = the head) and the pixel rows it owns: how the

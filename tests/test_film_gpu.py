@@ -307,11 +307,20 @@ def expected_kernel(pipeline, scene):
     if pipeline == "mega":
         return "k_mega"
     if pipeline == "rings":
-        return "wf2_smem"
+        # cornell has one shadow ray per hit and runs free; the probe scene has a light too, so it runs hard phases
+        return "wf2_smem.generic" if scene == "cornell" else "wf2_smem.hard"
     return "wf2_lq.specialized" if pipeline == "lanes" and scene == "cornell" else "wf2_lq.generic"
 
 
-@pytest.mark.parametrize("case,pipeline", FILTER_RUNS, ids=["%s-%s" % (c[0], p) for c, p in FILTER_RUNS])
+def run_id(case, pipeline):
+    """<case>-<pipeline>; a ring-queue run also names the ring kernel's scheduling mode it pins (rings-generic,
+    rings-hard), which the scene decides."""
+    if pipeline == "rings":
+        return "%s-rings-%s" % (case[0], expected_kernel(pipeline, case[3]).split(".")[1])
+    return "%s-%s" % (case[0], pipeline)
+
+
+@pytest.mark.parametrize("case,pipeline", FILTER_RUNS, ids=[run_id(c, p) for c, p in FILTER_RUNS])
 def test_filter_variants(case, pipeline, scenes):
     what, size, changes, scene = case
     snap, cam, opt = setup(scenes[scene], size, changes)

@@ -271,8 +271,8 @@ def test_max_depth_edge_cases(depth, pipeline):
 @pytest.mark.parametrize("cta", schedenv.CTAS)
 @pytest.mark.parametrize("sched", schedenv.SCHEDS)
 def test_both_scheduling_modes_bit_exact(sched, cta):
-    """Every scheduler variant x CTA size of the wavefront kernel (the per-scene heuristics of
-    api.cu build_scene pick one of them, see schedenv.sched_env) produces the same bits.  "free" at 512
+    """Every scheduler variant x CTA size of the wavefront kernel (the per-scene rule of
+    kernels.cu wavefront2_route picks one of them, see schedenv.sched_env) produces the same bits.  "free" at 512
     threads runs the lane-owned slot layout with bit-set queues on every scene without a split queue, "ring"
     the ring queues."""
     with schedenv.sched_env(sched, cta):

@@ -344,14 +344,10 @@ struct tb200_renderer {
     bool peerAccess = false;
 
     int pipeline = 2;             // 0 = mega (validation), 2 = wavefront (product)
-    int hardPhases = 1;           // wavefront scheduling mode (see wf2_rings.cuh)
-    int wideCta = 0;              // 768-thread CTAs for deep mesh BVHs (see wf2_common.cuh)
-    int laneQueues = 0;           // lane-owned slots + bit-set queues (see wf2_lanes.cuh)
-    uint32_t features = TB_FEAT_ALL;   // the scene's TB_FEAT_* features (scene_features)
-    int specialize = 1;           // scenes without any feature run the specialised lane-owned kernel (TINSEL_B200_SPECIALIZE=0: never)
+    Wf2Route route = {};          // the wavefront kernel's scheduling, decided at upload (kernels.cu: wavefront2_route)
     const char* lastKernel = "";  // the kernel the last path-tracing launch ran (tb200_last_kernel)
-    // Split trace queue on/off is decided by measurement (every variant produces the same bits): the
-    // second and third sizeable launches after tb200_create time one setting each, the faster stays.
+    // Split trace queue on/off is decided by measurement when route.tune (every variant produces the same bits):
+    // the second and third sizeable launches after tb200_create time one setting each, the faster stays.
     int tunePhase = 3;            // 0 warm-up (split), 1 measuring split, 2 measuring no split, 3 decided
     double tuneRate[2] = {0.0, 0.0};   // samples per ms with / without the split queue
     unsigned long long launchSamples = 0;   // samples of the launch whose time is in stats.gpuMs
@@ -589,45 +585,11 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
         meshes[m].rootRef = mi.rootRef;
     }
     if (!upload(meshes, &r->dMeshes, h2d)) return false;
-    // Scheduling mode of the wavefront kernel (measured): block-synchronous
-    // stages win when every surface hit spawns several shadow rays (the shade and trace stages then
-    // alternate several times per bounce and the barrier keeps all warps on one stage's code);
-    // free-running warps win otherwise, and by a wide margin when ray cost varies (deep mesh BVHs).
-    // TINSEL_B200_SCHED=hard|free overrides.
-    {
-        r->hardPhases = (img.numNee > 1 && img.maxTris <= 4096) ? 1 : 0;
-        const char* sched = getenv("TINSEL_B200_SCHED");
-        if (sched && strcmp(sched, "hard") == 0) r->hardPhases = 1;
-        if (sched && strcmp(sched, "free") == 0) r->hardPhases = 0;
-        // CTA size: deep mesh BVHs make traversal latency bound (L2 hits), which more warps hide; on
-        // scenes held in shared memory more warps only thrash the instruction cache.  TINSEL_B200_CTA=512|768.
-        r->wideCta = (!r->hardPhases && img.maxTris > 4096) ? 1 : 0;
-        // Split trace queue: rays entering the largest mesh's world bounds are queued apart from the
-        // rest (scheduling only).
-        r->scene.splitValid = 0;
-        const char* split = getenv("TINSEL_B200_SPLIT");   // 0: never, 1: whenever the scene has a mesh (tests)
-        if ((img.maxTris > 4096 || (split && atoi(split) == 1)) && img.splitBoxValid) {
-            r->scene.splitLo = img.splitLo;
-            r->scene.splitHi = img.splitHi;
-            r->scene.splitValid = 1;
-        }
-        if (split && atoi(split) == 0) r->scene.splitValid = 0;
-        r->tunePhase = (r->scene.splitValid && !split && !r->hardPhases) ? 0 : 3;   // an explicit TINSEL_B200_SPLIT is final
-        const char* cta = getenv("TINSEL_B200_CTA");
-        if (cta && atoi(cta) == 768) r->wideCta = 1;
-        if (cta && atoi(cta) == 512) r->wideCta = 0;
-        // Lane-owned slots with bit-set queues: scenes held on chip under the free-running scheduler, for launches
-        // big enough to reach a steady state (kernels.cu: launch_wavefront2; every other combination runs the
-        // ring queues).  TINSEL_B200_QUEUES=ring|lanes forces one or the other whatever the launch size.
-        r->laneQueues = 1;
-        const char* queues = getenv("TINSEL_B200_QUEUES");
-        if (queues && strcmp(queues, "ring") == 0) r->laneQueues = 0;
-        if (queues && strcmp(queues, "lanes") == 0) r->laneQueues = 2;
-        // TINSEL_B200_SPECIALIZE=0 runs the generic lane-owned kernel on scenes without features too (A/B runs, tests)
-        r->features = scene_features(img);
-        const char* spec = getenv("TINSEL_B200_SPECIALIZE");
-        r->specialize = (spec && atoi(spec) == 0) ? 0 : 1;
-    }
+    r->scene.splitValid = img.splitBoxValid;
+    r->scene.splitLo = img.splitLo;
+    r->scene.splitHi = img.splitHi;
+    r->route = wavefront2_route(img.numNee, img.maxTris, img.splitBoxValid, scene_features(img));
+    r->tunePhase = r->route.tune ? 0 : 3;
     // one element of padding each: the kernels' bulk copies round their length up to 16 bytes
     if (!upload(img.prims, &r->dPrims, h2d, 1)) return false;
     if (!upload(img.scenePairs, &r->dScenePairs, h2d, 1)) return false;
@@ -868,7 +830,6 @@ bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_opti
     if (!filter_options_ok(o)) return false;
     memset(P, 0, sizeof(*P));
     P->scene = r->scene;
-    if (r->tunePhase == 2) P->scene.splitValid = 0;
     camera_setup(*camera, o->width, o->height, &P->camera);
     P->film.width = o->width;
     P->film.height = o->height;
@@ -882,10 +843,6 @@ bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_opti
     P->accum = r->boundAccum ? r->boundAccum : r->dAccum;
     P->sampleCounter = r->dCounter;
     P->cold = r->dCold;
-    P->hardPhases = r->hardPhases;
-    P->wideCta = r->wideCta;
-    P->laneQueues = r->laneQueues;
-    P->specialized = (r->specialize && r->features == TB_FEAT_NONE) ? 1 : 0;
     P->firstRow = 0;
     P->numRows = o->height;
     P->film.rowLo = 0;
@@ -919,7 +876,7 @@ bool launch_frames(tb200_renderer* r, LaunchParams& P, bool recordStart = true)
         for (int f = 0; f < frames; f += framesPerLaunch) {
             P.frame0 = frame0 + f;
             P.numFrames = std::min(framesPerLaunch, frames - f);
-            const char* name = r->pipeline == 0 ? launch_mega(P, r->stream, &launches) : launch_wavefront2(P, r->numSMs, r->stream, &launches);
+            const char* name = r->pipeline == 0 ? launch_mega(P, r->stream, &launches) : launch_wavefront2(P, r->route, r->numSMs, r->stream, &launches);
             if (name) r->lastKernel = name;
         }
         P.frame0 = frame0;
@@ -947,11 +904,10 @@ void tune_update(tb200_renderer* r)
     if (r->tunePhase >= 3 || r->launchSamples < (1ull << 18) || !(r->stats.gpuMs > 0.0)) return;
     const double rate = (double)r->launchSamples / r->stats.gpuMs;
     if (r->tunePhase == 1) r->tuneRate[0] = rate;
-    if (r->tunePhase == 2) {
-        r->tuneRate[1] = rate;
-        r->scene.splitValid = r->tuneRate[0] >= r->tuneRate[1] ? 1 : 0;
-    }
+    if (r->tunePhase == 2) r->tuneRate[1] = rate;
     r->tunePhase += 1;
+    // phase 2 runs without the split queue; once it is measured, the faster setting stays
+    if (r->tunePhase >= 2) r->route.split = r->tunePhase == 3 && r->tuneRate[0] >= r->tuneRate[1];
 }
 
 bool finish_timing(tb200_renderer* r)

@@ -309,6 +309,7 @@ void launch_nlm(const NlmParams& p, cudaStream_t stream, unsigned long long* lau
 }
 
 #include <algorithm>
+#include <cstdlib>
 #include <mutex>
 
 // dynamic shared memory a CTA may opt in to on the current device (227 KB on sm_90a)
@@ -361,42 +362,75 @@ static const struct {
     Wf2Launcher launch;
     const char* name;   // reported by tb200_last_kernel
 } kWavefront2[] = {
-    {wf2_l2::launch_wavefront2_t<TB_WF2_THREADS_WIDE, wf2_l2::WF2_MODE_SPLIT>, "wf2_l2"},
-    {wf2_l2::launch_wavefront2_t<TB_WF2_THREADS_WIDE, wf2_l2::WF2_MODE_GENERIC>, "wf2_l2"},
+    {wf2_l2::launch_wavefront2_t<TB_WF2_THREADS_WIDE, wf2_l2::WF2_MODE_SPLIT>, "wf2_l2.split"},
+    {wf2_l2::launch_wavefront2_t<TB_WF2_THREADS_WIDE, wf2_l2::WF2_MODE_GENERIC>, "wf2_l2.generic"},
     {wf2_lq::launch_wavefront2_t<TB_WF2_THREADS, wf2_lq::WF2_MODE_GENERIC, TB_FEAT_NONE>, "wf2_lq.specialized"},
     {wf2_lq::launch_wavefront2_t<TB_WF2_THREADS, wf2_lq::WF2_MODE_GENERIC>, "wf2_lq.generic"},
-    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_HARD>, "wf2_smem"},
-    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_SPLIT>, "wf2_smem"},
-    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_GENERIC>, "wf2_smem"},
+    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_HARD>, "wf2_smem.hard"},
+    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_SPLIT>, "wf2_smem.split"},
+    {wf2_smem::launch_wavefront2_t<TB_WF2_THREADS, wf2_smem::WF2_MODE_GENERIC>, "wf2_smem.generic"},
 };
 enum { WF2_L2_SPLIT, WF2_L2_GENERIC, WF2_LQ_NONE, WF2_LQ_ALL, WF2_SMEM_HARD, WF2_SMEM_SPLIT, WF2_SMEM_GENERIC };
 
-// Launches the wavefront kernel the launch parameters call for; returns its name (nullptr: nothing to do).  With
-// split = the free-running scheduler with the split trace queue, the first rule that applies chooses:
-//  1. wideCta (768-thread CTAs, scenes with deep mesh BVHs): wf2_l2, SPLIT when split, else GENERIC, which runs
-//     hard phases too (P.hardPhases stays a run-time flag there).
-//  2. The free-running scheduler without the split trace queue, lane queues forced (laneQueues 2) or chosen
-//     (laneQueues 1) and a launch that is not small: wf2_lq, without the scene-feature code when p.specialized.
-//     The lane-owned layout wins in the steady state (cornell 32 spp on an H100: 1131 vs 893 Msamples/s) and loses
-//     while the slots fill and drain (1-spp frames, slabs of a multi-GPU render; measured in round 2): launches of
-//     fewer than six samples per slot are small and keep the rings.  The specialised kernel has 512-thread CTAs
-//     too: at 640 (20 warps, 96 registers) it spills 128 bytes and measured no faster on cornell.
-//  3. Otherwise wf2_smem: HARD when hardPhases, else SPLIT when split, else GENERIC.
-const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
+// Which of the seven kernels runs: every one produces the same bits, so the choice is speed alone.
+// Per scene (wavefront2_route, at upload in tb200_create / tb200_create_cached, reading the knobs then):
+//  * hardPhases = numNee > 1 && maxTris <= 4096 (TINSEL_B200_SCHED=hard|free overrides).  Block-synchronous stages
+//    win when every hit spawns several shadow rays (the barrier keeps all warps on one stage's code); free-running
+//    warps win otherwise, by a wide margin when ray cost varies (deep mesh BVHs).
+//  * wideCta = !hardPhases && maxTris > 4096 (TINSEL_B200_CTA=768|512 overrides): more warps hide the L2 latency of
+//    deep mesh BVHs; on scenes held in shared memory they only thrash the instruction cache.
+//  * The split trace queue (rays entering the largest mesh's box queued apart) is in use when that box exists and
+//    maxTris > 4096 or TINSEL_B200_SPLIT=1, never with TINSEL_B200_SPLIT=0; split = !hardPhases && in use.
+//    tune = split && TINSEL_B200_SPLIT unset: api.cu: tune_update keeps the faster of split on and off.
+//  * laneQueues = 1 (TINSEL_B200_QUEUES=ring: 0, =lanes: 2); specialized = no TB_FEAT_* feature and
+//    TINSEL_B200_SPECIALIZE is not 0.
+// Per launch (launch_wavefront2), with small = fewer than 6 x numSMs x 1024 samples, the first rule that applies:
+//  1. wideCta: wf2_l2.split when split, else wf2_l2.generic (which runs hard phases too: P.hardPhases is read there).
+//  2. !hardPhases, !split, and laneQueues 2, or 1 and not small: wf2_lq.specialized when specialized, else
+//     wf2_lq.generic.  The lane-owned layout wins in the steady state (cornell 32 spp on an H100: 1131 vs 893
+//     Msamples/s) and loses while the slots fill and drain (1-spp frames, slabs of a multi-GPU render; measured in
+//     round 2).  The specialised kernel has 512-thread CTAs too: at 640 (20 warps, 96 registers) it spills 128
+//     bytes and measured no faster on cornell.
+//  3. Otherwise wf2_smem.hard when hardPhases, else wf2_smem.split when split, else wf2_smem.generic.
+Wf2Route wavefront2_route(int numNee, int maxTris, bool splitBox, uint32_t features)
+{
+    const char* sched = getenv("TINSEL_B200_SCHED");
+    const char* split = getenv("TINSEL_B200_SPLIT");
+    const char* cta = getenv("TINSEL_B200_CTA");
+    const char* queues = getenv("TINSEL_B200_QUEUES");
+    const char* spec = getenv("TINSEL_B200_SPECIALIZE");
+    Wf2Route r;
+    r.hardPhases = numNee > 1 && maxTris <= 4096;
+    if (sched && strcmp(sched, "hard") == 0) r.hardPhases = true;
+    if (sched && strcmp(sched, "free") == 0) r.hardPhases = false;
+    r.wideCta = !r.hardPhases && maxTris > 4096;
+    if (cta && atoi(cta) == 768) r.wideCta = true;
+    if (cta && atoi(cta) == 512) r.wideCta = false;
+    const bool splitQueue = splitBox && (maxTris > 4096 || (split && atoi(split) == 1)) && !(split && atoi(split) == 0);
+    r.split = !r.hardPhases && splitQueue;
+    r.tune = r.split && !split;
+    r.laneQueues = !queues ? 1 : strcmp(queues, "ring") == 0 ? 0 : strcmp(queues, "lanes") == 0 ? 2 : 1;
+    r.specialized = features == TB_FEAT_NONE && !(spec && atoi(spec) == 0);
+    return r;
+}
+
+// Launches the kernel the route calls for (see above); returns its name (nullptr: nothing to do).
+const char* launch_wavefront2(const LaunchParams& p, const Wf2Route& route, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
     const unsigned long long total = p.samplesPerFrame * (unsigned long long)p.numFrames;
     if (total == 0ull) return nullptr;
     const bool small = total < 6ull * (unsigned long long)(numSMs > 0 ? numSMs : 132) * 1024ull;
-    const bool split = !p.hardPhases && p.scene.splitValid;
     int k;
-    if (p.wideCta)
-        k = split ? WF2_L2_SPLIT : WF2_L2_GENERIC;
-    else if (!p.hardPhases && !p.scene.splitValid && (p.laneQueues == 2 || (p.laneQueues == 1 && !small)))
-        k = p.specialized ? WF2_LQ_NONE : WF2_LQ_ALL;
+    if (route.wideCta)
+        k = route.split ? WF2_L2_SPLIT : WF2_L2_GENERIC;
+    else if (!route.hardPhases && !route.split && (route.laneQueues == 2 || (route.laneQueues == 1 && !small)))
+        k = route.specialized ? WF2_LQ_NONE : WF2_LQ_ALL;
     else
-        k = p.hardPhases ? WF2_SMEM_HARD : split ? WF2_SMEM_SPLIT : WF2_SMEM_GENERIC;
-    cudaMemsetAsync(p.sampleCounter, 0, sizeof(unsigned long long), stream);
-    kWavefront2[k].launch(p, numSMs, stream, total);
+        k = route.hardPhases ? WF2_SMEM_HARD : route.split ? WF2_SMEM_SPLIT : WF2_SMEM_GENERIC;
+    LaunchParams q = p;
+    q.hardPhases = route.hardPhases;
+    cudaMemsetAsync(q.sampleCounter, 0, sizeof(unsigned long long), stream);
+    kWavefront2[k].launch(q, numSMs, stream, total);
     if (launchCount) ++*launchCount;
     return kWavefront2[k].name;
 }

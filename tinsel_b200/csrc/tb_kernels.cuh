@@ -14,9 +14,7 @@ struct LaunchParams {
     DFilm film;
     float4* accum;        // width*height running sums
     unsigned long long* sampleCounter;   // per-renderer work counter of the wavefront kernel
-    int hardPhases;       // wavefront scheduling mode: 1 = block-synchronous stages, 0 = free-running warps
-    int wideCta;          // 1 = 768-thread CTAs (deep mesh BVHs), 0 = 512
-    int laneQueues;       // lane-owned slots with bit-set stage queues (free-running on-chip scenes): 0 never, 1 for big launches, 2 always
+    int hardPhases;       // wavefront scheduling mode: 1 = block-synchronous stages, 0 = free-running warps (set by launch_wavefront2)
     int frame0;           // first frame (sample index per pixel)
     int numFrames;        // frames to trace in this launch
     int firstRow;         // pixel rows [firstRow, firstRow+numRows) are traced ...
@@ -41,7 +39,16 @@ struct LaunchParams {
     // cold half of the wavefront's slot state: 8 x float4 per slot, TB_WF2_PATHS slots per CTA of the launch
     float4* cold;
     int treeletBytes;     // shared memory behind the slot arrays that the prologue fills with the top of DScene::treeletMesh's BVH
-    int specialized;      // the scene has none of the TB_FEAT_* features: the lane-owned layout runs its instantiation without them
+};
+
+// The per-scene part of the choice of wavefront kernel (kernels.cu: wavefront2_route, launch_wavefront2).
+struct Wf2Route {
+    bool hardPhases;    // block-synchronous stages rather than free-running warps
+    bool wideCta;       // 768-thread CTAs (wf2_l2) rather than 512
+    bool split;         // free-running with the split trace queue; the tuner may change it between launches
+    bool tune;          // the split-queue tuner decides `split` by measurement (api.cu: tune_update)
+    bool specialized;   // no TB_FEAT_* feature: the lane-owned kernel compiled without them
+    int laneQueues;     // lane-owned slots with bit-set queues: 0 never, 1 for launches that are not small, 2 always
 };
 
 #define TB_MAX_BANDS 64
@@ -54,8 +61,10 @@ void divisor_magic(uint32_t d, uint32_t* mul, uint32_t* shift);
 // The launches below return the name of the kernel they ran (nullptr when there was no work), for tb200_last_kernel.
 // one thread per (pixel, frame): the whole path in registers.  Validation / fallback pipeline.
 const char* launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned long long* launchCount);
-// persistent CTA-resident wavefront pipeline with a dedicated traversal stage (the product path)
-const char* launch_wavefront2(const LaunchParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
+// persistent CTA-resident wavefront pipeline with a dedicated traversal stage (the product path), and its route for
+// a scene of numNee shadow rays per hit, largest mesh maxTris triangles (splitBox: its box in DScene), features
+Wf2Route wavefront2_route(int numNee, int maxTris, bool splitBox, uint32_t features);
+const char* launch_wavefront2(const LaunchParams& p, const Wf2Route& route, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds: the per-stage cycle counters of the lane-owned wavefront layout (wf2_lanes.cuh), summed
 // over every launch since the last reset

@@ -131,9 +131,9 @@ struct DScene {
     const struct ProgOp* flat;     // flat scene program (numFlat == 0: use the ordered walk)
     int numFlat;
     // Scheduling hint only (never changes a result): world-space bounds of the scene's largest mesh
-    // when it is big enough for its BVH walk to dominate a ray's cost.  The wavefront kernel queues
-    // rays that enter this box separately from the rest, so that a warp's 32 rays either all walk
-    // the mesh or none does.
+    // (splitValid: splitLo/splitHi hold them).  With the split trace queue (kernels.cu: wavefront2_route) the
+    // wavefront kernel queues rays that enter this box separately from the rest, so that a warp's 32 rays
+    // either all walk the mesh or none does.
     int splitValid;
     V3 splitLo, splitHi;
     // Treelet: the first `treeletPairs` pair records (breadth-first = the top levels) of mesh `treeletMesh`'s BVH,
@@ -144,6 +144,9 @@ struct DScene {
     int treeletPairs;
     int treeletMesh;
 };
+// each CTA of the wavefront kernel copies DScene into its shared memory (Wf2Shared::scene): a change of its size
+// moves the shared-memory layout behind it (one such shift cost veach 1 %)
+static_assert(sizeof(DScene) == 192, "DScene's size moves the wavefront kernel's shared-memory layout");
 
 struct Hit {
     float t;

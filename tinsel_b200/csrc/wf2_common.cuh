@@ -220,7 +220,7 @@ TB_DEV bool wf2_scatter(Wf2SharedBase& S, float4* rec, const DScene& sc, int s, 
 
 // THREADS: 512 (16 warps, up to 128 registers) for scenes held in shared memory, where more warps
 // only add instruction-cache pressure; 768 (24 warps, 80 registers) for scenes with deep mesh BVHs,
-// whose traversal is latency bound on L2 and pays for the extra warps (LaunchParams::wideCta).
+// whose traversal is latency bound on L2 and pays for the extra warps (Wf2Route::wideCta).
 // MODE: the ring-queue kernel's scheduler, compiled in per instantiation because the kernel's speed is sensitive to
 // register allocation and code layout (measured in round 2); the lane-owned kernel takes GENERIC.
 //   WF2_MODE_GENERIC  both schedulers, run-time flag, no split trace queue (the free-running default;

@@ -28,9 +28,9 @@ enum { CC_SH = 4, CC_SUM = 5, CC_LA = 6, CC_CHUNKS = 8 };
 #endif
 
 // stage queues.  T, A, B, R in the cyclic order of the free-running sweep; F0/F1 hold the freshly regenerated camera
-// rays in hard-phase mode (double-buffered: R fills one while T drains the other).  TM (free-running mode, scenes
-// with DScene::splitValid): rays that enter the big mesh's box; same stage code as T, but a chunk taken from TM
-// walks the mesh with all of its lanes and a chunk taken from T with none.
+// rays in hard-phase mode (double-buffered: R fills one while T drains the other).  TM (WF2_MODE_SPLIT): rays
+// that enter the big mesh's box; same stage code as T, but a chunk taken from TM walks the mesh with all of its
+// lanes and a chunk taken from T with none.
 enum { WF2_Q_T = 0, WF2_Q_A = 1, WF2_Q_B = 2, WF2_Q_R = 3, WF2_Q_F0 = 4, WF2_Q_F1 = 5, WF2_Q_TM = 6 };
 
 struct Wf2Shared : Wf2SharedBase {
