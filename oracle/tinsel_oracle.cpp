@@ -1095,6 +1095,25 @@ void oracle_bsdf_sample(const tb200_material* m, float etaI, float etaO, const f
     rngAfter[0] = rng.a;
     rngAfter[1] = rng.b;
 }
+// oracle_bsdf_eval and oracle_bsdf_sample over n cases (tests/test_bsdf_gpu.py: CASE_DTYPE, REF_DTYPE)
+struct oracle_bsdf_case {
+    int32_t mat, seed;
+    float etaI, etaO, n[3], v[3], l[3];
+};
+struct oracle_bsdf_result {
+    float f[3], pdf, light[3], spdf;
+    int32_t type;
+    uint32_t rng[2];
+};
+void oracle_bsdf_cases(const tb200_material* mats, const oracle_bsdf_case* cases, int n, oracle_bsdf_result* out)
+{
+    for (int k = 0; k < n; ++k) {
+        const oracle_bsdf_case& c = cases[k];
+        oracle_bsdf_result& r = out[k];
+        oracle_bsdf_eval(&mats[c.mat], c.etaI, c.etaO, c.n, c.v, c.l, r.f, &r.pdf);
+        oracle_bsdf_sample(&mats[c.mat], c.etaI, c.etaO, c.n, c.v, c.seed, r.light, &r.spdf, &r.type, r.rng);
+    }
+}
 void oracle_generate_ray(const tb200_camera* c, int width, int height, float x, float y, float* origin, float* dir)
 {
     camera_t cs = make_camera(*c, width, height);

@@ -12,22 +12,14 @@ The cases are drawn from the edges where the splat can go wrong: raster position
 where int(raster +- width) flips, widths on and beside 1, steep and degenerate falloffs, offsets outside (0, 1),
 clamps of 0 and NaN, samples whose length or weighted value overflows, non-finite channels, tiny films and slabs."""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import tinsel_b200 as tb
-from tinsel_b200 import abi, build
+from tinsel_b200 import abi
+import cuda_harness
 import refdrv
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HARNESS = os.path.join(ROOT, "tests", "splat_harness.cu")
-CSRC = os.path.join(ROOT, "tinsel_b200", "csrc")
-DEPS = [HARNESS] + [os.path.join(CSRC, h) for h in build.HEADERS] + [os.path.join(ROOT, "include", h) for h in ("tinsel_b200.h", "tb200_detmath.h")]
 
 # struct SplatCase in splat_harness.cu
 CASE_DTYPE = np.dtype([("width", "<i4"), ("height", "<i4"), ("filterType", "<i4"), ("rowLo", "<i4"), ("rowHi", "<i4"),
@@ -45,24 +37,8 @@ INF = F32(np.inf)
 # ---- the harness ----
 
 
-def _compile_cmd(out):
-    return [build._nvcc(), "-ccbin", build._host_compiler(), *build.NVCC_FLAGS, "-I", os.path.join(ROOT, "include"),
-            "-I", CSRC, "-shared", "-o", out, HARNESS, "-lcudart"]
-
-
 def harness_path():
-    """The harness library, compiled on first use into a temporary directory keyed by its sources and flags (the
-    repository tree may be read-only)."""
-    h = hashlib.sha1(" ".join(_compile_cmd("")).encode())
-    for p in DEPS:
-        with open(p, "rb") as f:
-            h.update(f.read())
-    path = os.path.join(tempfile.gettempdir(), "tinsel_b200_splat_%s.so" % h.hexdigest()[:16])
-    if not os.path.exists(path):
-        tmp = "%s.%d.tmp" % (path, os.getpid())
-        subprocess.check_call(_compile_cmd(tmp))
-        os.replace(tmp, path)
-    return path
+    return cuda_harness.harness_path("splat_harness")
 
 
 _harness = None

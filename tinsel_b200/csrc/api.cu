@@ -70,48 +70,6 @@ Xf to_xf(const tb200_transform& t)
     return x;
 }
 
-// Per-material constants.  The double intermediates are the reference's own (SURVEY.md 7.2c):
-//   GetIndexOfRefraction  scene.h:72-78    2.0f/(1.0f-sqrtf(0.08*specular)) - 1.0f
-//   Cdlum                 disney.h:307     .3*r + .6*g + .1*b   (double, rounded to float)
-//   Ctint, Cspec0         disney.h:309-310 specular*.08 is a double product converted to Real
-//   clearcoat alpha       disney.h:387     Lerp(.1,.001,gloss) in double, converted to float
-DMaterial make_material(const tb200_material& m)
-{
-    DMaterial d;
-    d.emission = hv3(m.emission);
-    d.color = hv3(m.color);
-    d.absorption = hv3(m.absorption);
-    d.metallic = m.metallic;
-    d.subsurface = m.subsurface;
-    d.specular = m.specular;
-    d.roughness = m.roughness;
-    d.specularTint = m.specularTint;
-    d.clearcoat = m.clearcoat;
-    d.clearcoatGloss = m.clearcoatGloss;
-    d.transmission = m.transmission;
-
-    if (m.eta == 0.0f)
-        d.ior = 2.0f / (1.0f - sqrtf(float(0.08 * double(m.specular)))) - 1.0f;
-    else
-        d.ior = m.eta;
-
-    const float Cdlum = float(.3 * double(m.color[0]) + .6 * double(m.color[1]) + .1 * double(m.color[2]));
-    const V3 Cdlin = d.color;
-    const V3 Ctint = Cdlum > 0.0f ? Cdlin / Cdlum : v3s(1.0f);
-    const float spec08 = float(double(m.specular) * .08);
-    d.cspec0 = tb_lerp(spec08 * tb_lerp(v3s(1.0f), Ctint, m.specularTint), Cdlin, m.metallic);
-
-    d.sqrtColor = v3(sqrtf(m.color[0]), sqrtf(m.color[1]), sqrtf(m.color[2]));
-    d.alpha = tb_max(0.001f, m.roughness);
-
-    const float a = float(.1 + (.001 - .1) * double(m.clearcoatGloss));
-    d.gtr1Wide = (a >= 1) ? 1 : 0;
-    const float a2 = a * a;
-    d.gtr1A2m1 = a2 - 1;
-    d.gtr1PiLogA2 = TB_PI * logf(a2);
-    return d;
-}
-
 // BVHNode[] (bvh.h:9-19) -> BvhPair[]; see tb_scene.cuh.  Returns the root reference.  Pairs are laid out
 // in breadth-first order from the root, so that the first K records are the top of the tree: the treelet
 // (DScene::treelet) stages exactly that prefix in shared memory with bulk copies, and the upper levels
@@ -518,6 +476,7 @@ bool image_from_scene(const tb200_scene* s, SceneImage* img)
         d.mat = make_material(p.material);
         if (p.lightSamples > 0) img->numNee += p.lightSamples;
     }
+    set_fresnel_flags(img->prims.size(), [&](size_t i) -> DMaterial& { return img->prims[i].mat; });
     img->sceneRoot = build_pairs(s->bvhNodes, s->numBvhNodes, &img->scenePairs);
     build_program(s, &img->flat);
     img->horizon = hv3(s->sky.horizon);
@@ -544,17 +503,13 @@ bool image_from_scene(const tb200_scene* s, SceneImage* img)
 }
 
 // The scene's features (tb_scene.cuh: TB_FEAT_*).  A scene without any of them runs the lane-owned kernel compiled
-// without them (kernels.cu: launch_wavefront2); a NaN parameter counts as present.
+// without them (kernels.cu: launch_wavefront2).
 uint32_t scene_features(const SceneImage& img)
 {
     uint32_t f = img.probeValid ? TB_FEAT_PROBE : TB_FEAT_NONE;
     for (const DPrim& p : img.prims) {
-        const DMaterial& m = p.mat;
         if (!p.isStatic) f |= TB_FEAT_MOTION;
-        if (m.transmission != 0.0f) f |= TB_FEAT_TRANSMISSION;
-        if (m.subsurface != 0.0f) f |= TB_FEAT_SUBSURFACE;
-        if (m.clearcoat != 0.0f) f |= TB_FEAT_CLEARCOAT;
-        if (m.absorption.x != 0.0f || m.absorption.y != 0.0f || m.absorption.z != 0.0f) f |= TB_FEAT_ABSORPTION;
+        f |= material_features(p.mat);
     }
     return f;
 }
@@ -660,7 +615,7 @@ bool build_scene(tb200_renderer* r, const tb200_scene* s)
 // a stamp mismatch is refused and the caller falls back to tb200_create), then the SceneImage fields in
 // declaration order; every array as a 64-bit count followed by its bytes.
 const char kCacheMagic[8] = {'T', 'B', '2', 'C', 'A', 'C', 'H', 'E'};
-const uint32_t kCacheVersion = 2;
+const uint32_t kCacheVersion = 3;   // 3: DMaterial::flags
 
 struct CacheStamp {
     uint32_t version, sizeofPrim, sizeofPair, sizeofOp;

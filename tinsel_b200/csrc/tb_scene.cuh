@@ -70,6 +70,14 @@ struct __align__(16) BvhPair {
     uint32_t pad0, pad1;
 };
 
+// DMaterial::flags.  The two skips are decided on the host (make_material, set_fresnel_flags), because whether
+// they are exact depends on parameter values the loader accepts without checking.
+enum : uint32_t {
+    TB_MAT_GTR1_WIDE = 1u << 0,     // clearcoat alpha >= 1: GTR1 returns kInvPi (disney.h:58)
+    TB_MAT_NO_CLEARCOAT = 1u << 1,  // BSDFEval may skip the clearcoat lobe (tb_shade.cuh: bsdf_eval)
+    TB_MAT_NO_FRESNEL = 1u << 2,    // BSDFPdf may skip Fr for a front-facing view (tb_shade.cuh: bsdf_pdf)
+};
+
 struct DMaterial {
     V3 emission;
     V3 color;
@@ -83,7 +91,7 @@ struct DMaterial {
     float alpha;          // Max(0.001f, roughness), disney.h:139
     float gtr1A2m1;       // a2-1 for the clearcoat GTR1, disney.h:61-63,387
     float gtr1PiLogA2;    // kPi*logf(a2)
-    int gtr1Wide;         // a >= 1 -> GTR1 returns kInvPi
+    uint32_t flags;       // TB_MAT_*
 };
 
 struct DMesh {
@@ -163,12 +171,97 @@ enum : uint32_t {
     TB_FEAT_NONE = 0u,
     TB_FEAT_PROBE = 1u << 0,          // the sky has an environment probe
     TB_FEAT_MOTION = 1u << 1,         // a primitive moves (start != end transform)
-    TB_FEAT_TRANSMISSION = 1u << 2,   // a material has transmission != 0
+    TB_FEAT_TRANSMISSION = 1u << 2,   // a material has transmission != 0, or BSDFPdf must evaluate Fr for it
     TB_FEAT_SUBSURFACE = 1u << 3,     // a material has subsurface != 0
-    TB_FEAT_CLEARCOAT = 1u << 4,      // a material has clearcoat != 0
+    TB_FEAT_CLEARCOAT = 1u << 4,      // a material has clearcoat != 0, or a clearcoat lobe that is not finite
     TB_FEAT_ABSORPTION = 1u << 5,     // a material has a non-zero absorption component
     TB_FEAT_ALL = (1u << 6) - 1u,
 };
+
+// ---- per-material constants (host side; api.cu and tests/bsdf_harness.cu) ---------------------------------
+
+// The double intermediates are the reference's own (SURVEY.md 7.2c):
+//   GetIndexOfRefraction  scene.h:72-78    2.0f/(1.0f-sqrtf(0.08*specular)) - 1.0f
+//   Cdlum                 disney.h:307     .3*r + .6*g + .1*b   (double, rounded to float)
+//   Ctint, Cspec0         disney.h:309-310 specular*.08 is a double product converted to Real
+//   clearcoat alpha       disney.h:387     Lerp(.1,.001,gloss) in double, converted to float
+// Sets every flag but TB_MAT_NO_FRESNEL, which depends on the whole scene (set_fresnel_flags).
+inline DMaterial make_material(const tb200_material& m)
+{
+    DMaterial d;
+    d.emission = v3(m.emission[0], m.emission[1], m.emission[2]);
+    d.color = v3(m.color[0], m.color[1], m.color[2]);
+    d.absorption = v3(m.absorption[0], m.absorption[1], m.absorption[2]);
+    d.metallic = m.metallic;
+    d.subsurface = m.subsurface;
+    d.specular = m.specular;
+    d.roughness = m.roughness;
+    d.specularTint = m.specularTint;
+    d.clearcoat = m.clearcoat;
+    d.clearcoatGloss = m.clearcoatGloss;
+    d.transmission = m.transmission;
+
+    if (m.eta == 0.0f)
+        d.ior = 2.0f / (1.0f - sqrtf(float(0.08 * double(m.specular)))) - 1.0f;
+    else
+        d.ior = m.eta;
+
+    const float Cdlum = float(.3 * double(m.color[0]) + .6 * double(m.color[1]) + .1 * double(m.color[2]));
+    const V3 Cdlin = d.color;
+    const V3 Ctint = Cdlum > 0.0f ? Cdlin / Cdlum : v3s(1.0f);
+    const float spec08 = float(double(m.specular) * .08);
+    d.cspec0 = tb_lerp(spec08 * tb_lerp(v3s(1.0f), Ctint, m.specularTint), Cdlin, m.metallic);
+
+    d.sqrtColor = v3(sqrtf(m.color[0]), sqrtf(m.color[1]), sqrtf(m.color[2]));
+    d.alpha = tb_max(0.001f, m.roughness);
+
+    const float a = float(.1 + (.001 - .1) * double(m.clearcoatGloss));
+    const float a2 = a * a;
+    d.gtr1A2m1 = a2 - 1;
+    d.gtr1PiLogA2 = TB_PI * logf(a2);
+    d.flags = (a >= 1) ? TB_MAT_GTR1_WIDE : 0u;
+    // The clearcoat lobe is clearcoat*Gr*Fc*Dr.  With NDotL > 0 and NDotV >= 0, Gr and Fc are finite, so with
+    // clearcoat == 0 the lobe is +-0 -- and adding it changes at most the sign of a zero -- iff Dr = GTR1(NDotH) is
+    // finite.  The wide branch is kInvPi.  Otherwise Dr = (a2-1) / (kPi*logf(a2) * t), t = 1 + (a2-1)*NDotH^2,
+    // needs a finite a2 != 1 (logf(a2) == 0 at 1) and t > 0 for every NDotH^2 up to 1 plus the rounding of unit
+    // vectors (2^-20 bounds it): a2 > 1 gives t >= 1; for a2 < 1, t is smallest at the largest NDotH^2, and a tiny
+    // a2 -- a gloss near 1/.99, where the alpha crosses 0 -- makes it 0 there and Dr infinite.
+    const float t = 1 + d.gtr1A2m1 * 1.00000095367431640625f;   // 1 + 2^-20
+    const bool gtr1Finite = (d.flags & TB_MAT_GTR1_WIDE) || (a2 <= FLT_MAX && a2 != 1.0f && (a2 > 1.0f || t > 0.0f));
+    if (m.clearcoat == 0.0f && gtr1Finite) d.flags |= TB_MAT_NO_CLEARCOAT;
+    return d;
+}
+
+// Fr(VDotN, etaI, etaT) is finite for every VDotN > 0 when both etas lie in [1/256, 256]: the squared ratio and
+// eta*LDotN stay below 2^32, and no denominator of r1 or r2 can be 0.  A path's etaI and etaO are 1 or the ior of
+// some material of the scene (path_hit), so the bound is a property of the scene, not of one material.  Outside
+// it Fr can be NaN or infinite (a NaN, infinite, zero or negative ior: eta == 0 with specular < 0 or >= 12.5).
+inline bool ior_fresnel_safe(float ior) { return ior >= 1.0f / 256.0f && ior <= 256.0f; }
+
+// Sets TB_MAT_NO_FRESNEL on the materials of one scene: BSDFPdf's `Lerp(brdfPdf, pdfSpec*F, transmission)` is
+// brdfPdf plus (finite)*0 -- so Fr may be skipped -- when transmission == 0 and F is finite.  mat(i) returns a
+// reference to the scene's i-th DMaterial.
+template <class Mat>
+inline void set_fresnel_flags(size_t n, Mat mat)
+{
+    bool safe = true;
+    for (size_t i = 0; i < n; ++i) safe = safe && ior_fresnel_safe(mat(i).ior);
+    for (size_t i = 0; i < n; ++i)
+        if (safe && mat(i).transmission == 0.0f) mat(i).flags |= TB_MAT_NO_FRESNEL;
+}
+
+// The material's part of a scene's features (api.cu: scene_features); a NaN parameter counts as present.  The
+// kernel compiled without transmission and clearcoat skips Fr and the clearcoat lobe unconditionally, so a
+// material counts as having them unless both skips are exact (each flag implies transmission resp. clearcoat 0).
+inline uint32_t material_features(const DMaterial& m)
+{
+    uint32_t f = TB_FEAT_NONE;
+    if (!(m.flags & TB_MAT_NO_FRESNEL)) f |= TB_FEAT_TRANSMISSION;
+    if (m.subsurface != 0.0f) f |= TB_FEAT_SUBSURFACE;
+    if (!(m.flags & TB_MAT_NO_CLEARCOAT)) f |= TB_FEAT_CLEARCOAT;
+    if (m.absorption.x != 0.0f || m.absorption.y != 0.0f || m.absorption.z != 0.0f) f |= TB_FEAT_ABSORPTION;
+    return f;
+}
 
 template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV Xf prim_transform(const DPrim& p, float time)

@@ -32,7 +32,7 @@ TB_DEV float gtr2(float NDotH, float a)
 // GTR1 with the material-constant parts hoisted, disney.h:56-62
 TB_DEV float gtr1_clearcoat(const DMaterial& m, float NDotH)
 {
-    if (m.gtr1Wide) return TB_INV_PI;
+    if (m.flags & TB_MAT_GTR1_WIDE) return TB_INV_PI;
     const float t = 1 + m.gtr1A2m1 * NDotH * NDotH;
     return m.gtr1A2m1 / (m.gtr1PiLogA2 * t);
 }
@@ -86,10 +86,10 @@ TB_DEV float bsdf_pdf(const DMaterial& mat, float etaI, float etaO, V3 n, V3 V, 
     const float pdfSpec = 0.25f * pdfHalf / tb_max(1.e-6f, dot(L, half));
     const float pdfDiff = tb_abs(dot(L, n)) * TB_INV_PI * (1.0f - mat.subsurface);
     const float brdfPdf = tb_lerp(pdfDiff, pdfSpec, 0.5f);
-    // Lerp(brdfPdf, pdfSpec*F, transmission): with transmission == 0 and a front-facing view the
-    // Fresnel term is finite (both denominators of Fr are positive), so the lerp adds
-    // (finite)*0 = +-0 and returns brdfPdf unchanged; Fr is skipped then.
-    if ((!(FEAT & TB_FEAT_TRANSMISSION) || mat.transmission == 0.0f) && NV > 0.0f) return brdfPdf;
+    // Lerp(brdfPdf, pdfSpec*F, transmission): with transmission == 0, a front-facing view and every ior of the
+    // scene in the range where Fr is finite (TB_MAT_NO_FRESNEL, tb_scene.cuh: set_fresnel_flags), the lerp adds
+    // (finite)*0 = +-0 and returns brdfPdf up to the sign of a zero; Fr is skipped then.
+    if ((!(FEAT & TB_FEAT_TRANSMISSION) || (mat.flags & TB_MAT_NO_FRESNEL)) && NV > 0.0f) return brdfPdf;
     const float F = fresnel_dielectric(NV, etaI, etaO);
     const float bsdfPdf = pdfSpec * F;
     return tb_lerp(brdfPdf, bsdfPdf, mat.transmission);
@@ -143,10 +143,10 @@ TB_DEV V3 bsdf_eval(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3
             const float Fd = tb_lerp(1.0f, Fd90, FL) * tb_lerp(1.0f, Fd90, FV);
 
             brdf = TB_INV_PI * Fd * mat.color * (1.0f - mat.metallic) * (1.0f - mat.subsurface) + Gs * Fs * Ds;
-            // clearcoat lobe: `+ mat.clearcoat*Gr*Fc*Dr`.  With clearcoat == 0 the term is 0*finite = +-0
-            // (Gr, Fc, Dr are finite here: NDotL > 0, alpha in [.001,.1]) and adding it changes at most
-            // the sign of a zero, which no branch or sum downstream can observe; skip the lobe then.
-            if ((FEAT & TB_FEAT_CLEARCOAT) && mat.clearcoat != 0.0f) {
+            // clearcoat lobe: `+ mat.clearcoat*Gr*Fc*Dr`.  With clearcoat == 0 and a finite GTR1 (TB_MAT_NO_CLEARCOAT,
+            // tb_scene.cuh: make_material) the term is 0*finite = +-0 and adding it changes at most the sign of a
+            // zero, which no branch or sum downstream can observe; skip the lobe then.
+            if ((FEAT & TB_FEAT_CLEARCOAT) && !(mat.flags & TB_MAT_NO_CLEARCOAT)) {
                 const float Dr = gtr1_clearcoat(mat, NDotH);
                 const float Fc = tb_lerp(.04f, 1.0f, FH);
                 const float Gr = smith_ggx(NDotL, .25f) * smith_ggx(NDotV, .25f);
