@@ -40,7 +40,7 @@ def _port(path):
 def _trace(path, frame=2):
     """Per-sample radiance and raster position of one frame on the GPU, and the name of the kernel that traced it.
     The lane-owned kernel carries each sample's raster position in its slot from the sample's generation to its
-    splat (wf2_lanes.cuh: wf2_lq_stage_r), past every stage that must leave it alone."""
+    splat (wf2_common.cuh: wf2_stage_r, wf2_lanes.cuh: wf2_splat), past every stage that must leave it alone."""
     snap = tb.Snapshot(path)
     cam, opt = snap.camera, snap.options
     opt.width, opt.height = SIZE

@@ -35,8 +35,8 @@ enum { WF2_PH_EXT = 0, WF2_PH_NEE = 1 };
 
 // Cold half of a slot's state: 16-byte chunks, one record per slot, accessed by the one lane that owns the slot at
 // the time (ownership moves through the stage queues, whose pushes are preceded by a block-scope fence).  Chunks 0-3:
-//   0: T.xyz, eta        1: L.xyz, bsdfPdf     2: absorption.xyz, sample index     3: rng1, rng2 (.zw: layout's own;
-// the lane-owned layout keeps the sample's raster position there)
+//   0: T.xyz, eta        1: L.xyz, bsdfPdf     2: absorption.xyz, sample index     3: rng1, rng2, raster x, y (stage
+// R's generation stores the sample's raster position in .zw; the ring layout overwrites it with NEE bookkeeping)
 // TB_WF2_COLD_SMEM: the records live in shared memory (Wf2Shared::cold); otherwise in global memory (P.cold),
 // read with ld.global.cg / written with st.global.cg.
 enum { CC_T = 0, CC_L = 1, CC_A = 2, CC_RNG = 3 };
@@ -213,7 +213,7 @@ TB_DEV bool wf2_scatter(Wf2SharedBase& S, float4* rec, const DScene& sc, int s, 
     S.dx[s] = ps.d.x; S.dy[s] = ps.d.y; S.dz[s] = ps.d.z;
     cold_st(rec, CC_T, ps.T.x, ps.T.y, ps.T.z, ps.eta);
     cold_st(rec, CC_A, ps.absorb.x, ps.absorb.y, ps.absorb.z, u2f(sample));
-    cold_st2(rec, CC_RNG, u2f(ps.rng.s1), u2f(ps.rng.s2));   // .zw: the layout's own
+    cold_st2(rec, CC_RNG, u2f(ps.rng.s1), u2f(ps.rng.s2));   // .zw left alone: the lane-owned splat reads the raster position there
     S.flags[s] = ((uint32_t)ps.rayType << 1) | ((uint32_t)WF2_PH_EXT << 3) | ((uint32_t)(bounce + 1) << 8);
     return true;
 }
@@ -318,36 +318,49 @@ TB_DEV void wf2_await_scene(Shared& S)
                      : "memory");
 }
 
+// stage R's parts, timed separately in the clock build (tools/stage_clocks.py)
+enum { WF2_R_SPLAT = 0, WF2_R_CLAIM = 1, WF2_R_REGEN = 2, WF2_R_PARTS = 3 };
+#ifdef TB_WF2_STAGE_CLOCKS
+// (at a point where the warp has converged, so that lane 0's clock, the one counted, includes every lane's work)
+TB_DEV unsigned int wf2_now()
+{
+    __syncwarp();
+    return (unsigned int)clock64();
+}
+#else
+TB_DEV unsigned int wf2_now() { return 0u; }
+#endif
+
+// Splat finished sample `doneSample` (cold record `rec`, its chunk CC_L in cl) into the accumulator, defined by the
+// layout's own header: the splat is the one part of stage R the layouts do differently.
+TB_DEV void wf2_splat(const LaunchParams& P, const float4* rec, float4 cl, uint32_t doneSample);
+
 // Stage R, by a whole warp (`active` lanes hold slot s, cold record `rec`): splat the finished sample, claim a new one
 // and generate its camera ray.  Returns true where one was; the caller pushes those, then wf2_retire()s the others.
-// The ring kernels' stage R; the lane-owned kernel has its own (wf2_lanes.cuh: wf2_lq_stage_r).
+// rparts: the cycles of each part (WF2_R_*) add up there in the clock build.
 template <class Shared>
-TB_DEV bool wf2_stage_r(Shared& S, const LaunchParams& P, unsigned long long total, float4* rec, int s, bool active)
+TB_DEV bool wf2_stage_r(Shared& S, const LaunchParams& P, unsigned long long total, float4* rec, int s, bool active,
+                        unsigned int (&rparts)[WF2_R_PARTS])
 {
+    const unsigned int t0 = wf2_now();
     const int lane = threadIdx.x & 31;
     const bool finished = active && !(S.flags[s] & WF2_FLAG_EMPTY);
     uint32_t doneSample = 0xffffffffu;
     if (finished) {
         const float4 cl = cold_ld(rec, CC_L), ca = cold_ld(rec, CC_A);
         doneSample = f2u(ca.w);
-        int px, py, frame;
-        decode_sample(P, (unsigned long long)doneSample, px, py, frame);
-        // raster position of the sample: its first two RNG draws (render.cpp:476,481-482)
-        Rng rr = rng_seed(tb_sample_seed((uint32_t)(py * P.film.width + px), (uint32_t)frame));
-        float rx = rng_float(rr);
-        float ry = rng_float(rr);
-        rx += px;
-        ry += py;
-        sample_end(P, px, py, rx, ry, v3(cl.x, cl.y, cl.z));
+        wf2_splat(P, rec, cl, doneSample);
     }
     if (P.bandFlags)
         wf2_band_report(P.bandCount, P.bandFlags, P.bandSamples, (uint32_t)P.samplesPerFrame, P.bandTag, doneSample, finished);
     if (active) S.flags[s] = WF2_FLAG_EMPTY;
+    rparts[WF2_R_SPLAT] += wf2_now() - t0;
     // claim a new sample; indices on tile padding outside the image are skipped
     bool want = active && !*(volatile int*)&S.exhausted;
     bool fresh = false;
     for (int attempt = 0; attempt < 64; ++attempt) {
         if (!__any_sync(0xffffffffu, want)) break;
+        const unsigned int t1 = wf2_now();
         const unsigned m = __ballot_sync(0xffffffffu, want);
         const int leader = __ffs(m) - 1;
         unsigned long long base = 0ull;
@@ -357,6 +370,8 @@ TB_DEV bool wf2_stage_r(Shared& S, const LaunchParams& P, unsigned long long tot
         }
         base = __shfl_sync(0xffffffffu, base, leader);
         const unsigned long long idx = base + (unsigned long long)__popc(m & ((1u << lane) - 1u));
+        const unsigned int t2 = wf2_now();
+        rparts[WF2_R_CLAIM] += t2 - t1;
         if (want) {
             if (idx >= total) {
                 want = false;
@@ -372,7 +387,7 @@ TB_DEV bool wf2_stage_r(Shared& S, const LaunchParams& P, unsigned long long tot
                     cold_st(rec, CC_T, 1.0f, 1.0f, 1.0f, 1.0f);                     // throughput 1, eta 1
                     cold_st(rec, CC_L, 0.0f, 0.0f, 0.0f, 1.0f);                     // radiance 0, bsdfPdf 1
                     cold_st(rec, CC_A, 0.0f, 0.0f, 0.0f, u2f((uint32_t)idx));      // no absorption, the sample index
-                    cold_st(rec, CC_RNG, u2f(ps.rng.s1), u2f(ps.rng.s2), 0.0f, 0.0f);
+                    cold_st(rec, CC_RNG, u2f(ps.rng.s1), u2f(ps.rng.s2), rx, ry);      // the RNG, the raster position
                     S.flags[s] = ((uint32_t)TB_REFLECTED << 1) | ((uint32_t)WF2_PH_EXT << 3);
                     fresh = true;
                     want = false;
@@ -382,6 +397,7 @@ TB_DEV bool wf2_stage_r(Shared& S, const LaunchParams& P, unsigned long long tot
                 }
             }
         }
+        rparts[WF2_R_REGEN] += wf2_now() - t2;
     }
     return fresh;
 }

@@ -9,7 +9,8 @@
 // coherence: those keep the ring queues (wf2_rings.cuh).
 //
 // There is no stage B: stage A shades the whole bounce in place, in k_mega's order (see there), so no shadow ray
-// ever waits in a slot and stage T only traces extension rays.
+// ever waits in a slot and stage T only traces extension rays.  Stage R is the common one (wf2_stage_r); only its
+// splat (wf2_splat, below) is this layout's own.
 
 #ifndef TB_WF2_COLD_SMEM
 #error "the lane-owned layout keeps the cold state in shared memory"
@@ -97,26 +98,13 @@ TB_DEV unsigned wf2_claim_fullest(Wf2Shared& S, int stick, int& slot, int& stage
     }
 }
 
-// stage R's parts, timed separately in the clock build (tools/stage_clocks.py)
-enum { WF2_R_SPLAT = 0, WF2_R_CLAIM = 1, WF2_R_REGEN = 2, WF2_R_PARTS = 3 };
-#ifdef TB_WF2_STAGE_CLOCKS
-// (at a point where the warp has converged, so that lane 0's clock, the one counted, includes every lane's work)
-TB_DEV unsigned int wf2_now()
-{
-    __syncwarp();
-    return (unsigned int)clock64();
-}
-#else
-TB_DEV unsigned int wf2_now() { return 0u; }
-#endif
-
 #ifdef TB_WF2_STAGE_CLOCKS
 // Per-stage cycle accounting (development builds with -DTB_WF2_STAGE_CLOCKS, read by tb200_stage_clocks, see
 // tools/stage_clocks.py).  Every warp sums clock64() deltas in registers and adds its totals here when it exits.
 // Stage kinds k: 0 R, 1 T, 2 A, 3 B (no B in this kernel: its counters stay 0).
 //   [0] claims that got slots   [1] idle: empty claims and the back-off   [2 + k] cycles in stage k
 //   [6 + k] chunks of stage k   [10 + k] lanes active in those chunks      [14] warps
-//   [15 + p] stage R's cycles in part p: WF2_R_SPLAT, WF2_R_CLAIM, WF2_R_REGEN (see wf2_lq_stage_r)
+//   [15 + p] stage R's cycles in part p: WF2_R_SPLAT, WF2_R_CLAIM, WF2_R_REGEN (see wf2_stage_r)
 enum { WF2_CLK_CLAIM = 0, WF2_CLK_IDLE = 1, WF2_CLK_CYCLES = 2, WF2_CLK_CHUNKS = 6, WF2_CLK_LANES = 10, WF2_CLK_WARPS = 14, WF2_CLK_R_PARTS = 15,
        WF2_CLK_N = 18 };
 static_assert(WF2_CLK_N == TB_WF2_STAGE_CLOCK_WORDS, "tb_kernels.cuh states the counter count");
@@ -168,80 +156,19 @@ void wf2_stage_clocks(unsigned long long* out, bool reset)
 }
 #endif
 
-// Stage R, by a whole warp (`active` lanes hold slot s, cold record `rec`): splat the finished sample, claim a new one
-// and generate its camera ray.  Returns true where one was; the caller pushes those, then wf2_retire()s the others.
-// rparts: the cycles of each part (WF2_R_*) add up there in the clock build.  Unlike the ring kernels' stage R
-// (wf2_stage_r), the splat neither decodes the sample index nor draws the raster position again: the slot's RNG
-// chunk carries it in .zw from the sample's generation (wf2_scatter leaves .zw alone), and add_sample_small
-// weighs a 3x3 footprint with one filter evaluation per column and per row.
-TB_DEV bool wf2_lq_stage_r(Wf2Shared& S, const LaunchParams& P, unsigned long long total, float4* rec, int s, bool active,
-                           unsigned int (&rparts)[WF2_R_PARTS])
+// The lane-owned splat (stage R: wf2_stage_r).  It neither decodes the sample index nor draws the raster position
+// again: the slot's RNG chunk carries it in .zw from the sample's generation (wf2_scatter leaves .zw alone), and
+// add_sample_small weighs a 3x3 footprint with one filter evaluation per column and per row.
+TB_DEV void wf2_splat(const LaunchParams& P, const float4* rec, float4 cl, uint32_t doneSample)
 {
-    const unsigned int t0 = wf2_now();
-    const int lane = threadIdx.x & 31;
-    const bool finished = active && !(S.flags[s] & WF2_FLAG_EMPTY);
-    uint32_t doneSample = 0xffffffffu;
-    if (finished) {
-        // the raster position was kept in the RNG chunk when the sample was generated
-        const float4 cl = cold_ld(rec, CC_L), ca = cold_ld(rec, CC_A), cr = cold_ld(rec, CC_RNG);
-        doneSample = f2u(ca.w);
-        if (P.outRadiance) {
-            int px, py, frame;
-            decode_sample(P, (unsigned long long)doneSample, px, py, frame);
-            sample_end(P, px, py, cr.z, cr.w, v3(cl.x, cl.y, cl.z));
-        } else {
-            add_sample_small(P.film, P.accum, cr.z, cr.w, v3(cl.x, cl.y, cl.z));
-        }
+    const float4 cr = cold_ld(rec, CC_RNG);
+    if (P.outRadiance) {
+        int px, py, frame;
+        decode_sample(P, (unsigned long long)doneSample, px, py, frame);
+        sample_end(P, px, py, cr.z, cr.w, v3(cl.x, cl.y, cl.z));
+    } else {
+        add_sample_small(P.film, P.accum, cr.z, cr.w, v3(cl.x, cl.y, cl.z));
     }
-    if (P.bandFlags)
-        wf2_band_report(P.bandCount, P.bandFlags, P.bandSamples, (uint32_t)P.samplesPerFrame, P.bandTag, doneSample, finished);
-    if (active) S.flags[s] = WF2_FLAG_EMPTY;
-    rparts[WF2_R_SPLAT] += wf2_now() - t0;
-    // claim a new sample; indices on tile padding outside the image are skipped
-    bool want = active && !*(volatile int*)&S.exhausted;
-    bool fresh = false;
-    for (int attempt = 0; attempt < 64; ++attempt) {
-        if (!__any_sync(0xffffffffu, want)) break;
-        const unsigned int t1 = wf2_now();
-        const unsigned m = __ballot_sync(0xffffffffu, want);
-        const int leader = __ffs(m) - 1;
-        unsigned long long base = 0ull;
-        if (lane == leader) {
-            base = atomicAdd(P.sampleCounter, (unsigned long long)__popc(m));
-            if (base + __popc(m) >= total) *(volatile int*)&S.exhausted = 1;
-        }
-        base = __shfl_sync(0xffffffffu, base, leader);
-        const unsigned long long idx = base + (unsigned long long)__popc(m & ((1u << lane) - 1u));
-        const unsigned int t2 = wf2_now();
-        rparts[WF2_R_CLAIM] += t2 - t1;
-        if (want) {
-            if (idx >= total) {
-                want = false;
-            } else {
-                int px, py, frame;
-                if (decode_sample(P, idx, px, py, frame)) {
-                    PathState ps;
-                    float rx, ry;
-                    sample_begin(P, px, py, frame, ps, rx, ry);
-                    S.ox[s] = ps.o.x; S.oy[s] = ps.o.y; S.oz[s] = ps.o.z;
-                    S.dx[s] = ps.d.x; S.dy[s] = ps.d.y; S.dz[s] = ps.d.z;
-                    S.time[s] = ps.time;
-                    cold_st(rec, CC_T, 1.0f, 1.0f, 1.0f, 1.0f);                     // throughput 1, eta 1
-                    cold_st(rec, CC_L, 0.0f, 0.0f, 0.0f, 1.0f);                     // radiance 0, bsdfPdf 1
-                    cold_st(rec, CC_A, 0.0f, 0.0f, 0.0f, u2f((uint32_t)idx));      // no absorption, the sample index
-                    cold_st(rec, CC_RNG, u2f(ps.rng.s1), u2f(ps.rng.s2), rx, ry);      // the RNG, the raster position
-                    S.flags[s] = ((uint32_t)TB_REFLECTED << 1) | ((uint32_t)WF2_PH_EXT << 3);
-                    fresh = true;
-                    want = false;
-                } else if (P.bandFlags) {
-                    // tile padding outside the image retires at once
-                    wf2_band_pad(P.bandCount, P.bandFlags, P.bandSamples, (uint32_t)P.samplesPerFrame, P.bandTag, (uint32_t)idx);
-                }
-            }
-        }
-        rparts[WF2_R_REGEN] += wf2_now() - t2;
-    }
-    return fresh;
 }
 
 template <int THREADS, int MODE, uint32_t FEAT>
@@ -299,7 +226,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
 
         if (stage == WF2_Q_R) {
             // ===================== R: splat the finished sample, regenerate =======================
-            const bool fresh = wf2_lq_stage_r(S, P, total, coldBase + (size_t)s * CC_CHUNKS, s, active, rparts);
+            const bool fresh = wf2_stage_r(S, P, total, coldBase + (size_t)s * CC_CHUNKS, s, active, rparts);
             __threadfence_block();
             wf2_push(S, WF2_Q_T, fresh, s);
             wf2_retire(S, active && !fresh);

@@ -6,6 +6,7 @@
 //   A  extension result: miss -> sky -> R; hit -> absorption, emission MIS, first NEE sample -> T
 //   B  shadow result: connect the NEE sample; next NEE sample -> T, or BSDF sample, throughput
 //      update and next extension ray -> T, or termination -> R
+// Stage R is the common one (wf2_common.cuh: wf2_stage_r); only its splat (wf2_splat, below) is this layout's own.
 //
 // The queues are lock-free rings in shared memory: producers reserve cells with one warp-aggregated atomicAdd on
 // `tail` and store lap-tagged slot ids, so a chunk is always full while the queue holds >= 32 entries.
@@ -178,6 +179,22 @@ TB_DEV void wf2_store_shadow(Wf2Shared& S, float4* rec, int s, const ShadowRay& 
     cold_st(rec, CC_LA, c.Lacc.x, c.Lacc.y, c.Lacc.z, 0.0f);
 }
 
+// The ring layout's splat (stage R: wf2_stage_r).  The RNG chunk's .zw holds NEE bookkeeping by now, so the raster
+// position is drawn again from the sample's seed.  (The lane-owned splat, add_sample_small, would make veach's
+// hard-phase kernel bigger and slower.)
+TB_DEV void wf2_splat(const LaunchParams& P, const float4* rec, float4 cl, uint32_t doneSample)
+{
+    int px, py, frame;
+    decode_sample(P, (unsigned long long)doneSample, px, py, frame);
+    // raster position of the sample: its first two RNG draws (render.cpp:476,481-482)
+    Rng rr = rng_seed(tb_sample_seed((uint32_t)(py * P.film.width + px), (uint32_t)frame));
+    float rx = rng_float(rr);
+    float ry = rng_float(rr);
+    rx += px;
+    ry += py;
+    sample_end(P, px, py, rx, ry, v3(cl.x, cl.y, cl.z));
+}
+
 template <int THREADS, int MODE, uint32_t FEAT>
 __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(const __grid_constant__ LaunchParams P, unsigned long long total)
 {
@@ -235,6 +252,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
     int step = 0, cycle = 0;
     unsigned int stepTail = TB_WF2_PATHS;   // every slot starts in the R queue
     int stepQueue = WF2_Q_R;
+    unsigned int rparts[WF2_R_PARTS];   // stage R's part timing: only the lane-owned kernel reports it
 
     for (;;) {
         int s = 0, n = 0, stage = -1;
@@ -316,7 +334,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
 
         if (stage == WF2_Q_R) {
             // ===================== R: splat the finished sample, regenerate =======================
-            const bool fresh = wf2_stage_r(S, P, total, coldBase + (size_t)s * CC_CHUNKS, s, active);
+            const bool fresh = wf2_stage_r(S, P, total, coldBase + (size_t)s * CC_CHUNKS, s, active, rparts);
             __threadfence_block();
             wf2_push_trace(S, sc, split, hard ? WF2_Q_F0 + (cycle & 1) : WF2_Q_T, fresh, s);
             wf2_retire(S, active && !fresh);

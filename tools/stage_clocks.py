@@ -27,7 +27,7 @@ VARIANT = "libtinsel_b200_clocks.so"
 WORDS = 18                     # tb_kernels.cuh: TB_WF2_STAGE_CLOCK_WORDS
 WARPS_PER_CTA = 512 // 32
 STAGES = ["R", "T", "A", "B"]  # counter order (wf2_lanes.cuh: Wf2Clocks)
-R_PARTS = ["splat", "claim", "regenerate"]   # wf2_lanes.cuh: WF2_R_*
+R_PARTS = ["splat", "claim", "regenerate"]   # wf2_common.cuh: WF2_R_*
 
 
 def main():
