@@ -601,8 +601,10 @@ struct __align__(16) ProgOp {
     int bits;        // guard bit (TB_BIT_ALWAYS: unconditional) | own bit << 8 (BOX only)
 };
 
+// `flat` is sc.flat, or the same program where the caller can name it in shared memory (the lane-owned wavefront
+// kernel: Wf2Shared::flat), so that the op loads compile to shared-memory loads instead of generic ones.
 template <uint32_t FEAT = TB_FEAT_ALL>
-TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
+TB_DEV Hit trace_closest(const DScene& sc, const ProgOp* flat, V3 o, V3 d, float time, bool wantNormal)
 {
     const int n = sc.numFlat;
     const bool guard = (fabsf(o.x) < 1.0e7f) & (fabsf(o.y) < 1.0e7f) & (fabsf(o.z) < 1.0e7f) & (d.x == d.x) & (d.y == d.y) &
@@ -627,8 +629,8 @@ TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNorm
     uint32_t visited = 0u;
 
     for (int i = 0; i < n; ++i) {
-        const float4 a = *reinterpret_cast<const float4*>(sc.flat[i].a);
-        const float4 bk = *reinterpret_cast<const float4*>(sc.flat[i].b);   // b[0], b[1], kindPrim, bits
+        const float4 a = *reinterpret_cast<const float4*>(flat[i].a);
+        const float4 bk = *reinterpret_cast<const float4*>(flat[i].b);   // b[0], b[1], kindPrim, bits
         const int kindPrim = __float_as_int(bk.z), bits = __float_as_int(bk.w);
         const int gbit = bits & 0xff;
         if (gbit != TB_BIT_ALWAYS && !((visited >> gbit) & 1u)) continue;
@@ -673,4 +675,10 @@ TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNorm
     }
     h.n = face_forward(nrm, -d);
     return h;
+}
+
+template <uint32_t FEAT = TB_FEAT_ALL>
+TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
+{
+    return trace_closest<FEAT>(sc, sc.flat, o, d, time, wantNormal);
 }

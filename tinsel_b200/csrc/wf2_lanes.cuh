@@ -234,7 +234,9 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
             // ===================== T: trace the extension ray =====================================
             if (active) {
                 if (maxDepth > 0) {
-                    const Hit h = trace_closest<FEAT>(sc, v3(S.ox[s], S.oy[s], S.oz[s]), v3(S.dx[s], S.dy[s], S.dz[s]), S.time[s], true);
+                    // S.flat, not sc.flat: shared-memory loads (wf2_stage_scene stages every flat program -- api.cu's
+                    // build_program keeps them to the 32 ops S.flat holds -- and with numFlat == 0 no op is read)
+                    const Hit h = trace_closest<FEAT>(sc, S.flat, v3(S.ox[s], S.oy[s], S.oz[s]), v3(S.dx[s], S.dy[s], S.dz[s]), S.time[s], true);
                     S.ht[s] = h.t;
                     S.hnx[s] = h.n.x; S.hny[s] = h.n.y; S.hnz[s] = h.n.z;
                     S.hprim[s] = h.prim;
@@ -272,7 +274,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                     Rng rng = ps.rng;
                     int s2 = s;
                     while (nee_generate<FEAT>(sc, sf, time, c, rng, sr, lightEnd)) {
-                        const Hit sh = trace_closest<FEAT>(sc, sr.o, sr.d, time, false);
+                        const Hit sh = trace_closest<FEAT>(sc, S.flat, sr.o, sr.d, time, false);
                         asm volatile("" : "+r"(s2) : "f"(sh.t));
                         sf = wf2_surface(S, sc, s2, ct.w);
                         nee_connect<FEAT>(sc, sf, sr, sh, c);
