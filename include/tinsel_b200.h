@@ -306,7 +306,8 @@ int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200
  *   hits[i].t      its distance in units of |dir| (dir is used as given, never normalised)
  *   hits[i].normal the shading normal after FaceForward(n, -dir)
  * A miss leaves t = FLT_MAX and the face-forwarded zero normal.  `time` drives the motion-blur
- * interpolation of primitive transforms; `pad` is ignored.
+ * interpolation of primitive transforms; `pad` is ignored here (tb200_occluded_rays reads it as
+ * tmax, so one array of rays can feed both queries).
  * `rays`, `hits` and `prims` are DEVICE memory of the renderer's device (a multi-device renderer: its
  * head, devices[0]); `rays` and `hits` 16-byte aligned.  Host or foreign-device pointers, null pointers,
  * numRays < 0 and spans past the end of their allocation are refused before anything is launched.
@@ -314,9 +315,22 @@ int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200
  * in place.  Needs no tb200_init; leaves the accumulator, the frame counter, stats.frames,
  * stats.samples and tb200_last_kernel as they are; adds 1 to stats.kernelLaunches and sets stats.gpuMs
  * to the query kernel's time.  numRays == 0 launches nothing.  Returns 0 on success. */
+/* `pad`: tmax of the occlusion query (tb200_occluded_rays); the closest-hit query ignores it. */
 typedef struct tb200_ray { float origin[3]; float time; float dir[3]; float pad; } tb200_ray;   /* 32 B */
 typedef struct tb200_hit { float t; float normal[3]; } tb200_hit;                               /* 16 B */
 int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, int64_t numRays);
+
+/* ---- batched occlusion (any-hit) ray query --------------------------------------------------
+ * Per ray i, exactly: occluded[i] = 1 iff Trace(scene, Ray(origin, dir, time)) of src/render.cpp:17-62
+ * returns a primitive (prims[i] >= 0 from tb200_trace_rays) and its t < tmax, where tmax is the
+ * ray's `pad` field; else 0.  t is in units of |dir|, so dir = target - origin with tmax = 1 asks
+ * whether anything lies between two points.  tmax <= 0 or NaN gives 0, tmax = +inf "hits anything";
+ * a miss (t = FLT_MAX) is never occluded.  The walk stops at the first blocker and computes no normal.
+ * `rays` (16-byte aligned) and `occluded` (numRays bytes) are DEVICE memory of the renderer's
+ * device, with the refusals, stream, synchronisation and side effects of tb200_trace_rays: it adds
+ * 1 to stats.kernelLaunches, sets stats.gpuMs to its kernel's time, and touches nothing else.
+ * numRays == 0 launches nothing.  Returns 0 on success. */
+int tb200_occluded_rays(tb200_renderer* r, const tb200_ray* rays, uint8_t* occluded, int64_t numRays);
 
 /* Sets the frame counter (frame k seeds sample k of every pixel). */
 void tb200_set_frame(tb200_renderer* r, int frame);

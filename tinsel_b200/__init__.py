@@ -84,6 +84,8 @@ def load_library():
     lib.tb200_trace_frame.argtypes = [C.c_void_p, C.POINTER(Camera), C.POINTER(Options), C.c_int, f32p, f32p]
     lib.tb200_trace_rays.restype = C.c_int
     lib.tb200_trace_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_occluded_rays.restype = C.c_int
+    lib.tb200_occluded_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_set_frame.restype = None
     lib.tb200_set_frame.argtypes = [C.c_void_p, C.c_int]
     lib.tb200_get_stats.restype = None
@@ -295,6 +297,36 @@ class Renderer:
                     "tb200_trace_frame")
         return rad, ras
 
+    def _check_tensor(self, x, name, shape, dtype):
+        """What the ray queries require of a tensor argument: its type, dtype, shape, device (the head) and layout."""
+        import torch
+        if not isinstance(x, torch.Tensor):
+            raise TypeError("%s must be a torch tensor" % name)
+        if x.dtype != dtype:
+            raise TypeError("%s must be %s, not %s" % (name, dtype, x.dtype))
+        if tuple(x.shape) != shape:
+            raise ValueError("%s must have shape %s, not %s" % (name, shape, tuple(x.shape)))
+        dev = torch.device("cuda", self.device)
+        if x.device != dev:
+            raise ValueError("%s must be on %s (the renderer's head device), not %s" % (name, dev, x.device))
+        if not x.is_contiguous():
+            raise ValueError("%s must be contiguous" % name)
+
+    def _check_rays(self, rays):
+        """Checks a (N, 8) float32 ray tensor and returns N."""
+        import torch
+        if not isinstance(rays, torch.Tensor) or rays.dim() != 2:
+            raise ValueError("rays must be a (N, 8) tensor")
+        n = rays.shape[0]
+        self._check_tensor(rays, "rays", (n, 8), torch.float32)
+        return n
+
+    def _wait_for_torch(self):
+        """On the renderer's private stream, waits for torch's current stream, so that tensors written there are complete."""
+        import torch
+        if not self._external_stream:
+            torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()
+
     def trace_rays(self, rays, hits=None, prims=None):
         """Closest hit of every ray (tb200_trace_rays): Trace (src/render.cpp:17-62) bit for bit.
         rays: contiguous float32 CUDA tensor (N, 8) on the head device -- origin.xyz, time, dir.xyz, pad.
@@ -302,36 +334,35 @@ class Renderer:
         `hits` / `prims` when given.  On the renderer's private stream the call first waits for torch's current
         stream, so that tensors written there are complete; after set_stream the work is ordered on that stream."""
         import torch
+        n = self._check_rays(rays)
         dev = torch.device("cuda", self.device)
-
-        def check(x, name, shape, dtype):
-            if not isinstance(x, torch.Tensor):
-                raise TypeError("%s must be a torch tensor" % name)
-            if x.dtype != dtype:
-                raise TypeError("%s must be %s, not %s" % (name, dtype, x.dtype))
-            if tuple(x.shape) != shape:
-                raise ValueError("%s must have shape %s, not %s" % (name, shape, tuple(x.shape)))
-            if x.device != dev:
-                raise ValueError("%s must be on %s (the renderer's head device), not %s" % (name, dev, x.device))
-            if not x.is_contiguous():
-                raise ValueError("%s must be contiguous" % name)
-
-        if not isinstance(rays, torch.Tensor) or rays.dim() != 2:
-            raise ValueError("rays must be a (N, 8) tensor")
-        n = rays.shape[0]
-        check(rays, "rays", (n, 8), torch.float32)
         if hits is None:
             hits = torch.empty((n, 4), dtype=torch.float32, device=dev)
         if prims is None:
             prims = torch.empty((n,), dtype=torch.int32, device=dev)
-        check(hits, "hits", (n, 4), torch.float32)
-        check(prims, "prims", (n,), torch.int32)
+        self._check_tensor(hits, "hits", (n, 4), torch.float32)
+        self._check_tensor(prims, "prims", (n,), torch.int32)
         if n == 0:
             return hits, prims
-        if not self._external_stream:
-            torch.cuda.current_stream(dev).synchronize()
+        self._wait_for_torch()
         self._check(self.lib.tb200_trace_rays(self.h, rays.data_ptr(), hits.data_ptr(), prims.data_ptr(), n), "tb200_trace_rays")
         return hits, prims
+
+    def occluded(self, rays, out=None):
+        """Whether anything blocks each ray before its tmax (tb200_occluded_rays): exactly `Trace (src/render.cpp:17-62)
+        hits a primitive and its t < tmax`.  rays: as for trace_rays, with column 7 = tmax in units of |dir| (so
+        dir = target - origin, tmax = 1 asks about the segment between two points).  Returns a (N,) torch.bool
+        tensor, `out` when given.  Stream behaviour as for trace_rays."""
+        import torch
+        n = self._check_rays(rays)
+        if out is None:
+            out = torch.empty((n,), dtype=torch.bool, device=torch.device("cuda", self.device))
+        self._check_tensor(out, "out", (n,), torch.bool)
+        if n == 0:
+            return out
+        self._wait_for_torch()
+        self._check(self.lib.tb200_occluded_rays(self.h, rays.data_ptr(), out.data_ptr(), n), "tb200_occluded_rays")
+        return out
 
     def set_frame(self, frame):
         self.lib.tb200_set_frame(self.h, frame)

@@ -141,7 +141,7 @@ class Stats(C.Structure):
 
 
 class Ray(C.Structure):
-    """tb200_ray: one ray of tb200_trace_rays (32 bytes)."""
+    """tb200_ray: one ray of tb200_trace_rays and tb200_occluded_rays (32 bytes; `pad` is the occlusion query's tmax)."""
     _fields_ = [("origin", C.c_float * 3), ("time", C.c_float), ("dir", C.c_float * 3), ("pad", C.c_float)]
 
 
@@ -191,6 +191,7 @@ EXPORTS = [
     "tb200_nlm",
     "tb200_trace_frame",
     "tb200_trace_rays",
+    "tb200_occluded_rays",
     "tb200_set_frame",
     "tb200_get_stats",
     "tb200_last_kernel",

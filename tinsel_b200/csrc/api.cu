@@ -1862,9 +1862,9 @@ static MemRangeFn mem_range_fn()
 }
 
 // `bytes` from `ptr` lie inside one allocation of device memory on r's device
-static bool check_device_span(const tb200_renderer* r, const void* ptr, size_t bytes, size_t align, const char* what)
+static bool check_device_span(const char* entry, const tb200_renderer* r, const void* ptr, size_t bytes, size_t align, const char* what)
 {
-    const std::string name = std::string("tb200_trace_rays: ") + what;
+    const std::string name = std::string(entry) + ": " + what;
     if (!ptr) return set_error(name + " is null");
     if ((uintptr_t)ptr % align != 0) return set_error(name + " is not aligned to " + std::to_string(align) + " bytes");
     cudaPointerAttributes attr;
@@ -1877,7 +1877,7 @@ static bool check_device_span(const tb200_renderer* r, const void* ptr, size_t b
     if (attr.device != r->device)
         return set_error(name + " lies on device " + std::to_string(attr.device) + ", not on the renderer's device " + std::to_string(r->device));
     const MemRangeFn range = mem_range_fn();
-    if (!range) return set_error("tb200_trace_rays: cuMemGetAddressRange is not available from the driver");
+    if (!range) return set_error(std::string(entry) + ": cuMemGetAddressRange is not available from the driver");
     unsigned long long base = 0;
     size_t size = 0;
     if (range(&base, &size, (unsigned long long)(uintptr_t)ptr) != 0) return set_error(name + ": the driver knows no allocation at this address");
@@ -1887,21 +1887,55 @@ static bool check_device_span(const tb200_renderer* r, const void* ptr, size_t b
     return true;
 }
 
-int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, int64_t numRays)
+// The checks of a query's renderer and ray count: 0 when there are rays to trace (the renderer's device is then
+// current), 1 when there are none, -1 (error set) when either is refused
+static int query_begin(const char* entry, tb200_renderer* r, int64_t numRays)
 {
     if (!r) {
-        set_error("tb200_trace_rays: null renderer");
+        set_error(std::string(entry) + ": null renderer");
         return -1;
     }
     if (numRays < 0 || numRays > (int64_t)(SIZE_MAX / sizeof(tb200_ray))) {
-        set_error("tb200_trace_rays: numRays " + std::to_string((long long)numRays) + " is out of range");
+        set_error(std::string(entry) + ": numRays " + std::to_string((long long)numRays) + " is out of range");
         return -1;
     }
-    if (numRays == 0) return 0;
+    if (numRays == 0) return 1;
     cudaSetDevice(r->device);   // a multi-device renderer answers on its head, which holds a full copy of the scene
+    return 0;
+}
+
+// Runs launch(&launches) -- one query kernel -- on r's stream, waits for it and sets stats.gpuMs to its time
+static int query_run(const char* entry, tb200_renderer* r, const std::function<void(unsigned long long*)>& launch)
+{
+    unsigned long long launches = 0;
+    if (cudaEventRecord(r->evStart, r->stream) != cudaSuccess) {
+        set_error(std::string(entry) + ": " + cudaGetErrorString(cudaGetLastError()));
+        return -1;
+    }
+    launch(&launches);
+    r->stats.kernelLaunches += launches;
+    float ms = 0.0f;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaEventRecord(r->evStop, r->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, r->evStart, r->evStop);
+    if (e != cudaSuccess) {
+        set_error(std::string(entry) + ": " + cudaGetErrorString(e));
+        return -1;
+    }
+    r->stats.gpuMs = ms;
+    return 0;
+}
+
+int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, int64_t numRays)
+{
+    const char* entry = "tb200_trace_rays";
+    const int begin = query_begin(entry, r, numRays);
+    if (begin != 0) return begin < 0 ? -1 : 0;
     const size_t n = (size_t)numRays;
-    if (!check_device_span(r, rays, n * sizeof(tb200_ray), 16, "rays") || !check_device_span(r, hits, n * sizeof(tb200_hit), 16, "hits") ||
-        !check_device_span(r, prims, n * sizeof(int32_t), 4, "prims"))
+    if (!check_device_span(entry, r, rays, n * sizeof(tb200_ray), 16, "rays") ||
+        !check_device_span(entry, r, hits, n * sizeof(tb200_hit), 16, "hits") ||
+        !check_device_span(entry, r, prims, n * sizeof(int32_t), 4, "prims"))
         return -1;
     static_assert(sizeof(tb200_ray) == 32 && sizeof(tb200_hit) == 16, "the query kernel reads two float4 per ray and writes one");
     QueryParams Q;
@@ -1911,24 +1945,25 @@ int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, 
     Q.prims = prims;
     Q.numRays = numRays;
     Q.counter = r->dCounter;   // the wavefront's work counter: free between launches on this stream
-    unsigned long long launches = 0;
-    if (cudaEventRecord(r->evStart, r->stream) != cudaSuccess) {
-        set_error(std::string("tb200_trace_rays: ") + cudaGetErrorString(cudaGetLastError()));
+    return query_run(entry, r, [&](unsigned long long* launches) { launch_trace_rays(Q, r->numSMs, r->stream, launches); });
+}
+
+int tb200_occluded_rays(tb200_renderer* r, const tb200_ray* rays, uint8_t* occluded, int64_t numRays)
+{
+    const char* entry = "tb200_occluded_rays";
+    const int begin = query_begin(entry, r, numRays);
+    if (begin != 0) return begin < 0 ? -1 : 0;
+    const size_t n = (size_t)numRays;
+    if (!check_device_span(entry, r, rays, n * sizeof(tb200_ray), 16, "rays") ||
+        !check_device_span(entry, r, occluded, n, 1, "occluded"))
         return -1;
-    }
-    launch_trace_rays(Q, r->numSMs, r->stream, &launches);
-    r->stats.kernelLaunches += launches;
-    float ms = 0.0f;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaEventRecord(r->evStop, r->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, r->evStart, r->evStop);
-    if (e != cudaSuccess) {
-        set_error(std::string("tb200_trace_rays: ") + cudaGetErrorString(e));
-        return -1;
-    }
-    r->stats.gpuMs = ms;
-    return 0;
+    OcclusionParams Q;
+    Q.scene = r->scene;
+    Q.rays = reinterpret_cast<const float4*>(rays);
+    Q.occluded = occluded;
+    Q.numRays = numRays;
+    Q.counter = r->dCounter;
+    return query_run(entry, r, [&](unsigned long long* launches) { launch_occluded_rays(Q, r->numSMs, r->stream, launches); });
 }
 
 #ifdef TB_WF2_STAGE_CLOCKS

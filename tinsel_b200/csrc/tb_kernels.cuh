@@ -105,3 +105,13 @@ struct QueryParams {
     unsigned long long* counter;   // work counter, cleared by the launch
 };
 const char* launch_trace_rays(const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
+
+// Batched occlusion query (tb200_occluded_rays, tb_query.cuh): whether Trace of every ray hits something before its tmax.
+struct OcclusionParams {
+    DScene scene;
+    const float4* rays;   // 2 per ray: origin.xyz, time; dir.xyz, tmax
+    unsigned char* occluded;   // 1 per ray: 1 when occluded, else 0
+    long long numRays;
+    unsigned long long* counter;   // work counter, cleared by the launch
+};
+const char* launch_occluded_rays(const OcclusionParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);

@@ -682,3 +682,208 @@ TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNorm
 {
     return trace_closest<FEAT>(sc, sc.flat, o, d, time, wantNormal);
 }
+
+// ---- occlusion (any-hit) query: trace_occluded() answers `Trace(o, d, time) hits a primitive with t < tmax`
+// (tb200_occluded_rays) exactly, without finding the closest hit.
+//
+// Why stopping at the first blocker is exact:
+//   * Scene level.  Trace has no closest-t culling, so the set of primitives it tests depends only on the slab
+//     tests, never on what it has found or in which order (the premise of the flat scene program).  It records a
+//     primitive when 0 < t < minT, minT starting at FLT_MAX, so its closest t is below tmax iff some tested
+//     primitive has 0 < t < min(tmax, FLT_MAX).  Any visit order may stop at the first such primitive, and exact-t
+//     ties do not matter: no tie fallback, no winner records.
+//   * Mesh level.  The mesh walk does cull boxes with its own closest hit, so it keeps the reference's order and
+//     truncation, starting from FLT_MAX.  A triangle is recorded only when 0 < t < closestT, so the records
+//     strictly decrease: the first record below tmax proves that the mesh's final t is below tmax, and no record
+//     below tmax proves that it is not.
+//   * Boxes are never culled with the query's tmax.  A box's slab entry can round above the t of a triangle inside
+//     it; the reference, whose bound is its own closest hit, still descends into that box, and a walk culled at
+//     tmax would not (DESIGN §8b).
+// No u/v/w, no normals, no treelet (the query kernel stages none).
+
+// ray_mesh() that stops at the first recorded triangle with t < tmax; true when there is one.
+static __device__ __noinline__ bool ray_mesh_occluded(const DMesh& m, V3 origin, V3 dir, float tmax)
+{
+    V3 rcp;
+    rcp.x = 1.0f / dir.x;
+    rcp.y = 1.0f / dir.y;
+    rcp.z = 1.0f / dir.z;
+
+    uint32_t stack[TB_STACK];
+    float closestT = FLT_MAX;
+    stack[0] = m.rootRef;
+    int count = 1;
+    while (count) {
+        const uint32_t ref = stack[--count];
+        if (ref & TB_LEAF) {
+            const uint32_t i = ref & ~TB_LEAF;
+            const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
+            const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
+            const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
+            float t, u, v, w, sign;
+            V3 n;
+            if (ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n) &&
+                t > 0.0f && t < closestT) {
+                if (t < tmax) return true;
+                closestT = t;
+            }
+        } else {
+            const BvhPair* pr = &m.pairs[ref];
+            const float4 a = pr->a, b = pr->b, c = pr->c;
+            const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
+            float tLeft, tRight;
+            const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < closestT;
+            const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < closestT;
+            uint32_t left = kids.x, right = kids.y;
+            if (hitLeft && hitRight && (tLeft < tRight)) {
+                const uint32_t tmp = left;
+                left = right;
+                right = tmp;
+            }
+            if (hitLeft) stack[count++] = left;
+            if (hitRight) stack[count++] = right;
+        }
+    }
+    return false;
+}
+
+// ray_mesh_small()'s trees (one leaf, or one pair over two leaves): the reference tests every leaf whose box passes
+// `tChild < FLT_MAX` and no box test follows, so the triangles tested do not depend on their order.
+// Returns false, having done nothing, for any other tree; else sets `occluded`.
+TB_DEV bool ray_mesh_small_occluded(const DMesh& m, V3 origin, V3 dir, float tmax, bool& occluded)
+{
+    uint32_t first = m.rootRef, second = 0u;
+    if (!(first & TB_LEAF)) {
+        const BvhPair* pr = &m.pairs[first];
+        const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
+        if (!(kids.x & kids.y & TB_LEAF)) return false;
+        const float4 a = pr->a, b = pr->b, c = pr->c;
+        V3 rcp;
+        rcp.x = 1.0f / dir.x;
+        rcp.y = 1.0f / dir.y;
+        rcp.z = 1.0f / dir.z;
+        float tLeft, tRight;
+        const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < FLT_MAX;
+        const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < FLT_MAX;
+        first = hitLeft ? kids.x : 0u;
+        second = hitRight ? kids.y : 0u;
+    }
+    occluded = false;
+#pragma unroll 1
+    for (int k = 0; k < 2 && !occluded; ++k) {
+        const uint32_t ref = k == 0 ? first : second;
+        if (!(ref & TB_LEAF)) continue;
+        const uint32_t i = ref & ~TB_LEAF;
+        const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
+        const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
+        const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
+        float t, u, v, w, sign;
+        V3 n;
+        // a triangle with 0 < t < tmax is recorded unless an earlier record is already below it, so either way the
+        // mesh's closest t is below tmax
+        occluded = ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n) &&
+                   t > 0.0f && t < tmax;
+    }
+    return true;
+}
+
+// prim_test() and the scene-level acceptance `0 < t`, then `t < tmax`: whether primitive p has a hit that makes the
+// ray occluded.  Meshes take the early-exit walks above; prim_test serves only spheres and planes here (a sphere
+// hit can have t <= 0).
+template <uint32_t FEAT = TB_FEAT_ALL>
+TB_DEV bool prim_occludes(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, float tmax)
+{
+    if (p.type != TB200_PLANE && p.type != TB200_SPHERE) {
+        const Xf xf = prim_transform<FEAT>(p, time);
+        const V3 lo = inverse_transform_point(xf, o);
+        const V3 ld = inverse_transform_vector(xf, d);
+        const DMesh& m = sc.meshes[p.mesh];
+        bool occluded;
+        if (ray_mesh_small_occluded(m, lo, ld, tmax, occluded)) return occluded;
+        return ray_mesh_occluded(m, lo, ld, tmax);
+    }
+    PrimHit ph;
+    return prim_test<FEAT>(sc, p, o, d, time, ph) && ph.t > 0.0f && ph.t < tmax;
+}
+
+// trace_ordered()'s stack walk, stopping at the first primitive that occludes.  The near-first order is kept only
+// because it tends to find a blocker sooner.
+template <uint32_t FEAT = TB_FEAT_ALL>
+TB_ORDERED_ATTR bool occluded_ordered(const DScene& sc, V3 o, V3 d, float time, float tmax)
+{
+    V3 rcp;
+    rcp.x = 1.0f / d.x;
+    rcp.y = 1.0f / d.y;
+    rcp.z = 1.0f / d.z;
+
+    uint32_t stack[TB_STACK];
+    stack[0] = sc.rootRef;
+    int count = 1;
+    while (count) {
+        const uint32_t ref = stack[--count];
+        if (ref & TB_LEAF) {
+            if (prim_occludes<FEAT>(sc, sc.prims[ref & ~TB_LEAF], o, d, time, tmax)) return true;
+        } else {
+            const BvhPair* pr = &sc.pairs[ref];
+            const float4 a = pr->a, b = pr->b, c = pr->c;
+            float tLeft, tRight;
+            const bool hitLeft = ray_aabb(o, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft);
+            const bool hitRight = ray_aabb(o, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight);
+            uint32_t left = pr->left, right = pr->right;
+            if (hitLeft && hitRight && (tLeft < tRight)) {
+                const uint32_t tmp = left;
+                left = right;
+                right = tmp;
+            }
+            if (hitLeft) stack[count++] = left;
+            if (hitRight) stack[count++] = right;
+        }
+    }
+    return false;
+}
+
+// Whether Trace(o, d, time) returns a primitive with t < tmax.  tmax <= 0 or NaN: never; a miss (t = FLT_MAX):
+// never, whatever tmax.  The flat scene program where trace_closest() runs it (the same guard), else the early-exit
+// stack walk.
+template <uint32_t FEAT = TB_FEAT_ALL>
+TB_DEV bool trace_occluded(const DScene& sc, V3 o, V3 d, float time, float tmax)
+{
+    if (!(tmax > 0.0f)) return false;
+    if (tmax > FLT_MAX) tmax = FLT_MAX;   // Trace records only t < FLT_MAX
+    const int n = sc.numFlat;
+    const bool guard = (fabsf(o.x) < 1.0e7f) & (fabsf(o.y) < 1.0e7f) & (fabsf(o.z) < 1.0e7f) & (d.x == d.x) & (d.y == d.y) &
+                       (d.z == d.z);
+    if (n == 0 || !guard) return occluded_ordered<FEAT>(sc, o, d, time, tmax);
+
+    V3 rcp;
+    rcp.x = 1.0f / d.x;
+    rcp.y = 1.0f / d.y;
+    rcp.z = 1.0f / d.z;
+    uint32_t visited = 0u;
+    for (int i = 0; i < n; ++i) {
+        const float4 a = *reinterpret_cast<const float4*>(sc.flat[i].a);
+        const float4 bk = *reinterpret_cast<const float4*>(sc.flat[i].b);   // b[0], b[1], kindPrim, bits
+        const int kindPrim = __float_as_int(bk.z), bits = __float_as_int(bk.w);
+        const int gbit = bits & 0xff;
+        if (gbit != TB_BIT_ALWAYS && !((visited >> gbit) & 1u)) continue;
+        const int kind = kindPrim & 0xff;
+        if (kind == TB_OP_PLANE) {
+            // IntersectRayPlane, intersection.h:85-99
+            const float dd = a.x * d.x + a.y * d.y + a.z * d.z + a.w * 0.0f;
+            if (dd == 0.0f) continue;
+            const float t = -(a.x * o.x + a.y * o.y + a.z * o.z + a.w * 1.0f) / dd;
+            if (t > 0.0f && t < tmax) return true;
+            continue;
+        }
+        if (kind != TB_OP_LEAF) {
+            float tbox;
+            if (!ray_aabb(o, rcp, a.x, a.y, a.z, a.w, bk.x, bk.y, tbox)) continue;
+            if (kind == TB_OP_BOX) {
+                visited |= 1u << ((bits >> 8) & 0xff);
+                continue;
+            }
+        }
+        if (prim_occludes<FEAT>(sc, sc.prims[kindPrim >> 8], o, d, time, tmax)) return true;
+    }
+    return false;
+}
