@@ -1,7 +1,7 @@
 """Meshes whose BVH is one leaf or one interior pair over two leaves (a quad: cornell's light) are walked inline
 without the traversal stack, and transforms whose rotation is exactly (+0, +0, +0, +1) skip the quaternion
 arithmetic (tb_math.cuh: rotate_xf).  Both are exact: per sample in both pipelines against the CPU restatement,
-and per ray through the batched query, for quads that are unrotated, rotated, scaled, or carry a -0 quaternion
+and per ray through the batched closest-hit and occlusion queries, for quads that are unrotated, rotated, scaled, or carry a -0 quaternion
 component, beside a one-triangle mesh, a bent quad whose triangles' boxes differ (the near-first swap) and a mesh
 too deep for the inline walk.  Rays aimed at the quads' shared diagonal, where the two triangles tie in t, and
 rays along it in the quad's plane, are traced on their own."""
@@ -14,6 +14,7 @@ import pytest
 import tinsel_b200 as tb
 from tinsel_b200 import abi
 import fuzzscene
+import occlusionsets
 import rayoracle
 import raysets
 import refdrv
@@ -148,6 +149,14 @@ def test_small_meshes_per_ray(variant, tmp_path):
         assert len(bad) == 0, "%s/%s: %d of %d rays differ; first ray %s: device %s %s, port %s %s" % (
             variant, what, len(bad), len(rays), rays[bad[0]], prims[bad[0]], hits[bad[0]], want_p[bad[0]], want_h[bad[0]])
         hit_meshes.update(int(x) for x in np.unique(prims))
+        tmax_sets = occlusionsets.tmax_sets(want_h, want_p, rng)
+        for name in ("inf", "t", "t_up", "t_down"):
+            sub = occlusionsets.with_tmax(rays, tmax_sets[name])
+            got = r.occluded(torch.from_numpy(np.ascontiguousarray(sub)).cuda()).cpu().numpy()
+            want = occlusionsets.occluded(want_h, want_p, tmax_sets[name])
+            bad = np.nonzero(got != want)[0]
+            assert len(bad) == 0, "%s/%s/tmax=%s: %d of %d occlusion verdicts differ; first ray %s: device %s, port %s (prim %d, t %r)" % (
+                variant, what, name, len(bad), len(rays), sub[bad[0]], got[bad[0]], want[bad[0]], want_p[bad[0]], float(want_h[bad[0], 0]))
     assert {1, 2, 3, 4, 5} <= hit_meshes, hit_meshes   # every mesh was hit
     r.close()
     port.close()

@@ -9,39 +9,43 @@
 
 #define TB_QUERY_THREADS 256
 
+// The claim loop of both query kernels: one atomic per warp claims 32 consecutive rays; each lane loads its ray (two
+// 16-byte loads) and hands it to ray(i, a, b), which writes its answer with streaming stores, so that the outputs
+// do not evict mesh BVH lines from L2.
+template <class Ray>
+static __device__ __forceinline__ void query_claim_rays(unsigned long long* counter, long long numRays, const float4* rays, Ray ray)
+{
+    const int lane = threadIdx.x & 31;
+    const unsigned long long n = (unsigned long long)numRays;
+    for (;;) {
+        unsigned long long base = 0ull;
+        if (lane == 0) base = atomicAdd(counter, 32ull);
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (base >= n) break;
+        const unsigned long long i = base + (unsigned long long)lane;
+        if (i < n) ray(i, __ldg(&rays[2 * i]), __ldg(&rays[2 * i + 1]));
+    }
+}
+
 __global__ void __launch_bounds__(TB_QUERY_THREADS) k_trace_rays(const __grid_constant__ QueryParams P)
 {
     // one copy of the scene descriptor per CTA: trace_closest takes it by reference, and a per-thread copy would
     // live in local memory
     __shared__ struct { DScene scene; } S;
-    const int tid = threadIdx.x;
 
     // The scene tables stay in global memory: staging the primitive records, scene-level BVH pairs and flat scene
     // program in shared memory with TMA bulk copies, as k_wavefront2 does, measured no faster (DESIGN §5.6).  No
     // mesh treelet either (the host leaves DScene::treelet null).
-    if (tid == 0) S.scene = P.scene;
+    if (threadIdx.x == 0) S.scene = P.scene;
     __syncthreads();
     const DScene& sc = S.scene;
 
-    // ---- rays: one atomic per warp claims 32 consecutive rays; each lane loads its ray (two 16-byte loads),
-    // traces it and writes the hit with streaming stores, which keep the outputs from evicting mesh BVH lines
-    // from L2
-    const int lane = tid & 31;
-    const unsigned long long n = (unsigned long long)P.numRays;
-    for (;;) {
-        unsigned long long base = 0ull;
-        if (lane == 0) base = atomicAdd(P.counter, 32ull);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= n) break;
-        const unsigned long long i = base + (unsigned long long)lane;
-        if (i < n) {
-            const float4 a = __ldg(&P.rays[2 * i]);       // origin.xyz, time
-            const float4 b = __ldg(&P.rays[2 * i + 1]);   // dir.xyz, pad
-            const Hit h = trace_closest<TB_FEAT_ALL>(sc, v3(a.x, a.y, a.z), v3(b.x, b.y, b.z), a.w, true);
-            __stcs(&P.hits[i], make_float4(h.t, h.n.x, h.n.y, h.n.z));
-            __stcs(&P.prims[i], h.prim);
-        }
-    }
+    // a: origin.xyz, time; b: dir.xyz, pad
+    query_claim_rays(P.counter, P.numRays, P.rays, [&](unsigned long long i, float4 a, float4 b) {
+        const Hit h = trace_closest<TB_FEAT_ALL>(sc, v3(a.x, a.y, a.z), v3(b.x, b.y, b.z), a.w, true);
+        __stcs(&P.hits[i], make_float4(h.t, h.n.x, h.n.y, h.n.z));
+        __stcs(&P.prims[i], h.prim);
+    });
 }
 
 // CTAs of a persistent query kernel: as many as the SMs hold at once, but no more than there are 32-ray chunks
@@ -71,26 +75,15 @@ const char* launch_trace_rays(const QueryParams& p, int numSMs, cudaStream_t str
 __global__ void __launch_bounds__(TB_QUERY_THREADS) k_occluded_rays(const __grid_constant__ OcclusionParams P)
 {
     __shared__ struct { DScene scene; } S;
-    const int tid = threadIdx.x;
-    if (tid == 0) S.scene = P.scene;
+    if (threadIdx.x == 0) S.scene = P.scene;
     __syncthreads();
     const DScene& sc = S.scene;
 
-    const int lane = tid & 31;
-    const unsigned long long n = (unsigned long long)P.numRays;
-    for (;;) {
-        unsigned long long base = 0ull;
-        if (lane == 0) base = atomicAdd(P.counter, 32ull);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= n) break;
-        const unsigned long long i = base + (unsigned long long)lane;
-        if (i < n) {
-            const float4 a = __ldg(&P.rays[2 * i]);       // origin.xyz, time
-            const float4 b = __ldg(&P.rays[2 * i + 1]);   // dir.xyz, tmax
-            const bool occ = trace_occluded<TB_FEAT_ALL>(sc, v3(a.x, a.y, a.z), v3(b.x, b.y, b.z), a.w, b.w);
-            __stcs(&P.occluded[i], (unsigned char)occ);
-        }
-    }
+    // a: origin.xyz, time; b: dir.xyz, tmax
+    query_claim_rays(P.counter, P.numRays, P.rays, [&](unsigned long long i, float4 a, float4 b) {
+        const bool occ = trace_occluded<TB_FEAT_ALL>(sc, v3(a.x, a.y, a.z), v3(b.x, b.y, b.z), a.w, b.w);
+        __stcs(&P.occluded[i], (unsigned char)occ);
+    });
 }
 
 const char* launch_occluded_rays(const OcclusionParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)

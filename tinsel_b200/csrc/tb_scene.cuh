@@ -1,4 +1,4 @@
-// tb_scene.cuh -- GPU-side scene layout and the two-level closest-hit traversal.
+// tb_scene.cuh -- GPU-side scene layout and the two-level traversal of the closest-hit and occlusion queries.
 //
 // Layout (built on the host by api.cu from a tb200_scene):
 //   * DPrim[]     one record per Primitive (scene.h:142-159) with the per-primitive constants the
@@ -270,6 +270,16 @@ TB_DEV Xf prim_transform(const DPrim& p, float time)
     return interpolate_transform(p.start, p.end, time);
 }
 
+// the reciprocal direction of the slab tests: three IEEE divisions, as the reference computes it
+TB_DEV V3 ray_rcp(const V3& d)
+{
+    V3 rcp;
+    rcp.x = 1.0f / d.x;
+    rcp.y = 1.0f / d.y;
+    rcp.z = 1.0f / d.z;
+    return rcp;
+}
+
 // IntersectRayAABBFast, intersection.h:373-397 (minf/maxf are the ternaries of :368-369)
 TB_DEV bool ray_aabb(V3 pos, V3 rcp, float lx, float ly, float lz, float ux, float uy, float uz, float& t)
 {
@@ -322,49 +332,45 @@ TB_DEV bool ray_tri(V3 p, V3 dir, V3 a, V3 b, V3 c, float& t, float& u, float& v
     return true;
 }
 
+// ray_tri() against triangle i of mesh m, read from its pre-gathered vertices
+TB_DEV bool tri_hit(const DMesh& m, uint32_t i, const V3& origin, const V3& dir, float& t, float& u, float& v, float& w, float& sign, V3& n)
+{
+    const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
+    const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
+    const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
+    return ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n);
+}
+
 struct MeshHit {
     float t, u, v, w;
     int tri;
     V3 n;   // closestNormal = n*sign, unnormalised (intersection.h:658)
 };
 
-// IntersectRayMesh + MeshQuery, intersection.h:629-749: the reference's stack walk, one triangle or interior
-// pair per iteration in the reference's order.  Pair records below `topCount` are read from `top` (the staged
-// treelet), the rest from the mesh's own array.
-// Returns the closest hit; tri == -1 (and t == FLT_MAX) when the ray misses the mesh.
-static __device__ __noinline__ MeshHit ray_mesh(const DMesh& m, const unsigned char* top, uint32_t topCount, V3 origin, V3 dir)
+// IntersectRayMesh + MeshQuery, intersection.h:629-749: the reference's stack walk, one triangle or interior pair
+// per iteration in the reference's order, with children culled at the mesh's own closest hit.  Pair records below
+// `topCount` are read from `top` (the staged treelet), the rest from the mesh's own array.  Each triangle with
+// 0 < t < closestT lowers closestT to t and is handed to record(t, i, u, v, w, sign, n); the walk stops when that
+// returns true.  Returns closestT: FLT_MAX when nothing was recorded.
+template <class Record>
+TB_DEV float mesh_walk(const DMesh& m, const unsigned char* top, uint32_t topCount, const V3& origin, const V3& dir, Record record)
 {
-    MeshHit out;
-    V3 rcp;
-    rcp.x = 1.0f / dir.x;
-    rcp.y = 1.0f / dir.y;
-    rcp.z = 1.0f / dir.z;
-
+    const V3 rcp = ray_rcp(dir);
     uint32_t stack[TB_STACK];
     float closestT = FLT_MAX;
     float tmax = FLT_MAX;
-    out.tri = -1;
-    out.u = out.v = out.w = 0.0f;
-    out.n = v3s(0.0f);
     stack[0] = m.rootRef;
     int count = 1;
     while (count) {
         const uint32_t ref = stack[--count];
         if (ref & TB_LEAF) {
             const uint32_t i = ref & ~TB_LEAF;
-            const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
-            const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
-            const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
             float t, u, v, w, sign;
             V3 n;
-            if (ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n)) {
+            if (tri_hit(m, i, origin, dir, t, u, v, w, sign, n)) {
                 if (t > 0.0f && t < closestT) {
                     closestT = t;
-                    out.u = u;
-                    out.v = v;
-                    out.w = w;
-                    out.tri = (int)i;
-                    out.n = n * sign;
+                    if (record(t, i, u, v, w, sign, n)) break;
                 }
             }
             tmax = closestT;  // "truncate ray", intersection.h:700
@@ -387,35 +393,58 @@ static __device__ __noinline__ MeshHit ray_mesh(const DMesh& m, const unsigned c
             if (hitRight) stack[count++] = right;
         }
     }
-    out.t = closestT;
+    return closestT;
+}
+
+// The closest hit of mesh_walk(); tri == -1 (and t == FLT_MAX) when the ray misses the mesh.
+static __device__ __noinline__ MeshHit ray_mesh(const DMesh& m, const unsigned char* top, uint32_t topCount, V3 origin, V3 dir)
+{
+    MeshHit out;
+    out.tri = -1;
+    out.u = out.v = out.w = 0.0f;
+    out.n = v3s(0.0f);
+    out.t = mesh_walk(m, top, topCount, origin, dir, [&](float, uint32_t i, float u, float v, float w, float sign, V3 n) {
+        out.u = u;
+        out.v = v;
+        out.w = w;
+        out.tri = (int)i;
+        out.n = n * sign;
+        return false;
+    });
     return out;
 }
 
-// ray_mesh() for a BVH that is one leaf, or one interior pair over two leaves (a quad: cornell's light), inline and
-// without the stack.  The reference pops the root, pushes each child whose box passes `tChild < tmax` (tmax is
-// still FLT_MAX), the nearer one last when both do, then pops and tests the triangles in turn; no box test follows,
-// so the truncation of the ray changes nothing.  Returns false, having done nothing, for any other tree.
+// The leaves of a BVH that is one leaf, or one interior pair over two leaves (a quad: cornell's light), in the order
+// the reference pops them; a reference without TB_LEAF ends the list.  The reference pops the root, pushes each
+// child whose box passes `tChild < tmax` (tmax is still FLT_MAX), the nearer one last when both do, then pops and
+// tests the triangles in turn; no box test follows, so the truncation of the ray changes nothing and the walk needs
+// no stack.  Returns false for any other tree.
+TB_DEV bool small_mesh_leaves(const DMesh& m, const V3& origin, const V3& dir, uint32_t& first, uint32_t& second)
+{
+    first = m.rootRef;
+    second = 0u;
+    if (first & TB_LEAF) return true;
+    const BvhPair* pr = &m.pairs[first];
+    const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
+    if (!(kids.x & kids.y & TB_LEAF)) return false;
+    const float4 a = pr->a, b = pr->b, c = pr->c;
+    const V3 rcp = ray_rcp(dir);
+    float tLeft, tRight;
+    const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < FLT_MAX;
+    const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < FLT_MAX;
+    const bool both = hitLeft && hitRight;
+    const bool swap = both && (tLeft < tRight);   // left pushed last: it pops first
+    first = hitRight ? (swap ? kids.x : kids.y) : (hitLeft ? kids.x : 0u);
+    second = both ? (swap ? kids.y : kids.x) : 0u;
+    return true;
+}
+
+// ray_mesh() for small_mesh_leaves()' trees, inline and without the stack.  Returns false, having done nothing, for
+// any other tree.
 TB_DEV bool ray_mesh_small(const DMesh& m, V3 origin, V3 dir, MeshHit& out)
 {
-    // the leaves in the order the reference pops them; a reference without TB_LEAF ends the list
-    uint32_t first = m.rootRef, second = 0u;
-    if (!(first & TB_LEAF)) {
-        const BvhPair* pr = &m.pairs[first];
-        const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
-        if (!(kids.x & kids.y & TB_LEAF)) return false;
-        const float4 a = pr->a, b = pr->b, c = pr->c;
-        V3 rcp;
-        rcp.x = 1.0f / dir.x;
-        rcp.y = 1.0f / dir.y;
-        rcp.z = 1.0f / dir.z;
-        float tLeft, tRight;
-        const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < FLT_MAX;
-        const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < FLT_MAX;
-        const bool both = hitLeft && hitRight;
-        const bool swap = both && (tLeft < tRight);   // left pushed last: it pops first
-        first = hitRight ? (swap ? kids.x : kids.y) : (hitLeft ? kids.x : 0u);
-        second = both ? (swap ? kids.y : kids.x) : 0u;
-    }
+    uint32_t first, second;
+    if (!small_mesh_leaves(m, origin, dir, first, second)) return false;
     float closestT = FLT_MAX;
     out.tri = -1;
     out.u = out.v = out.w = 0.0f;
@@ -423,12 +452,9 @@ TB_DEV bool ray_mesh_small(const DMesh& m, V3 origin, V3 dir, MeshHit& out)
 #pragma unroll 1
     for (uint32_t ref = first; ref & TB_LEAF; ref = second, second = 0u) {
         const uint32_t i = ref & ~TB_LEAF;
-        const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
-        const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
-        const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
         float t, u, v, w, sign;
         V3 n;
-        if (ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n)) {
+        if (tri_hit(m, i, origin, dir, t, u, v, w, sign, n)) {
             if (t > 0.0f && t < closestT) {
                 closestT = t;
                 out.u = u;
@@ -526,11 +552,7 @@ TB_DEV V3 prim_normal(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, 
 template <uint32_t FEAT = TB_FEAT_ALL>
 TB_ORDERED_ATTR Hit trace_ordered(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
 {
-    V3 rcp;
-    rcp.x = 1.0f / d.x;
-    rcp.y = 1.0f / d.y;
-    rcp.z = 1.0f / d.z;
-
+    const V3 rcp = ray_rcp(d);
     uint32_t stack[TB_STACK];
     stack[0] = sc.rootRef;
     int count = 1;
@@ -601,20 +623,22 @@ struct __align__(16) ProgOp {
     int bits;        // guard bit (TB_BIT_ALWAYS: unconditional) | own bit << 8 (BOX only)
 };
 
+// The rays the flat program serves: the origin inside |o| < 1e7, where the planes' +-1e8 boxes cannot miss, and a
+// direction without NaN.  Every other ray takes the stack walk.
+TB_DEV bool flat_guard(const V3& o, const V3& d)
+{
+    return (fabsf(o.x) < 1.0e7f) & (fabsf(o.y) < 1.0e7f) & (fabsf(o.z) < 1.0e7f) & (d.x == d.x) & (d.y == d.y) & (d.z == d.z);
+}
+
 // `flat` is sc.flat, or the same program where the caller can name it in shared memory (the lane-owned wavefront
 // kernel: Wf2Shared::flat), so that the op loads compile to shared-memory loads instead of generic ones.
 template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV Hit trace_closest(const DScene& sc, const ProgOp* flat, V3 o, V3 d, float time, bool wantNormal)
 {
     const int n = sc.numFlat;
-    const bool guard = (fabsf(o.x) < 1.0e7f) & (fabsf(o.y) < 1.0e7f) & (fabsf(o.z) < 1.0e7f) & (d.x == d.x) & (d.y == d.y) &
-                       (d.z == d.z);
-    if (n == 0 || !guard) return trace_ordered<FEAT>(sc, o, d, time, wantNormal);
+    if (n == 0 || !flat_guard(o, d)) return trace_ordered<FEAT>(sc, o, d, time, wantNormal);
 
-    V3 rcp;
-    rcp.x = 1.0f / d.x;
-    rcp.y = 1.0f / d.y;
-    rcp.z = 1.0f / d.z;
+    const V3 rcp = ray_rcp(d);
 
     float minT = FLT_MAX;
     int closest = -1;
@@ -701,88 +725,29 @@ TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNorm
 //     tmax would not (DESIGN §8b).
 // No u/v/w, no normals, no treelet (the query kernel stages none).
 
-// ray_mesh() that stops at the first recorded triangle with t < tmax; true when there is one.
+// mesh_walk() that stops at the first recorded triangle with t < tmax; true when there is one (the walk then
+// returns that t, and otherwise a closestT that no record brought below tmax).
 static __device__ __noinline__ bool ray_mesh_occluded(const DMesh& m, V3 origin, V3 dir, float tmax)
 {
-    V3 rcp;
-    rcp.x = 1.0f / dir.x;
-    rcp.y = 1.0f / dir.y;
-    rcp.z = 1.0f / dir.z;
-
-    uint32_t stack[TB_STACK];
-    float closestT = FLT_MAX;
-    stack[0] = m.rootRef;
-    int count = 1;
-    while (count) {
-        const uint32_t ref = stack[--count];
-        if (ref & TB_LEAF) {
-            const uint32_t i = ref & ~TB_LEAF;
-            const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
-            const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
-            const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
-            float t, u, v, w, sign;
-            V3 n;
-            if (ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n) &&
-                t > 0.0f && t < closestT) {
-                if (t < tmax) return true;
-                closestT = t;
-            }
-        } else {
-            const BvhPair* pr = &m.pairs[ref];
-            const float4 a = pr->a, b = pr->b, c = pr->c;
-            const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
-            float tLeft, tRight;
-            const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < closestT;
-            const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < closestT;
-            uint32_t left = kids.x, right = kids.y;
-            if (hitLeft && hitRight && (tLeft < tRight)) {
-                const uint32_t tmp = left;
-                left = right;
-                right = tmp;
-            }
-            if (hitLeft) stack[count++] = left;
-            if (hitRight) stack[count++] = right;
-        }
-    }
-    return false;
+    return mesh_walk(m, nullptr, 0u, origin, dir, [&](float t, uint32_t, float, float, float, float, V3) { return t < tmax; }) <
+           tmax;
 }
 
-// ray_mesh_small()'s trees (one leaf, or one pair over two leaves): the reference tests every leaf whose box passes
-// `tChild < FLT_MAX` and no box test follows, so the triangles tested do not depend on their order.
+// small_mesh_leaves()' trees: the reference tests every leaf whose box passes `tChild < FLT_MAX` and no box test
+// follows, so the triangles tested, and with them the verdict, do not depend on their order.
 // Returns false, having done nothing, for any other tree; else sets `occluded`.
 TB_DEV bool ray_mesh_small_occluded(const DMesh& m, V3 origin, V3 dir, float tmax, bool& occluded)
 {
-    uint32_t first = m.rootRef, second = 0u;
-    if (!(first & TB_LEAF)) {
-        const BvhPair* pr = &m.pairs[first];
-        const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
-        if (!(kids.x & kids.y & TB_LEAF)) return false;
-        const float4 a = pr->a, b = pr->b, c = pr->c;
-        V3 rcp;
-        rcp.x = 1.0f / dir.x;
-        rcp.y = 1.0f / dir.y;
-        rcp.z = 1.0f / dir.z;
-        float tLeft, tRight;
-        const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < FLT_MAX;
-        const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < FLT_MAX;
-        first = hitLeft ? kids.x : 0u;
-        second = hitRight ? kids.y : 0u;
-    }
+    uint32_t first, second;
+    if (!small_mesh_leaves(m, origin, dir, first, second)) return false;
     occluded = false;
 #pragma unroll 1
-    for (int k = 0; k < 2 && !occluded; ++k) {
-        const uint32_t ref = k == 0 ? first : second;
-        if (!(ref & TB_LEAF)) continue;
-        const uint32_t i = ref & ~TB_LEAF;
-        const float4 q0 = __ldg(&m.triVerts[i * 3 + 0]);
-        const float4 q1 = __ldg(&m.triVerts[i * 3 + 1]);
-        const float4 q2 = __ldg(&m.triVerts[i * 3 + 2]);
+    for (uint32_t ref = first; (ref & TB_LEAF) && !occluded; ref = second, second = 0u) {
         float t, u, v, w, sign;
         V3 n;
         // a triangle with 0 < t < tmax is recorded unless an earlier record is already below it, so either way the
         // mesh's closest t is below tmax
-        occluded = ray_tri(origin, dir, v3(q0.x, q0.y, q0.z), v3(q0.w, q1.x, q1.y), v3(q1.z, q1.w, q2.x), t, u, v, w, sign, n) &&
-                   t > 0.0f && t < tmax;
+        occluded = tri_hit(m, ref & ~TB_LEAF, origin, dir, t, u, v, w, sign, n) && t > 0.0f && t < tmax;
     }
     return true;
 }
@@ -807,15 +772,13 @@ TB_DEV bool prim_occludes(const DScene& sc, const DPrim& p, V3 o, V3 d, float ti
 }
 
 // trace_ordered()'s stack walk, stopping at the first primitive that occludes.  The near-first order is kept only
-// because it tends to find a blocker sooner.
+// because it tends to find a blocker sooner.  This walk and trace_occluded()'s op loop stay separate from
+// trace_ordered()'s and trace_closest()'s: sharing them through a template that takes the query's action changed
+// the closest-hit kernels' register allocation and cost the cornell benchmark 3 % (DESIGN §5.7).
 template <uint32_t FEAT = TB_FEAT_ALL>
 TB_ORDERED_ATTR bool occluded_ordered(const DScene& sc, V3 o, V3 d, float time, float tmax)
 {
-    V3 rcp;
-    rcp.x = 1.0f / d.x;
-    rcp.y = 1.0f / d.y;
-    rcp.z = 1.0f / d.z;
-
+    const V3 rcp = ray_rcp(d);
     uint32_t stack[TB_STACK];
     stack[0] = sc.rootRef;
     int count = 1;
@@ -851,14 +814,9 @@ TB_DEV bool trace_occluded(const DScene& sc, V3 o, V3 d, float time, float tmax)
     if (!(tmax > 0.0f)) return false;
     if (tmax > FLT_MAX) tmax = FLT_MAX;   // Trace records only t < FLT_MAX
     const int n = sc.numFlat;
-    const bool guard = (fabsf(o.x) < 1.0e7f) & (fabsf(o.y) < 1.0e7f) & (fabsf(o.z) < 1.0e7f) & (d.x == d.x) & (d.y == d.y) &
-                       (d.z == d.z);
-    if (n == 0 || !guard) return occluded_ordered<FEAT>(sc, o, d, time, tmax);
+    if (n == 0 || !flat_guard(o, d)) return occluded_ordered<FEAT>(sc, o, d, time, tmax);
 
-    V3 rcp;
-    rcp.x = 1.0f / d.x;
-    rcp.y = 1.0f / d.y;
-    rcp.z = 1.0f / d.z;
+    const V3 rcp = ray_rcp(d);
     uint32_t visited = 0u;
     for (int i = 0; i < n; ++i) {
         const float4 a = *reinterpret_cast<const float4*>(sc.flat[i].a);

@@ -97,12 +97,9 @@ TB_DEV void wf2_push_trace(Wf2Shared& S, const DScene& sc, bool split, int q, bo
             o = o + d * S.ht[s];
             d = v3(S.sdx[s], S.sdy[s], S.sdz[s]);
         }
-        V3 rcp;
-        rcp.x = 1.0f / d.x;
-        rcp.y = 1.0f / d.y;
-        rcp.z = 1.0f / d.z;
+        const V3 rcp = ray_rcp(d);
         float t;
-        big = ray_aabb(o, rcp, sc.splitLo.x, sc.splitLo.y, sc.splitLo.z, sc.splitHi.x, sc.splitHi.y, sc.splitHi.z, t);
+        big = ray_aabb(o, rcp,sc.splitLo.x, sc.splitLo.y, sc.splitLo.z, sc.splitHi.x, sc.splitHi.y, sc.splitHi.z, t);
     }
     wf2_push(S, q, flag && !big, s);
     wf2_push(S, WF2_Q_TM, flag && big, s);
