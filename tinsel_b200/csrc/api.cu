@@ -46,17 +46,27 @@ bool set_error(const std::string& what)
         }                                                                                               \
     } while (0)
 
+// Owners of one cudaMalloc'd (DevPtr) or cudaHostAlloc'd (HostPtr) allocation.  Moving an owner keeps the address.
+struct CudaFree {
+    void operator()(void* p) const { cudaFree(p); }
+};
+struct CudaFreeHost {
+    void operator()(void* p) const { cudaFreeHost(p); }
+};
 template <typename T>
-bool upload(const std::vector<T>& host, T** dev, uint64_t* h2d, size_t padElems = 0)
+using DevPtr = std::unique_ptr<T, CudaFree>;
+template <typename T>
+using HostPtr = std::unique_ptr<T, CudaFreeHost>;
+
+// *out = a new allocation of n elements.  What *out held is freed first, so that a resize never holds both.
+template <typename T>
+cudaError_t dev_alloc(DevPtr<T>* out, size_t n)
 {
-    *dev = nullptr;
-    const size_t n = host.size() + padElems;
-    if (n == 0) return true;
-    TB_CUDA(cudaMalloc((void**)dev, n * sizeof(T)));
-    if (padElems) TB_CUDA(cudaMemset(*dev, 0, n * sizeof(T)));
-    if (!host.empty()) TB_CUDA(cudaMemcpy(*dev, host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice));
-    *h2d += host.size() * sizeof(T);
-    return true;
+    out->reset();
+    T* p = nullptr;
+    const cudaError_t e = cudaMalloc((void**)&p, n * sizeof(T));
+    if (e == cudaSuccess) out->reset(p);
+    return e;
 }
 
 V3 hv3(const float* f) { return v3(f[0], f[1], f[2]); }
@@ -251,38 +261,35 @@ struct tb200_renderer {
     float4* boundAccum = nullptr;         // caller-owned accumulator (tb200_bind_accumulator)
     cudaEvent_t evStart = nullptr, evStop = nullptr;
 
-    // device scene
+    // Device memory.  Every owner frees its allocation when it is reset, reassigned or destroyed; tb200_destroy
+    // releases them all at once, with the renderer's device current and before its streams go.
+    struct Memory {
+        std::vector<DevPtr<void>> scene;   // the scene's arrays (`scene` below points into them)
+        DevPtr<float4> accum;
+        DevPtr<float> radiance, raster;   // tb200_trace_frame scratch, allocated on first use per image size
+        DevPtr<unsigned long long> counter;
+        DevPtr<float4> cold;              // cold half of the wavefront's slot state (wf2_common.cuh): 128 B per slot
+        DevPtr<float4> filtered;          // tb200_finish, per image size
+        DevPtr<unsigned char> rgb8;
+        DevPtr<uint2> dither;
+        DevPtr<float4> means, denoised;   // tb200_nlm scratch + output, allocated on first use per finish size
+        DevPtr<unsigned int> bandCount;   // streamed read-back: band counters on the device,
+        HostPtr<unsigned int> bandFlags;  // completion flags in mapped host memory
+    } mem;
+
     DScene scene;
-    DPrim* dPrims = nullptr;
-    BvhPair* dScenePairs = nullptr;
-    ProgOp* dFlat = nullptr;
-    DMesh* dMeshes = nullptr;
-    std::vector<void*> owned;   // every other device allocation
 
     // film
     int width = 0, height = 0;
-    float4* dAccum = nullptr;
-    float* dRadiance = nullptr;   // tb200_trace_frame scratch
-    float* dRaster = nullptr;
-    unsigned long long* dCounter = nullptr;
-    float4* dCold = nullptr;      // cold half of the wavefront's slot state (wf2_common.cuh): 128 B per slot
     int frame = 0;
 
     // display/finish step (tb200_finish)
-    float4* dFiltered = nullptr;
-    unsigned char* dRgb8 = nullptr;
-    uint2* dDither = nullptr;
-    float4* dMeans = nullptr;                // tb200_nlm scratch + output
-    float4* dDenoised = nullptr;
-    int finishWidth = 0, finishHeight = 0;   // size the buffers above were made for
+    int finishWidth = 0, finishHeight = 0;   // size mem.filtered, rgb8 and dither were made for
     bool ditherReady = false;
-    bool filteredValid = false;              // dFiltered holds the image of a tb200_finish since the last tb200_init
+    bool filteredValid = false;              // mem.filtered holds the image of a tb200_finish since the last tb200_init
 
-    // streamed read-back (tb200_render): band counters on the device, completion flags in mapped
-    // host memory, a private copy stream
-    unsigned int* dBandCount = nullptr;
-    volatile unsigned int* hBandFlags = nullptr;
-    unsigned int* dBandFlags = nullptr;   // device alias of hBandFlags
+    // streamed read-back (tb200_render): the band flags' device alias and a private copy stream
+    unsigned int* dBandFlags = nullptr;
     cudaStream_t copyStream = nullptr;
     unsigned int bandTag = 0;
     int streamedReadback = 1;             // TINSEL_B200_READBACK=plain turns it off
@@ -316,50 +323,6 @@ struct tb200_renderer {
 };
 
 namespace {
-
-void free_device(tb200_renderer* r)
-{
-    if (r->registered) {
-        cudaHostUnregister(r->registered);
-        r->registered = nullptr;
-    }
-    for (void* p : r->owned) cudaFree(p);
-    r->owned.clear();
-    cudaFree(r->dPrims);
-    cudaFree(r->dScenePairs);
-    cudaFree(r->dFlat);
-    r->dFlat = nullptr;
-    cudaFree(r->dMeshes);
-    cudaFree(r->dAccum);
-    cudaFree(r->dRadiance);
-    cudaFree(r->dRaster);
-    cudaFree(r->dCounter);
-    r->dCounter = nullptr;
-    cudaFree(r->dCold);
-    r->dCold = nullptr;
-    cudaFree(r->dBandCount);
-    r->dBandCount = nullptr;
-    cudaFree(r->dFiltered);
-    cudaFree(r->dRgb8);
-    cudaFree(r->dDither);
-    cudaFree(r->dMeans);
-    cudaFree(r->dDenoised);
-    r->dFiltered = nullptr;
-    r->dRgb8 = nullptr;
-    r->dDither = nullptr;
-    r->dMeans = r->dDenoised = nullptr;
-    r->finishWidth = r->finishHeight = 0;
-    r->ditherReady = false;
-    r->filteredValid = false;
-    if (r->hBandFlags) cudaFreeHost((void*)r->hBandFlags);
-    r->hBandFlags = nullptr;
-    r->dBandFlags = nullptr;
-    r->dPrims = nullptr;
-    r->dScenePairs = nullptr;
-    r->dMeshes = nullptr;
-    r->dAccum = nullptr;
-    r->dRadiance = r->dRaster = nullptr;
-}
 
 // ---------------------------------------------------------------------------------------------------
 // Scene image: everything build_scene() derives from a tb200_scene, in exactly the layouts the device
@@ -514,50 +477,52 @@ uint32_t scene_features(const SceneImage& img)
     return f;
 }
 
+// Copies `host` and padElems zeroed elements after it into a new allocation of r's scene memory; *dev = its
+// address, null for no elements
+template <typename T>
+bool upload(tb200_renderer* r, const std::vector<T>& host, const T** dev, size_t padElems = 0)
+{
+    *dev = nullptr;
+    const size_t n = host.size() + padElems;
+    if (n == 0) return true;
+    DevPtr<T> mem;
+    TB_CUDA(dev_alloc(&mem, n));
+    if (padElems) TB_CUDA(cudaMemset(mem.get(), 0, n * sizeof(T)));
+    if (!host.empty()) TB_CUDA(cudaMemcpy(mem.get(), host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice));
+    r->stats.h2dBytes += host.size() * sizeof(T);
+    *dev = mem.get();
+    r->mem.scene.push_back(std::move(mem));
+    return true;
+}
+
 // device upload of a scene image + the per-scene scheduling decisions (which read the environment)
 bool upload_image(tb200_renderer* r, const SceneImage& img)
 {
-    uint64_t* h2d = &r->stats.h2dBytes;
     memset(&r->scene, 0, sizeof(r->scene));
     std::vector<DMesh> meshes(img.meshes.size());
     for (size_t m = 0; m < img.meshes.size(); ++m) {
         const MeshImage& mi = img.meshes[m];
-        BvhPair* dPairs;
-        float4 *dVerts, *dNorms;
-        float* dCdf;
-        if (!upload(mi.pairs, &dPairs, h2d) || !upload(mi.verts, &dVerts, h2d) || !upload(mi.norms, &dNorms, h2d) ||
-            !upload(mi.cdf, &dCdf, h2d))
+        if (!upload(r, mi.pairs, &meshes[m].pairs) || !upload(r, mi.verts, &meshes[m].triVerts) ||
+            !upload(r, mi.norms, &meshes[m].triNormals) || !upload(r, mi.cdf, &meshes[m].cdf))
             return false;
-        r->owned.push_back(dPairs);
-        r->owned.push_back(dVerts);
-        r->owned.push_back(dNorms);
-        r->owned.push_back(dCdf);
-        meshes[m].pairs = dPairs;
-        meshes[m].triVerts = dVerts;
-        meshes[m].triNormals = dNorms;
-        meshes[m].cdf = dCdf;
         meshes[m].numTris = mi.numTris;
         meshes[m].rootRef = mi.rootRef;
     }
-    if (!upload(meshes, &r->dMeshes, h2d)) return false;
-    r->scene.splitValid = img.splitBoxValid;
-    r->scene.splitLo = img.splitLo;
-    r->scene.splitHi = img.splitHi;
+    DScene& sc = r->scene;
+    if (!upload(r, meshes, &sc.meshes)) return false;
+    sc.splitValid = img.splitBoxValid;
+    sc.splitLo = img.splitLo;
+    sc.splitHi = img.splitHi;
     r->route = wavefront2_route(img.numNee, img.maxTris, img.splitBoxValid, scene_features(img));
     r->tunePhase = r->route.tune ? 0 : 3;
     // one element of padding each: the kernels' bulk copies round their length up to 16 bytes
-    if (!upload(img.prims, &r->dPrims, h2d, 1)) return false;
-    if (!upload(img.scenePairs, &r->dScenePairs, h2d, 1)) return false;
-
-    DScene& sc = r->scene;
-    sc.prims = r->dPrims;
+    if (!upload(r, img.prims, &sc.prims, 1)) return false;
+    if (!upload(r, img.scenePairs, &sc.pairs, 1)) return false;
     sc.numPrims = (int)img.prims.size();
-    sc.pairs = r->dScenePairs;
     sc.numPairs = (int)img.scenePairs.size();
     static const std::vector<ProgOp> noFlat;
     const std::vector<ProgOp>& flat = getenv("TINSEL_B200_NO_FLAT") ? noFlat : img.flat;
-    if (!upload(flat, &r->dFlat, h2d, 1)) return false;
-    sc.flat = r->dFlat;
+    if (!upload(r, flat, &sc.flat, 1)) return false;
     sc.numFlat = (int)flat.size();
     // treelet: the top of the largest mesh's BVH staged in the shared memory the slot arrays leave, for the
     // mesh walk.  Measured in round 2: slower on every scene (ajax, env, meshlight) because the top levels already
@@ -576,30 +541,17 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
         }
     }
     sc.rootRef = img.sceneRoot;
-    sc.meshes = r->dMeshes;
     sc.numMeshes = (int)img.meshes.size();
     sc.horizon = img.horizon;
     sc.zenith = img.zenith;
     sc.numNee = img.numNee;
     if (img.probeValid) {
-        float4* dData;
-        float *dPdfX, *dCdfX, *dPdfY, *dCdfY;
-        if (!upload(img.probeData, &dData, h2d) || !upload(img.pdfX, &dPdfX, h2d) || !upload(img.cdfX, &dCdfX, h2d) ||
-            !upload(img.pdfY, &dPdfY, h2d) || !upload(img.cdfY, &dCdfY, h2d))
+        if (!upload(r, img.probeData, &sc.probe.data) || !upload(r, img.pdfX, &sc.probe.pdfX) || !upload(r, img.cdfX, &sc.probe.cdfX) ||
+            !upload(r, img.pdfY, &sc.probe.pdfY) || !upload(r, img.cdfY, &sc.probe.cdfY))
             return false;
-        r->owned.push_back(dData);
-        r->owned.push_back(dPdfX);
-        r->owned.push_back(dCdfX);
-        r->owned.push_back(dPdfY);
-        r->owned.push_back(dCdfY);
         sc.probe.valid = 1;
         sc.probe.width = img.probeW;
         sc.probe.height = img.probeH;
-        sc.probe.data = dData;
-        sc.probe.pdfX = dPdfX;
-        sc.probe.cdfX = dCdfX;
-        sc.probe.pdfY = dPdfY;
-        sc.probe.cdfY = dCdfY;
     }
     return true;
 }
@@ -621,42 +573,64 @@ struct CacheStamp {
     uint32_t version, sizeofPrim, sizeofPair, sizeofOp;
 };
 
-template <typename T>
-bool put_vec(FILE* f, const std::vector<T>& v)
-{
-    const uint64_t n = v.size();
-    return fwrite(&n, 8, 1, f) == 1 && (n == 0 || fwrite(v.data(), sizeof(T), n, f) == n);
-}
-template <typename T>
-bool put_pod(FILE* f, const T& v) { return fwrite(&v, sizeof(T), 1, f) == 1; }
+struct CacheWriter {
+    FILE* f;
+    template <typename T>
+    bool pod(const T& v) { return fwrite(&v, sizeof(T), 1, f) == 1; }
+    template <typename T>
+    bool vec(const std::vector<T>& v)
+    {
+        const uint64_t n = v.size();
+        return pod(n) && (n == 0 || fwrite(v.data(), sizeof(T), n, f) == n);
+    }
+    bool count(const std::vector<MeshImage>& v) { return pod(uint64_t(v.size())); }
+};
 
-template <typename T>
-bool get_vec(FILE* f, std::vector<T>* v, uint64_t fileBytes)
+// Every count is checked against the file's size before anything is allocated for it.
+struct CacheReader {
+    FILE* f;
+    uint64_t fileBytes;
+    template <typename T>
+    bool pod(T& v) { return fread(&v, sizeof(T), 1, f) == 1; }
+    template <typename T>
+    bool vec(std::vector<T>& v)
+    {
+        uint64_t n = 0;
+        if (!pod(n) || n > fileBytes / sizeof(T)) return false;   // a count can never exceed the file
+        v.resize(size_t(n));
+        return n == 0 || fread(v.data(), sizeof(T), size_t(n), f) == n;
+    }
+    bool count(std::vector<MeshImage>& v)
+    {
+        uint64_t n = 0;
+        if (!pod(n) || n > fileBytes) return false;
+        v.resize(size_t(n));
+        return true;
+    }
+};
+
+// The SceneImage fields in file order, for a CacheWriter (Image = const SceneImage) or a CacheReader: the one
+// statement of the format after the stamp.  vec(v) is a 64-bit count followed by the elements; count(meshes) is
+// the number of meshes, whose fields follow mesh by mesh.
+template <typename IO, typename Image>
+bool cache_fields(IO& io, Image& img)
 {
-    uint64_t n = 0;
-    if (fread(&n, 8, 1, f) != 1 || n > fileBytes / sizeof(T)) return false;   // a count can never exceed the file
-    v->resize(size_t(n));
-    return n == 0 || fread(v->data(), sizeof(T), size_t(n), f) == n;
+    bool ok = io.vec(img.prims) && io.vec(img.scenePairs) && io.pod(img.sceneRoot) && io.vec(img.flat) && io.count(img.meshes);
+    for (auto& m : img.meshes)
+        ok = ok && io.vec(m.pairs) && io.vec(m.verts) && io.vec(m.norms) && io.vec(m.cdf) && io.pod(m.numTris) && io.pod(m.rootRef) &&
+             io.pod(m.depth);
+    return ok && io.pod(img.horizon) && io.pod(img.zenith) && io.pod(img.numNee) && io.pod(img.maxTris) && io.pod(img.splitBoxValid) &&
+           io.pod(img.splitLo) && io.pod(img.splitHi) && io.pod(img.probeValid) && io.pod(img.probeW) && io.pod(img.probeH) &&
+           io.vec(img.probeData) && io.vec(img.pdfX) && io.vec(img.cdfX) && io.vec(img.pdfY) && io.vec(img.cdfY);
 }
-template <typename T>
-bool get_pod(FILE* f, T* v) { return fread(v, sizeof(T), 1, f) == 1; }
 
 bool image_save(const SceneImage& img, const char* path)
 {
     FILE* f = fopen(path, "wb");
     if (!f) return set_error(std::string("tb200_scene_cache_save: cannot open ") + path);
     const CacheStamp stamp = {kCacheVersion, (uint32_t)sizeof(DPrim), (uint32_t)sizeof(BvhPair), (uint32_t)sizeof(ProgOp)};
-    bool ok = fwrite(kCacheMagic, 1, 8, f) == 8 && put_pod(f, stamp);
-    ok = ok && put_vec(f, img.prims) && put_vec(f, img.scenePairs) && put_pod(f, img.sceneRoot) && put_vec(f, img.flat);
-    const uint64_t numMeshes = img.meshes.size();
-    ok = ok && put_pod(f, numMeshes);
-    for (const MeshImage& m : img.meshes)
-        ok = ok && put_vec(f, m.pairs) && put_vec(f, m.verts) && put_vec(f, m.norms) && put_vec(f, m.cdf) && put_pod(f, m.numTris) &&
-             put_pod(f, m.rootRef) && put_pod(f, m.depth);
-    ok = ok && put_pod(f, img.horizon) && put_pod(f, img.zenith) && put_pod(f, img.numNee) && put_pod(f, img.maxTris) &&
-         put_pod(f, img.splitBoxValid) && put_pod(f, img.splitLo) && put_pod(f, img.splitHi);
-    ok = ok && put_pod(f, img.probeValid) && put_pod(f, img.probeW) && put_pod(f, img.probeH) && put_vec(f, img.probeData) &&
-         put_vec(f, img.pdfX) && put_vec(f, img.cdfX) && put_vec(f, img.pdfY) && put_vec(f, img.cdfY);
+    CacheWriter w{f};
+    bool ok = fwrite(kCacheMagic, 1, 8, f) == 8 && w.pod(stamp) && cache_fields(w, img);
     ok = (fclose(f) == 0) && ok;
     return ok ? true : set_error(std::string("tb200_scene_cache_save: write failed: ") + path);
 }
@@ -670,27 +644,14 @@ bool image_load(const char* path, SceneImage* img)
     fseek(f, 0, SEEK_SET);
     char magic[8];
     CacheStamp stamp;
-    bool ok = fread(magic, 1, 8, f) == 8 && memcmp(magic, kCacheMagic, 8) == 0 && get_pod(f, &stamp);
+    CacheReader rd{f, fileBytes};
+    bool ok = fread(magic, 1, 8, f) == 8 && memcmp(magic, kCacheMagic, 8) == 0 && rd.pod(stamp);
     if (ok && (stamp.version != kCacheVersion || stamp.sizeofPrim != sizeof(DPrim) || stamp.sizeofPair != sizeof(BvhPair) ||
                stamp.sizeofOp != sizeof(ProgOp))) {
         fclose(f);
         return set_error(std::string("tb200_create_cached: ") + path + " was written by another build of this library (layout stamp differs): recreate it");
     }
-    ok = ok && get_vec(f, &img->prims, fileBytes) && get_vec(f, &img->scenePairs, fileBytes) && get_pod(f, &img->sceneRoot) &&
-         get_vec(f, &img->flat, fileBytes);
-    uint64_t numMeshes = 0;
-    ok = ok && get_pod(f, &numMeshes) && numMeshes <= fileBytes;
-    if (ok) img->meshes.resize(size_t(numMeshes));
-    for (size_t m = 0; ok && m < img->meshes.size(); ++m) {
-        MeshImage& mi = img->meshes[m];
-        ok = get_vec(f, &mi.pairs, fileBytes) && get_vec(f, &mi.verts, fileBytes) && get_vec(f, &mi.norms, fileBytes) &&
-             get_vec(f, &mi.cdf, fileBytes) && get_pod(f, &mi.numTris) && get_pod(f, &mi.rootRef) && get_pod(f, &mi.depth);
-    }
-    ok = ok && get_pod(f, &img->horizon) && get_pod(f, &img->zenith) && get_pod(f, &img->numNee) && get_pod(f, &img->maxTris) &&
-         get_pod(f, &img->splitBoxValid) && get_pod(f, &img->splitLo) && get_pod(f, &img->splitHi);
-    ok = ok && get_pod(f, &img->probeValid) && get_pod(f, &img->probeW) && get_pod(f, &img->probeH) && get_vec(f, &img->probeData, fileBytes) &&
-         get_vec(f, &img->pdfX, fileBytes) && get_vec(f, &img->cdfX, fileBytes) && get_vec(f, &img->pdfY, fileBytes) &&
-         get_vec(f, &img->cdfY, fileBytes);
+    ok = ok && cache_fields(rd, *img);
     fclose(f);
     if (!ok) return set_error(std::string("tb200_create_cached: truncated or malformed cache file ") + path);
     return true;
@@ -779,7 +740,7 @@ bool filter_options_ok(const tb200_options* o)
 
 bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_options* o, LaunchParams* P)
 {
-    if (!r->dAccum) return set_error("tb200_init has not been called");
+    if (!r->mem.accum) return set_error("tb200_init has not been called");
     if (o->width != r->width || o->height != r->height)
         return set_error("options.width/height differ from the last tb200_init");
     if (!filter_options_ok(o)) return false;
@@ -795,9 +756,9 @@ bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_opti
     P->film.clamp = o->clamp;
     P->film.maxDepth = o->maxDepth;
     P->film.filterArgZero = film_filter_arg_zero(o->filterOffset);
-    P->accum = r->boundAccum ? r->boundAccum : r->dAccum;
-    P->sampleCounter = r->dCounter;
-    P->cold = r->dCold;
+    P->accum = r->boundAccum ? r->boundAccum : r->mem.accum.get();
+    P->sampleCounter = r->mem.counter.get();
+    P->cold = r->mem.cold.get();
     P->firstRow = 0;
     P->numRows = o->height;
     P->film.rowLo = 0;
@@ -865,13 +826,13 @@ void tune_update(tb200_renderer* r)
     if (r->tunePhase >= 2) r->route.split = r->tunePhase == 3 && r->tuneRate[0] >= r->tuneRate[1];
 }
 
-bool finish_timing(tb200_renderer* r)
+// waits for the work between evStart and evStop and sets stats.gpuMs to its time
+bool sync_gpu_ms(tb200_renderer* r)
 {
-    TB_CUDA(cudaStreamSynchronize(r->stream));
+    TB_CUDA(cudaEventSynchronize(r->evStop));
     float ms = 0.0f;
     TB_CUDA(cudaEventElapsedTime(&ms, r->evStart, r->evStop));
     r->stats.gpuMs = ms;
-    tune_update(r);
     return true;
 }
 
@@ -896,7 +857,7 @@ bool read_back(tb200_renderer* r, float* output)
     owned_rows(r, &row0, &row1);
     const size_t rowBytes = size_t(r->width) * sizeof(float4);
     const size_t bytes = size_t(row1 - row0) * rowBytes;
-    const char* accum = (const char*)(r->boundAccum ? r->boundAccum : r->dAccum);
+    const char* accum = (const char*)(r->boundAccum ? r->boundAccum : r->mem.accum.get());
     if (bytes)
         TB_CUDA(cudaMemcpyAsync((char*)output + size_t(row0) * rowBytes, accum + size_t(row0) * rowBytes, bytes, cudaMemcpyDeviceToHost, r->stream));
     TB_CUDA(cudaStreamSynchronize(r->stream));
@@ -909,7 +870,7 @@ bool read_back(tb200_renderer* r, float* output)
 // (wf2_common.cuh, wf2_band_report), and this thread copies every owned pixel row that no
 // unfinished sample can still touch while the kernel is tracing the rest.  What is left when the
 // kernel ends is the last band or two instead of the whole slab.
-bool render_streamed(tb200_renderer* r, LaunchParams& P, float* output, bool recordStart = true)
+bool render_streamed(tb200_renderer* r, LaunchParams& P, float* output, bool recordStart)
 {
     const float4* accum = P.accum;
     const size_t rowBytes = size_t(r->width) * sizeof(float4);
@@ -924,14 +885,15 @@ bool render_streamed(tb200_renderer* r, LaunchParams& P, float* output, bool rec
 
     r->bandTag += 1;
     if (r->bandTag == 0) r->bandTag = 1;
-    P.bandCount = r->dBandCount;
+    P.bandCount = r->mem.bandCount.get();
     P.bandFlags = r->dBandFlags;
     P.bandSamples = (unsigned)bandTileRows * (unsigned)P.tilesX * 32u;
     P.bandTag = r->bandTag;
     if (recordStart) TB_CUDA(cudaEventRecord(r->evStart, r->stream));
-    TB_CUDA(cudaMemsetAsync(r->dBandCount, 0, TB_MAX_BANDS * sizeof(unsigned int), r->stream));
+    TB_CUDA(cudaMemsetAsync(P.bandCount, 0, TB_MAX_BANDS * sizeof(unsigned int), r->stream));
     if (!launch_frames(r, P, false)) return false;
 
+    const volatile unsigned int* bandFlags = r->mem.bandFlags.get();
     int done = 0;          // bands 0..done-1 are complete
     int copied = own0;     // owned pixel rows [own0, copied) are already on their way to the host
     bool copyFailed = false;
@@ -945,7 +907,7 @@ bool render_streamed(tb200_renderer* r, LaunchParams& P, float* output, bool rec
     };
     unsigned spins = 0;
     for (;;) {
-        while (done < numBands && r->hBandFlags[done] == r->bandTag) ++done;
+        while (done < numBands && bandFlags[done] == r->bandTag) ++done;
         if (done >= numBands) break;
         // unfinished samples sit in local tile rows >= done*bandTileRows, i.e. global pixel rows
         // >= firstRow + done*bandTileRows*numShards*4 (decode_sample)
@@ -966,6 +928,30 @@ bool render_streamed(tb200_renderer* r, LaunchParams& P, float* output, bool rec
     TB_CUDA(cudaStreamSynchronize(r->copyStream));
     if (copyFailed) TB_CUDA(cudaErrorUnknown);
     r->stats.d2hBytes += size_t(own1 - own0) * rowBytes;
+    return true;
+}
+
+// Runs frames r->frame .. r->frame + n - 1 (n >= 1) of P, filled by fill_params, and sets stats.gpuMs to the time
+// from the first launch to the end of the last.  With `output`, the caller's whole image, it also delivers the owned
+// rows there: streamed under the last frame when the wavefront kernel runs it and its sample indices fit in 31 bits,
+// else copied after the frames.  The frame counters advance only when all of this succeeded.
+bool run_frames(tb200_renderer* r, LaunchParams& P, int n, float* output)
+{
+    const bool streamed = output && r->streamedReadback && r->pipeline != 0 && P.samplesPerFrame > 0 && P.samplesPerFrame < 0x7fffffffull;
+    const int head = streamed ? n - 1 : n;   // frames launched before the streamed one
+    P.frame0 = r->frame;
+    P.numFrames = head;
+    if (head > 0 && !launch_frames(r, P)) return false;
+    if (streamed) {
+        P.frame0 = r->frame + head;
+        P.numFrames = 1;
+        if (!render_streamed(r, P, output, head == 0)) return false;
+    } else if (output && !read_back(r, output)) {
+        return false;
+    }
+    if (!sync_gpu_ms(r)) return false;
+    r->frame += n;
+    r->stats.frames += n;
     return true;
 }
 
@@ -1233,20 +1219,18 @@ static tb200_renderer* create_with(int device, const std::function<bool(tb200_re
         if (n > 0) r->maxLaunchSamples = std::min(n, r->maxLaunchSamples);
     }
     unsigned int* hostFlags = nullptr;
-    // cold slot state for every CTA a launch can have (one or two per SM, see launch_wavefront2)
-    if (cudaMalloc((void**)&r->dCold, size_t(r->numSMs) * TB_WF2_MAX_CTAS_PER_SM * TB_WF2_SLOTS * 128) != cudaSuccess ||
-        cudaMalloc((void**)&r->dCounter, sizeof(unsigned long long)) != cudaSuccess ||
-        cudaMalloc((void**)&r->dBandCount, TB_MAX_BANDS * sizeof(unsigned int)) != cudaSuccess ||
-        cudaHostAlloc((void**)&hostFlags, TB_MAX_BANDS * sizeof(unsigned int), cudaHostAllocMapped) != cudaSuccess ||
-        cudaHostGetDevicePointer((void**)&r->dBandFlags, hostFlags, 0) != cudaSuccess ||
+    // cold slot state for every CTA a launch can have (one or two per SM, see launch_wavefront2): 8 float4 per slot
+    ok = dev_alloc(&r->mem.cold, size_t(r->numSMs) * TB_WF2_MAX_CTAS_PER_SM * TB_WF2_SLOTS * 8) == cudaSuccess &&
+         dev_alloc(&r->mem.counter, 1) == cudaSuccess && dev_alloc(&r->mem.bandCount, TB_MAX_BANDS) == cudaSuccess &&
+         cudaHostAlloc((void**)&hostFlags, TB_MAX_BANDS * sizeof(unsigned int), cudaHostAllocMapped) == cudaSuccess;
+    if (ok) r->mem.bandFlags.reset(hostFlags);
+    if (!ok || cudaHostGetDevicePointer((void**)&r->dBandFlags, hostFlags, 0) != cudaSuccess ||
         cudaStreamCreateWithFlags(&r->copyStream, cudaStreamNonBlocking) != cudaSuccess) {
         set_error("tb200_create: counter allocation failed");
-        if (hostFlags) cudaFreeHost(hostFlags);
         tb200_destroy(r);
         return nullptr;
     }
     memset(hostFlags, 0, TB_MAX_BANDS * sizeof(unsigned int));
-    r->hBandFlags = hostFlags;
     if (!build(r)) {
         tb200_destroy(r);
         return nullptr;
@@ -1306,20 +1290,17 @@ static int init_one(tb200_renderer* r, int width, int height)
 {
     cudaSetDevice(r->device);
     const size_t n = size_t(width) * height;
-    if (width != r->width || height != r->height || !r->dAccum) {
-        cudaFree(r->dAccum);
-        cudaFree(r->dRadiance);
-        cudaFree(r->dRaster);
-        r->dAccum = nullptr;
-        r->dRadiance = r->dRaster = nullptr;
-        if (cudaMalloc((void**)&r->dAccum, n * sizeof(float4)) != cudaSuccess) {
+    if (width != r->width || height != r->height || !r->mem.accum) {
+        r->mem.radiance.reset();
+        r->mem.raster.reset();
+        if (dev_alloc(&r->mem.accum, n) != cudaSuccess) {
             set_error("tb200_init: accumulator allocation failed");
             return -1;
         }
         r->width = width;
         r->height = height;
     }
-    if (cudaMemsetAsync(r->dAccum, 0, n * sizeof(float4), r->stream) != cudaSuccess ||
+    if (cudaMemsetAsync(r->mem.accum.get(), 0, n * sizeof(float4), r->stream) != cudaSuccess ||
         cudaStreamSynchronize(r->stream) != cudaSuccess) {
         set_error("tb200_init: accumulator clear failed");
         return -1;
@@ -1337,23 +1318,24 @@ int tb200_init(tb200_renderer* r, int width, int height)
         set_error("tb200_init: bad arguments");
         return -1;
     }
-    if (r->peers.empty()) return init_one(r, width, height);
-    // multi-device: contiguous row slabs cut at tile rows, one per device
-    const int n = (int)r->peers.size() + 1;
-    r->slabRow0 = 0;
-    r->slabRows = slab_cut(height, 1, n);
-    for (int k = 1; k < n; ++k) {
-        r->peers[k - 1]->slabRow0 = slab_cut(height, k, n);
-        r->peers[k - 1]->slabRows = slab_cut(height, k + 1, n) - slab_cut(height, k, n);
+    if (!r->peers.empty()) {
+        // multi-device: contiguous row slabs cut at tile rows, one per device
+        const int n = (int)r->peers.size() + 1;
+        r->slabRow0 = 0;
+        r->slabRows = slab_cut(height, 1, n);
+        for (int k = 1; k < n; ++k) {
+            r->peers[k - 1]->slabRow0 = slab_cut(height, k, n);
+            r->peers[k - 1]->slabRows = slab_cut(height, k + 1, n) - slab_cut(height, k, n);
+        }
     }
     return group_run(r, [=](tb200_renderer* m) { return init_one(m, width, height); });
 }
 
-static int render_one(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options, float* output)
+static bool render_one(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options, float* output)
 {
     cudaSetDevice(r->device);
     LaunchParams P;
-    if (!fill_params(r, camera, options, &P)) return -1;
+    if (!fill_params(r, camera, options, &P)) return false;
     if (options->mode == TB200_MODE_NORMALS) {
         unsigned long long launches = 0;
         if (r->slabRows >= 0) {
@@ -1362,35 +1344,19 @@ static int render_one(tb200_renderer* r, const tb200_camera* camera, const tb200
             P.numRows = P.film.rowHi - P.film.rowLo;
             finalize_params(&P);
         }
-        cudaEventRecord(r->evStart, r->stream);
+        TB_CUDA(cudaEventRecord(r->evStart, r->stream));
         launch_normals(P, r->stream, &launches);
-        cudaEventRecord(r->evStop, r->stream);
+        TB_CUDA(cudaEventRecord(r->evStop, r->stream));
+        TB_CUDA(cudaGetLastError());
         r->stats.kernelLaunches += launches;
-    } else {
-        P.frame0 = r->frame;
-        P.numFrames = 1;
-        const bool streamed = r->streamedReadback && r->pipeline != 0 && P.samplesPerFrame > 0 && P.samplesPerFrame < 0x7fffffffull;
-        if (streamed) {
-            if (!render_streamed(r, P, output)) return -1;
-        } else if (!launch_frames(r, P)) {
-            return -1;
-        }
-        r->frame += 1;
-        r->stats.frames += 1;
-        if (streamed) {
-            float ms = 0.0f;
-            cudaEventElapsedTime(&ms, r->evStart, r->evStop);
-            r->stats.gpuMs = ms;
-            tune_update(r);
-            return 0;
-        }
+        return read_back(r, output) && sync_gpu_ms(r);
     }
-    if (!read_back(r, output)) return -1;
-    float ms = 0.0f;
-    cudaEventElapsedTime(&ms, r->evStart, r->evStop);
-    r->stats.gpuMs = ms;
-    if (options->mode == TB200_MODE_PATHTRACE) tune_update(r);
-    return 0;
+    if (!run_frames(r, P, 1, output)) return false;
+    // The tuner compares launchSamples with stats.gpuMs.  tb200_render_n does not call it: with a streamed read-back
+    // its gpuMs spans the launch of the first n - 1 frames and the last frame's launch, while launchSamples counts
+    // only the last frame's launch.
+    tune_update(r);
+    return true;
 }
 
 int tb200_render(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options, float* output)
@@ -1400,9 +1366,8 @@ int tb200_render(tb200_renderer* r, const tb200_camera* camera, const tb200_opti
         return -1;
     }
     if (options->mode == TB200_MODE_COMPLEXITY) return 0;   // render.cpp:516-519
-    if (r->peers.empty()) return render_one(r, camera, options, output);
     // every device traces its slab and streams its own rows into `output` over its own PCIe link
-    return group_run(r, [=](tb200_renderer* m) { return render_one(m, camera, options, output); });
+    return group_run(r, [=](tb200_renderer* m) { return render_one(m, camera, options, output) ? 0 : -1; });
 }
 
 static int render_device_one(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options, int spp,
@@ -1428,14 +1393,13 @@ static int render_device_one(tb200_renderer* r, const tb200_camera* camera, cons
         P.numRows = numRows;
         finalize_params(&P);
     }
-    P.frame0 = r->frame;
-    P.numFrames = spp;
-    if (spp > 0 && P.numRows > 0) {
-        if (!launch_frames(r, P)) return -1;
-        if (!finish_timing(r)) return -1;
+    if (spp == 0 || P.numRows <= 0) {   // nothing to trace: the frames count, stats.gpuMs keeps the last launch's time
+        r->frame += spp;
+        r->stats.frames += spp;
+        return 0;
     }
-    r->frame += spp;
-    r->stats.frames += spp;
+    if (!run_frames(r, P, spp, nullptr)) return -1;
+    tune_update(r);
     return 0;
 }
 
@@ -1446,7 +1410,6 @@ int tb200_render_device(tb200_renderer* r, const tb200_camera* camera, const tb2
         set_error("tb200_render_device: bad argument");
         return -1;
     }
-    if (r->peers.empty()) return render_device_one(r, camera, options, spp, firstRow, numRows);
     return group_run(r, [=](tb200_renderer* m) { return render_device_one(m, camera, options, spp, firstRow, numRows); });
 }
 
@@ -1532,7 +1495,7 @@ int tb200_unpin_output(tb200_renderer* r)
 
 int tb200_bind_accumulator(tb200_renderer* r, float* deviceAccum)
 {
-    if (!r || !r->dAccum) {
+    if (!r || !r->mem.accum) {
         set_error("tb200_bind_accumulator: call tb200_init first");
         return -1;
     }
@@ -1544,12 +1507,12 @@ int tb200_bind_accumulator(tb200_renderer* r, float* deviceAccum)
 float* tb200_device_accumulator(tb200_renderer* r)
 {
     if (!r) return nullptr;
-    return (float*)(r->boundAccum ? r->boundAccum : r->dAccum);
+    return (float*)(r->boundAccum ? r->boundAccum : r->mem.accum.get());
 }
 
 int tb200_read_accumulator(tb200_renderer* r, float* output)
 {
-    if (!r || !output || !r->dAccum) {
+    if (!r || !output || !r->mem.accum) {
         set_error("tb200_read_accumulator: bad argument");
         return -1;
     }
@@ -1561,7 +1524,7 @@ int tb200_read_accumulator(tb200_renderer* r, float* output)
 
 int tb200_gather_device(tb200_renderer* r)
 {
-    if (!r || !r->dAccum) {
+    if (!r || !r->mem.accum) {
         set_error("tb200_gather_device: call tb200_init first");
         return -1;
     }
@@ -1572,7 +1535,7 @@ int tb200_gather_device(tb200_renderer* r)
         owned_rows(p, &row0, &row1);
         if (row1 <= row0) continue;
         cudaSetDevice(p->device);
-        if (cudaMemcpyPeerAsync((char*)r->dAccum + size_t(row0) * rowBytes, r->device, (const char*)p->dAccum + size_t(row0) * rowBytes,
+        if (cudaMemcpyPeerAsync((char*)r->mem.accum.get() + size_t(row0) * rowBytes, r->device, (const char*)p->mem.accum.get() + size_t(row0) * rowBytes,
                                 p->device, size_t(row1 - row0) * rowBytes, p->stream) != cudaSuccess) {
             set_error(std::string("tb200_gather_device: ") + cudaGetErrorString(cudaGetLastError()));
             return -1;
@@ -1621,30 +1584,7 @@ static int render_n_one(tb200_renderer* r, const tb200_camera* camera, const tb2
 {
     cudaSetDevice(r->device);
     LaunchParams P;
-    if (!fill_params(r, camera, options, &P)) return -1;
-    // frames k .. k+n-2 in one launch, the last one with the read-back streamed underneath it
-    const bool streamed = r->streamedReadback && r->pipeline != 0 && P.samplesPerFrame > 0 && P.samplesPerFrame < 0x7fffffffull;
-    const int head = streamed ? n - 1 : n;
-    bool started = false;
-    if (head > 0) {
-        P.frame0 = r->frame;
-        P.numFrames = head;
-        if (!launch_frames(r, P)) return -1;
-        started = true;
-    }
-    if (streamed) {
-        P.frame0 = r->frame + head;
-        P.numFrames = 1;
-        if (!render_streamed(r, P, output, !started)) return -1;
-    } else if (!read_back(r, output)) {
-        return -1;
-    }
-    r->frame += n;
-    r->stats.frames += n;
-    float ms = 0.0f;
-    cudaEventElapsedTime(&ms, r->evStart, r->evStop);
-    r->stats.gpuMs = ms;
-    return 0;
+    return fill_params(r, camera, options, &P) && run_frames(r, P, n, output) ? 0 : -1;
 }
 
 int tb200_render_n(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options, int n, float* output)
@@ -1657,14 +1597,13 @@ int tb200_render_n(tb200_renderer* r, const tb200_camera* camera, const tb200_op
         set_error("tb200_render_n: only ePathTrace is batched");
         return -1;
     }
-    if (r->peers.empty()) return render_n_one(r, camera, options, n, output);
     return group_run(r, [=](tb200_renderer* m) { return render_n_one(m, camera, options, n, output); });
 }
 
 int tb200_finish(tb200_renderer* r, float exposure, float limit, float* filtered, unsigned char* rgb8)
 {
     (void)limit;   // ToneMap's filmic branch ignores it (util.h:25-42), kept for the call shape of main.cpp:269
-    if (!r || !r->dAccum) {
+    if (!r || !r->mem.accum) {
         set_error("tb200_finish: tb200_init has not been called");
         return -1;
     }
@@ -1674,21 +1613,13 @@ int tb200_finish(tb200_renderer* r, float exposure, float limit, float* filtered
     const size_t n = size_t(W) * H;
     const size_t rgbBytes = ((n + 3) / 4) * 12;
     if (r->finishWidth != W || r->finishHeight != H) {
-        cudaFree(r->dFiltered);
-        cudaFree(r->dRgb8);
-        cudaFree(r->dDither);
-        cudaFree(r->dMeans);
-        cudaFree(r->dDenoised);
-        r->dFiltered = nullptr;
-        r->dRgb8 = nullptr;
-        r->dDither = nullptr;
-        r->dMeans = r->dDenoised = nullptr;
+        r->mem.means.reset();
+        r->mem.denoised.reset();
         r->ditherReady = false;
         r->filteredValid = false;
         r->finishWidth = r->finishHeight = 0;
-        if (cudaMalloc((void**)&r->dFiltered, n * sizeof(float4)) != cudaSuccess ||
-            cudaMalloc((void**)&r->dRgb8, rgbBytes) != cudaSuccess ||
-            cudaMalloc((void**)&r->dDither, n * sizeof(uint2)) != cudaSuccess) {
+        if (dev_alloc(&r->mem.filtered, n) != cudaSuccess || dev_alloc(&r->mem.rgb8, rgbBytes) != cudaSuccess ||
+            dev_alloc(&r->mem.dither, n) != cudaSuccess) {
             set_error("tb200_finish: buffer allocation failed");
             return -1;
         }
@@ -1709,7 +1640,7 @@ int tb200_finish(tb200_renderer* r, float exposure, float limit, float* filtered
                 s2 = s1 ^ ((b << 12) | (b >> 20));
             }
         }
-        if (cudaMemcpyAsync(r->dDither, states.data(), n * sizeof(uint2), cudaMemcpyHostToDevice, r->stream) != cudaSuccess ||
+        if (cudaMemcpyAsync(r->mem.dither.get(), states.data(), n * sizeof(uint2), cudaMemcpyHostToDevice, r->stream) != cudaSuccess ||
             cudaStreamSynchronize(r->stream) != cudaSuccess) {
             set_error("tb200_finish: dither table upload failed");
             return -1;
@@ -1718,12 +1649,12 @@ int tb200_finish(tb200_renderer* r, float exposure, float limit, float* filtered
         r->ditherReady = true;
     }
     FinishParams F;
-    F.accum = r->boundAccum ? r->boundAccum : r->dAccum;
+    F.accum = r->boundAccum ? r->boundAccum : r->mem.accum.get();
     F.numPixels = (int)n;
     F.exposure = exposure;
-    F.filtered = r->dFiltered;   // always kept on the device: tb200_nlm reads it
-    F.rgb8 = rgb8 ? r->dRgb8 : nullptr;
-    F.ditherState = r->dDither;
+    F.filtered = r->mem.filtered.get();   // always kept on the device: tb200_nlm reads it
+    F.rgb8 = rgb8 ? r->mem.rgb8.get() : nullptr;
+    F.ditherState = r->mem.dither.get();
     unsigned long long launches = 0;
     cudaEventRecord(r->evStart, r->stream);
     launch_finish(F, r->stream, &launches);
@@ -1731,11 +1662,11 @@ int tb200_finish(tb200_renderer* r, float exposure, float limit, float* filtered
     r->stats.kernelLaunches += launches;
     bool ok = cudaGetLastError() == cudaSuccess;
     if (ok && filtered) {
-        ok = cudaMemcpyAsync(filtered, r->dFiltered, n * sizeof(float4), cudaMemcpyDeviceToHost, r->stream) == cudaSuccess;
+        ok = cudaMemcpyAsync(filtered, r->mem.filtered.get(), n * sizeof(float4), cudaMemcpyDeviceToHost, r->stream) == cudaSuccess;
         r->stats.d2hBytes += n * sizeof(float4);
     }
     if (ok && rgb8) {
-        ok = cudaMemcpyAsync(rgb8, r->dRgb8, n * 3, cudaMemcpyDeviceToHost, r->stream) == cudaSuccess;
+        ok = cudaMemcpyAsync(rgb8, r->mem.rgb8.get(), n * 3, cudaMemcpyDeviceToHost, r->stream) == cudaSuccess;
         r->stats.d2hBytes += n * 3;
     }
     ok = ok && cudaStreamSynchronize(r->stream) == cudaSuccess;
@@ -1744,10 +1675,7 @@ int tb200_finish(tb200_renderer* r, float exposure, float limit, float* filtered
         return -1;
     }
     r->filteredValid = true;
-    float ms = 0.0f;
-    cudaEventElapsedTime(&ms, r->evStart, r->evStop);
-    r->stats.gpuMs = ms;
-    return 0;
+    return sync_gpu_ms(r) ? 0 : -1;
 }
 
 int tb200_nlm(tb200_renderer* r, float falloff, int radius, float* out)
@@ -1762,17 +1690,16 @@ int tb200_nlm(tb200_renderer* r, float falloff, int radius, float* out)
     }
     cudaSetDevice(r->device);
     const size_t n = size_t(r->width) * r->height;
-    if (!r->dMeans) {
-        if (cudaMalloc((void**)&r->dMeans, n * sizeof(float4)) != cudaSuccess ||
-            cudaMalloc((void**)&r->dDenoised, n * sizeof(float4)) != cudaSuccess) {
+    if (!r->mem.means || !r->mem.denoised) {
+        if (dev_alloc(&r->mem.means, n) != cudaSuccess || dev_alloc(&r->mem.denoised, n) != cudaSuccess) {
             set_error("tb200_nlm: buffer allocation failed");
             return -1;
         }
     }
     NlmParams N;
-    N.in = r->dFiltered;
-    N.means = r->dMeans;
-    N.out = r->dDenoised;
+    N.in = r->mem.filtered.get();
+    N.means = r->mem.means.get();
+    N.out = r->mem.denoised.get();
     N.width = r->width;
     N.height = r->height;
     N.radius = radius;
@@ -1783,16 +1710,13 @@ int tb200_nlm(tb200_renderer* r, float falloff, int radius, float* out)
     cudaEventRecord(r->evStop, r->stream);
     r->stats.kernelLaunches += launches;
     if (cudaGetLastError() != cudaSuccess ||
-        cudaMemcpyAsync(out, r->dDenoised, n * sizeof(float4), cudaMemcpyDeviceToHost, r->stream) != cudaSuccess ||
+        cudaMemcpyAsync(out, r->mem.denoised.get(), n * sizeof(float4), cudaMemcpyDeviceToHost, r->stream) != cudaSuccess ||
         cudaStreamSynchronize(r->stream) != cudaSuccess) {
         set_error(std::string("tb200_nlm: ") + cudaGetErrorString(cudaGetLastError()));
         return -1;
     }
     r->stats.d2hBytes += n * sizeof(float4);
-    float ms = 0.0f;
-    cudaEventElapsedTime(&ms, r->evStart, r->evStop);
-    r->stats.gpuMs = ms;
-    return 0;
+    return sync_gpu_ms(r) ? 0 : -1;
 }
 
 int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options, int frame,
@@ -1813,28 +1737,27 @@ int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200
         if (!ok) return -1;
     }
     const size_t n = size_t(r->width) * r->height;
-    if (!r->dRadiance) {
-        if (cudaMalloc((void**)&r->dRadiance, n * 3 * sizeof(float)) != cudaSuccess ||
-            cudaMalloc((void**)&r->dRaster, n * 2 * sizeof(float)) != cudaSuccess) {
+    if (!r->mem.radiance || !r->mem.raster) {
+        if (dev_alloc(&r->mem.radiance, n * 3) != cudaSuccess || dev_alloc(&r->mem.raster, n * 2) != cudaSuccess) {
             set_error("tb200_trace_frame: scratch allocation failed");
             return -1;
         }
     }
     P.frame0 = frame;
     P.numFrames = 1;
-    P.outRadiance = r->dRadiance;
-    P.outRaster = r->dRaster;
+    P.outRadiance = r->mem.radiance.get();
+    P.outRaster = r->mem.raster.get();
     // pixels of other shards (tb200_set_shard) are not traced by this renderer: they read back as zero
-    if (cudaMemsetAsync(r->dRadiance, 0, n * 3 * sizeof(float), r->stream) != cudaSuccess ||
-        cudaMemsetAsync(r->dRaster, 0, n * 2 * sizeof(float), r->stream) != cudaSuccess) {
+    if (cudaMemsetAsync(P.outRadiance, 0, n * 3 * sizeof(float), r->stream) != cudaSuccess ||
+        cudaMemsetAsync(P.outRaster, 0, n * 2 * sizeof(float), r->stream) != cudaSuccess) {
         set_error("tb200_trace_frame: scratch clear failed");
         return -1;
     }
     const uint64_t samplesBefore = r->stats.samples;
     if (!launch_frames(r, P)) return -1;
     r->stats.samples = samplesBefore;
-    if (cudaMemcpyAsync(radiance, r->dRadiance, n * 3 * sizeof(float), cudaMemcpyDeviceToHost, r->stream) != cudaSuccess ||
-        cudaMemcpyAsync(raster, r->dRaster, n * 2 * sizeof(float), cudaMemcpyDeviceToHost, r->stream) != cudaSuccess ||
+    if (cudaMemcpyAsync(radiance, P.outRadiance, n * 3 * sizeof(float), cudaMemcpyDeviceToHost, r->stream) != cudaSuccess ||
+        cudaMemcpyAsync(raster, P.outRaster, n * 2 * sizeof(float), cudaMemcpyDeviceToHost, r->stream) != cudaSuccess ||
         cudaStreamSynchronize(r->stream) != cudaSuccess) {
         set_error(std::string("tb200_trace_frame: ") + cudaGetErrorString(cudaGetLastError()));
         return -1;
@@ -1914,17 +1837,14 @@ static int query_run(const char* entry, tb200_renderer* r, const std::function<v
     }
     launch(&launches);
     r->stats.kernelLaunches += launches;
-    float ms = 0.0f;
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaEventRecord(r->evStop, r->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, r->evStart, r->evStop);
     if (e != cudaSuccess) {
         set_error(std::string(entry) + ": " + cudaGetErrorString(e));
         return -1;
     }
-    r->stats.gpuMs = ms;
-    return 0;
+    return sync_gpu_ms(r) ? 0 : -1;
 }
 
 int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, int64_t numRays)
@@ -1944,7 +1864,7 @@ int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, 
     Q.hits = reinterpret_cast<float4*>(hits);
     Q.prims = prims;
     Q.numRays = numRays;
-    Q.counter = r->dCounter;   // the wavefront's work counter: free between launches on this stream
+    Q.counter = r->mem.counter.get();   // the wavefront's work counter: free between launches on this stream
     return query_run(entry, r, [&](unsigned long long* launches) { launch_trace_rays(Q, r->numSMs, r->stream, launches); });
 }
 
@@ -1962,7 +1882,7 @@ int tb200_occluded_rays(tb200_renderer* r, const tb200_ray* rays, uint8_t* occlu
     Q.rays = reinterpret_cast<const float4*>(rays);
     Q.occluded = occluded;
     Q.numRays = numRays;
-    Q.counter = r->dCounter;
+    Q.counter = r->mem.counter.get();
     return query_run(entry, r, [&](unsigned long long* launches) { launch_occluded_rays(Q, r->numSMs, r->stream, launches); });
 }
 
@@ -2044,7 +1964,7 @@ void tb200_destroy(tb200_renderer* r)
     tb200_unpin_output(r);
     cudaSetDevice(r->device);
     if (r->stream) cudaStreamSynchronize(r->stream);
-    free_device(r);
+    r->mem = tb200_renderer::Memory();
     r->stream = r->ownStream;
     if (r->evStart) cudaEventDestroy(r->evStart);
     if (r->evStop) cudaEventDestroy(r->evStop);
