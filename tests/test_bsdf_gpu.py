@@ -18,7 +18,6 @@ produce: N face-forwarded towards V (dot(N, V) >= 0), with V at grazing angles, 
 and L over the whole sphere, along N, perpendicular to it, along the mirror direction and along -V.
 
 The edge-materials scenes at the end trace the same materials per sample through the renderer in every route."""
-import contextlib
 import ctypes as C
 import os
 
@@ -576,37 +575,14 @@ def make_edge_scene(seed, path, unsafe, width=96, height=64):
     return mats
 
 
-ROUTES = {
-    "mega": {"TINSEL_B200_PIPELINE": "mega"},
-    "wavefront": {},
-    "lane-owned": {"TINSEL_B200_QUEUES": "lanes", "TINSEL_B200_SCHED": "free", "TINSEL_B200_CTA": "512", "TINSEL_B200_SPLIT": "0"},
-    "lane-owned, TINSEL_B200_SPECIALIZE=0": {"TINSEL_B200_QUEUES": "lanes", "TINSEL_B200_SCHED": "free", "TINSEL_B200_CTA": "512",
-                                             "TINSEL_B200_SPLIT": "0", "TINSEL_B200_SPECIALIZE": "0"},
-    "TINSEL_B200_SPECIALIZE=0": {"TINSEL_B200_SPECIALIZE": "0"},
-}
-ENV_KEYS = ("TINSEL_B200_PIPELINE", "TINSEL_B200_SPECIALIZE") + schedenv.KEYS
+EDGE_ROUTES = {r: schedenv.ROUTES[r] for r in ("mega", "wavefront", "lanes", "lanes-generic")}
+EDGE_ROUTES["SPECIALIZE=0"] = dict(SPECIALIZE="0")
 EDGE_SCENES = [(False, s) for s in range(3)] + [(True, s) for s in range(3)]
 
 
-@contextlib.contextmanager
-def _route_env(env):
-    """The renderer's environment variables set to `env` alone; None leaves the environment as it is."""
-    if env is None:
-        yield
-        return
-    saved = {k: os.environ.pop(k, None) for k in ENV_KEYS}
-    os.environ.update(env)
-    try:
-        yield
-    finally:
-        for k, v in saved.items():
-            os.environ.pop(k, None)
-            if v is not None:
-                os.environ[k] = v
-
-
 def _trace_routes(path, routes, frames):
-    """{(route, frame): samples that differ from the restatement}, {route: kernel that ran}, NaN samples per frame."""
+    """{(route, frame): samples that differ from the restatement}, {route: kernel that ran}, NaN samples per frame.
+    routes: {route: its knob settings}."""
     port = refdrv.PortScene.from_snapshot(path)
     expect = {f: port.trace_frame(f, 8) for f in frames}
     port.close()
@@ -614,19 +590,19 @@ def _trace_routes(path, routes, frames):
     cam, opt = snap.camera, snap.options
     bad, kernels = {}, {}
     try:
-        for route, env in routes.items():
-            with _route_env(env):
+        for route, settings in routes.items():
+            with schedenv.knobs(**settings):
                 r = tb.Renderer(snap.scene)
-                r.Init(opt.width, opt.height)
-                for f in frames:
-                    rad, ras = r.trace_frame(cam, opt, f)
-                    prad, pras = expect[f]
-                    assert np.array_equal(ras, pras)
-                    n = int((~_bits_equal(rad, prad).all(-1)).sum())
-                    if n:
-                        bad[(route, f)] = n
-                kernels[route] = r.last_kernel()
-                r.close()
+            r.Init(opt.width, opt.height)
+            for f in frames:
+                rad, ras = r.trace_frame(cam, opt, f)
+                prad, pras = expect[f]
+                assert np.array_equal(ras, pras)
+                n = int((~_bits_equal(rad, prad).all(-1)).sum())
+                if n:
+                    bad[(route, f)] = n
+            kernels[route] = r.last_kernel()
+            r.close()
     finally:
         snap.close()
     return bad, kernels, {f: int(np.isnan(expect[f][0]).any(-1).sum()) for f in frames}
@@ -640,10 +616,10 @@ def test_edge_material_scenes_match_restatement(unsafe, seed, tmp_path):
     others never do, and their NaN samples land where the restatement's do."""
     path = str(tmp_path / "edge.tsnap")
     make_edge_scene(seed, path, unsafe)
-    bad, kernels, nan = _trace_routes(path, ROUTES, (0, 3))
+    bad, kernels, nan = _trace_routes(path, EDGE_ROUTES, (0, 3))
     assert not bad, "samples differ: %s" % bad
-    assert kernels["lane-owned"] == ("wf2_lq.generic" if unsafe else "wf2_lq.specialized"), kernels
-    assert kernels["lane-owned, TINSEL_B200_SPECIALIZE=0"] == "wf2_lq.generic", kernels
+    assert kernels["lanes"] == ("wf2_lq.generic" if unsafe else "wf2_lq.specialized"), kernels
+    assert kernels["lanes-generic"] == "wf2_lq.generic", kernels
     print("edge scene unsafe=%s seed %d: kernels %s, NaN samples per frame %s" % (unsafe, seed, kernels, nan))
 
 
@@ -653,8 +629,7 @@ def test_edge_material_scenes_under_every_scheduler_variant(sched, cta, tmp_path
     for unsafe, seed in EDGE_SCENES[::2]:
         path = str(tmp_path / ("edge%d%d.tsnap" % (unsafe, seed)))
         make_edge_scene(seed, path, unsafe)
-        with schedenv.sched_env(sched, cta):
-            bad, _, _ = _trace_routes(path, {sched: None}, (3, 4))
+        bad, _, _ = _trace_routes(path, {sched: schedenv.sched_knobs(sched, cta)}, (3, 4))
         assert not bad, "unsafe=%s seed %d: samples differ %s" % (unsafe, seed, bad)
 
 

@@ -17,10 +17,17 @@ import pytest
 import tinsel_b200 as tb
 from tinsel_b200 import abi
 import refdrv
+import schedenv
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MAX_LEVELS = 31   # TB200_MAX_BVH_LEVELS
+
+
+@pytest.fixture(autouse=True)
+def default_knobs():
+    with schedenv.knobs():
+        yield
 
 
 def _mesh_arrays(mesh):
@@ -97,7 +104,6 @@ def _biggest_mesh(scene):
 def test_gpu_built_bvh_structure_and_parity(name, size):
     if not os.path.exists(tb.scene_path(name)):
         pytest.skip("snapshot scenes/%s.tsnap not present" % name)
-    os.environ["TINSEL_B200_PIPELINE"] = "wavefront"
     snap = tb.Snapshot(tb.scene_path(name))
     cam, opt = snap.camera, snap.options
     opt.width, opt.height = size
@@ -262,7 +268,6 @@ def test_bvh_build_on_a_large_random_mesh():
     cam.rotation[:] = [0.0, 0.0, 0.0, 1.0]
     opt.width, opt.height, opt.maxDepth = 96, 64, 3
     oracle = refdrv.PortScene(C.pointer(sc), cam, opt, keepalive=(keep, meshes, nodes, pos, nrm, idx, cdf))
-    os.environ["TINSEL_B200_PIPELINE"] = "wavefront"
     r = tb.Renderer(C.pointer(sc))
     r.Init(96, 64)
     rad, ras = r.trace_frame(cam, opt, 0)

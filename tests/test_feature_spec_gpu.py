@@ -11,6 +11,7 @@ import pytest
 import tinsel_b200 as tb
 from tinsel_b200 import abi
 import refdrv
+import schedenv
 
 pytestmark = pytest.mark.gpu
 
@@ -19,15 +20,9 @@ SIZE = (96, 64)
 
 
 @pytest.fixture(autouse=True)
-def lane_layout(monkeypatch):
-    # the lane-owned layout whatever the launch size and mesh size: free-running scheduler, 512-thread CTAs, no split
-    # trace queue
-    monkeypatch.setenv("TINSEL_B200_QUEUES", "lanes")
-    monkeypatch.setenv("TINSEL_B200_SCHED", "free")
-    monkeypatch.setenv("TINSEL_B200_CTA", "512")
-    monkeypatch.setenv("TINSEL_B200_SPLIT", "0")
-    monkeypatch.delenv("TINSEL_B200_PIPELINE", raising=False)
-    monkeypatch.delenv("TINSEL_B200_SPECIALIZE", raising=False)
+def lane_layout():
+    with schedenv.knobs(**schedenv.ROUTES["lanes"]):
+        yield
 
 
 def _port(path):
@@ -72,19 +67,19 @@ def test_routing(name, kernel):
     assert ran == kernel
 
 
-def test_override_runs_generic(monkeypatch):
-    monkeypatch.setenv("TINSEL_B200_SPECIALIZE", "0")
-    _, ran = _trace(tb.scene_path("cornell"))
+def test_override_runs_generic():
+    with schedenv.knobs(**schedenv.ROUTES["lanes-generic"]):
+        _, ran = _trace(tb.scene_path("cornell"))
     assert ran == GENERIC
 
 
 @pytest.mark.parametrize("name", ["cornell", "meshlight"])
-def test_specialized_equals_generic_and_restatement(name, monkeypatch):
+def test_specialized_equals_generic_and_restatement(name):
     path = tb.scene_path(name)
     rad, ran = _trace(path)
     assert ran == SPECIALIZED
-    monkeypatch.setenv("TINSEL_B200_SPECIALIZE", "0")
-    grad, gran = _trace(path)
+    with schedenv.knobs(**schedenv.ROUTES["lanes-generic"]):
+        grad, gran = _trace(path)
     assert gran == GENERIC
     assert all((a.view(np.uint32) == b.view(np.uint32)).all() for a, b in zip(rad, grad))
     _assert_matches_port(path, rad)

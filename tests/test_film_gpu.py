@@ -5,7 +5,6 @@ Per-sample inputs come from the CPU restatement (PortScene.trace_frame), so the 
 GPU.  assert_film_close allows only what a correct GPU film can differ by: the order of its fp32 additions and
 the L2 adder's flush to zero.  Counting mode (box filter of width 0) checks that every pixel received exactly
 the samples it should have, bit for bit."""
-import contextlib
 import os
 
 import numpy as np
@@ -24,7 +23,6 @@ pytestmark = pytest.mark.gpu
 THREADS = min(os.cpu_count() or 8, 32)   # more threads than a cgroup CPU quota allows only thrash
 MATRIX_SCENES = ["meshlight", "motionblur", "many", "veach", "big-mesh"]
 MATRIX_VARIANTS = [(s, c) for s in schedenv.SCHEDS for c in schedenv.CTAS] + [("mega", None), ("no-flat", None)]
-CAP_KEY = "TINSEL_B200_TEST_LAUNCH_SAMPLES"
 
 
 @pytest.fixture(scope="module")
@@ -44,28 +42,10 @@ def scenes(tmp_path_factory):
     return paths
 
 
-@contextlib.contextmanager
-def env(**kv):
-    old = {k: os.environ.get(k) for k in kv}
-    for k, v in kv.items():
-        if v is None:
-            os.environ.pop(k, None)
-        else:
-            os.environ[k] = str(v)
-    try:
-        yield
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-
-
 @pytest.fixture(autouse=True)
-def clean_env():
-    for k in schedenv.KEYS + ("TINSEL_B200_PIPELINE", "TINSEL_B200_READBACK", CAP_KEY):
-        os.environ.pop(k, None)
+def default_knobs():
+    with schedenv.knobs():
+        yield
 
 
 _refs = {}
@@ -115,8 +95,7 @@ def test_benchmark_shape_cornell_1024(scenes):
     f011 += reference(scenes["cornell"], size, range(7, 11), [opt])[0]
     f064 = f011.copy()
     f064 += reference(scenes["cornell"], size, range(11, 64), [opt])[0]
-    with env(TINSEL_B200_PIPELINE=None):
-        r = renderer(snap, opt)
+    r = renderer(snap, opt)
     stream = torch.cuda.Stream()
     with torch.cuda.stream(stream):
         r.set_stream(stream.cuda_stream)
@@ -150,8 +129,7 @@ def test_veach_1920x1080_render_device_16(scenes):
     size = (1920, 1080)
     snap, cam, opt = setup(scenes["veach"], size)
     ref = reference(scenes["veach"], size, range(16), [opt])[0]
-    with env(TINSEL_B200_PIPELINE=None):
-        r = renderer(snap, opt)
+    r = renderer(snap, opt)
     r.render_device(cam, opt, 16)
     filmref.assert_film_close(r.read_accumulator(), ref, "veach 1920x1080 render_device(16)")
     r.close()
@@ -166,21 +144,16 @@ def matrix_reference(scenes, name):
     return snap, cam, opt, films
 
 
-def variant_env(sched, cta):
-    if sched == "mega":
-        return env(TINSEL_B200_PIPELINE="mega")
-    if sched == "no-flat":
-        return env(TINSEL_B200_PIPELINE=None, TINSEL_B200_NO_FLAT="1")
-    return schedenv.sched_env(sched, cta)
+def variant_knobs(sched, cta):
+    return schedenv.sched_env(sched, cta) if cta else schedenv.knobs(**schedenv.ROUTES[sched])
 
 
 @pytest.mark.parametrize("sched,cta", MATRIX_VARIANTS, ids=["%s-%s" % v if v[1] else v[0] for v in MATRIX_VARIANTS])
 def test_scheduler_variants_steady_state(sched, cta, scenes):
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
     for name in MATRIX_SCENES:
         snap, cam, opt, (gauss, counts) = matrix_reference(scenes, name)
         copt = filmref.counting_options(opt)
-        with variant_env(sched, cta):
+        with variant_knobs(sched, cta):
             r = renderer(snap, opt)
             rc = renderer(snap, copt)
         what = "%s %s/%s 256^2 x 16" % (name, sched, cta)
@@ -211,8 +184,7 @@ def test_interleaved_shards(scenes):
         gauss, counts = reference(scenes["cornell"], size, range(4), [opt, copt], mask)
         assert gauss.samples == sharding.shard_sample_count(size[0], size[1], shard, 3, 4)
         for o, ref, check in ((opt, gauss, filmref.assert_film_close), (copt, counts, filmref.assert_counts)):
-            with env(TINSEL_B200_PIPELINE=None):
-                r = renderer(snap, o)
+            r = renderer(snap, o)
             r.set_shard(shard, 3)
             r.render_device(cam, o, 4)
             assert r.stats().samples == ref.samples
@@ -241,7 +213,7 @@ def test_row_slabs(name, size, parts, filt, queues, scenes):
     ref = reference(scenes[name], size, range(4), [opt], key=("slab", name, size, fname))[0]
     cuts = [sharding.slab_rows(size[1], k, parts) for k in range(parts)] if isinstance(parts, int) else parts
     what = "%s %dx%d %s queues=%s" % (name, size[0], size[1], fname, queues)
-    with env(**QUEUES[queues]):
+    with schedenv.knobs(**schedenv.ROUTES[queues]):
         render_out = np.full((size[1], size[0], 4), SENTINEL, np.float32)
         device_out = render_out.copy()
         for row0, nrows in cuts:
@@ -257,7 +229,7 @@ def test_row_slabs(name, size, parts, filt, queues, scenes):
             r.close()
         filmref.assert_film_close(render_out, ref, "%s: %d set_slab renderers, Render() x 4" % (what, len(cuts)))
         filmref.assert_film_close(device_out, ref, "%s: %d set_slab renderers, render_device(4)" % (what, len(cuts)))
-        with env(TINSEL_B200_TEST_DUP_DEVICES="1"):
+        with schedenv.knobs(TEST_DUP_DEVICES="1", **schedenv.ROUTES[queues]):
             m = tb.Renderer(snap.scene, devices=[0] * len(cuts))
         m.Init(*size)
         out = np.full_like(render_out, SENTINEL)
@@ -281,7 +253,7 @@ def test_ragged_sizes(size, queues, scenes):
     copt = filmref.counting_options(opt)
     gauss, counts = reference(scenes["cornell"], size, range(4), [opt, copt])
     for o, ref, check in ((opt, gauss, filmref.assert_film_close), (copt, counts, filmref.assert_counts)):
-        with env(TINSEL_B200_PIPELINE=None, TINSEL_B200_QUEUES=queues):
+        with schedenv.knobs(QUEUES=queues):
             r = renderer(snap, o)
         r.render_device(cam, o, 4)
         assert r.stats().samples == ref.samples
@@ -293,13 +265,8 @@ def test_ragged_sizes(size, queues, scenes):
 # ---- the film's edges: every filter variant in every kernel ----
 
 FILTER_CASES = [(v[0], v[1], v[2], "cornell") for v in VARIANTS] + [("nan-probe", (40, 30), NAN_FILTER, "nan-probe")]
-# the lane-owned layout whatever the launch size, as in test_feature_spec_gpu.py
-LANES = dict(TINSEL_B200_PIPELINE=None, TINSEL_B200_QUEUES="lanes", TINSEL_B200_SCHED="free", TINSEL_B200_SPLIT="0",
-             TINSEL_B200_CTA="512")
-QUEUES = {"rings": dict(TINSEL_B200_PIPELINE=None, TINSEL_B200_QUEUES="ring"), "lanes": LANES}
-PIPELINES = {"mega": dict(TINSEL_B200_PIPELINE="mega"), "rings": QUEUES["rings"], "lanes": LANES,
-             "lanes-generic": dict(LANES, TINSEL_B200_SPECIALIZE="0")}
-FILTER_RUNS = [(c, p) for c in FILTER_CASES for p in PIPELINES if p != "lanes-generic" or c[3] == "cornell"]
+FILTER_RUNS = [(c, p) for c in FILTER_CASES for p in ("mega", "rings", "lanes", "lanes-generic")
+               if p != "lanes-generic" or c[3] == "cornell"]
 
 
 def expected_kernel(pipeline, scene):
@@ -327,7 +294,7 @@ def test_filter_variants(case, pipeline, scenes):
     ref = reference(scenes[scene], size, range(4), [opt], key=("filter", what))[0]
     if scene == "nan-probe":
         assert np.isnan(ref.sums).any() and np.isfinite(ref.sums).any()
-    with env(**dict({"TINSEL_B200_SPECIALIZE": None}, **PIPELINES[pipeline])):
+    with schedenv.knobs(**schedenv.ROUTES[pipeline]):
         r = renderer(snap, opt)
     r.render_device(cam, opt, 4)
     assert r.last_kernel() == expected_kernel(pipeline, scene)
@@ -349,9 +316,9 @@ def test_launch_split_small(pipeline, scenes):
     f13 = f8.copy()
     f13 += reference(scenes["cornell"], size, range(8, 13), [opt])[0]
     f7 = reference(scenes["cornell"], size, range(7), [opt])[0]
-    with env(TINSEL_B200_PIPELINE=pipeline, **{CAP_KEY: 2 * spf + 100}):
+    with schedenv.knobs(TEST_LAUNCH_SAMPLES=2 * spf + 100, **schedenv.ROUTES[pipeline]):
         r = renderer(snap, opt)
-    with env(TINSEL_B200_PIPELINE=pipeline):
+    with schedenv.knobs(**schedenv.ROUTES[pipeline]):
         whole = renderer(snap, opt)
     l0 = r.stats().kernelLaunches
     r.render_device(cam, opt, 8)
@@ -385,8 +352,7 @@ def test_launch_split_at_the_31_bit_boundary(scenes):
     port.set_size(*size)
     port.options = copt
     expect = port.box_counts(0, frames, THREADS)
-    with env(TINSEL_B200_PIPELINE=None):
-        r = renderer(snap, copt)
+    r = renderer(snap, copt)
     r.render_device(cam, copt, frames)
     assert r.stats().samples == frames * 4096
     img = r.read_accumulator()

@@ -11,8 +11,15 @@ import pytest
 
 import tinsel_b200 as tb
 import refdrv
+import schedenv
 
 GOLD = os.path.join(refdrv.ROOT, "tests", "golden", "finish.npz")
+
+
+@pytest.fixture(autouse=True)
+def default_knobs():
+    with schedenv.knobs():
+        yield
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -144,7 +151,6 @@ def test_gpu_render_n_then_finish_matches_oracle(name, size):
     """n x Render with one read-back, then the finish step on the device, against the oracle chain
     (seeded accumulation -> finish -> quantise) on the GPU's own accumulator (bit-exact) and on the
     oracle's accumulator (8-bit values within 1)."""
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
     snap = tb.Snapshot(tb.scene_path(name))
     cam, opt = snap.camera, snap.options
     opt.width, opt.height = size

@@ -2,7 +2,6 @@
 scaled spheres, sphere lights with 1-2 samples, gradient skies.  CPU: the restatement against the
 reference's own compiled PathTrace, per sample, bit for bit.  GPU: the CUDA path against the same."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
@@ -15,6 +14,12 @@ import schedenv
 
 SEEDS = list(range(12))            # GPU part
 CPU_SEEDS = list(range(48))        # restatement vs the reference's compiled code
+
+
+@pytest.fixture(autouse=True)
+def default_knobs():
+    with schedenv.knobs():
+        yield
 
 
 def _same(a, b):
@@ -41,7 +46,6 @@ def test_port_matches_reference_on_random_scenes(seed, tmp_path):
 @pytest.mark.gpu
 @pytest.mark.parametrize("seed", SEEDS)
 def test_gpu_matches_oracle_on_random_scenes(seed, tmp_path):
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
     path = str(tmp_path / "fuzz.tsnap")
     what = fuzzscene.make_scene(seed, path, width=96, height=64)
     port = refdrv.PortScene.from_snapshot(path)
@@ -67,6 +71,7 @@ MESH_CASES = ([("instanced", s) for s in range(8)] + [("ties", s) for s in range
 MATRIX_CASES = [("instanced", 1), ("ties", 0), ("many", 1), ("big", 0), ("probe", 1), ("caterpillar", 0)]
 CPU_MESH_CASES = [(f, s) for f in fuzzscene.FAMILIES for s in range(4)]
 LIMIT = 31    # TB200_MAX_BVH_LEVELS
+PIPELINES = {p: schedenv.ROUTES[p] for p in ("mega", "wavefront")}
 
 
 def _bad_samples(rad, ras, prad, pras):
@@ -74,26 +79,23 @@ def _bad_samples(rad, ras, prad, pras):
     return int((~((rad.view(np.uint32) == prad.view(np.uint32)) | (np.isnan(rad) & np.isnan(prad))).all(-1)).sum())
 
 
-def _gpu_vs_port(path, pipelines=("mega", "wavefront"), frames=(0, 3)):
+def _gpu_vs_port(path, routes=PIPELINES, frames=(0, 3)):
+    """routes: {route: its knob settings}."""
     port = refdrv.PortScene.from_snapshot(path)
     snap = tb.Snapshot(path)
     cam, opt = snap.camera, snap.options
     bad = {}
-    try:
-        for pipeline in pipelines:
-            if pipeline:
-                os.environ["TINSEL_B200_PIPELINE"] = pipeline
+    for route, settings in routes.items():
+        with schedenv.knobs(**settings):
             r = tb.Renderer(snap.scene)
-            r.Init(opt.width, opt.height)
-            for frame in frames:
-                rad, ras = r.trace_frame(cam, opt, frame)
-                prad, pras = port.trace_frame(frame, 8)
-                n = _bad_samples(rad, ras, prad, pras)
-                if n:
-                    bad[(pipeline, frame)] = n
-            r.close()
-    finally:
-        os.environ.pop("TINSEL_B200_PIPELINE", None)
+        r.Init(opt.width, opt.height)
+        for frame in frames:
+            rad, ras = r.trace_frame(cam, opt, frame)
+            prad, pras = port.trace_frame(frame, 8)
+            n = _bad_samples(rad, ras, prad, pras)
+            if n:
+                bad[(route, frame)] = n
+        r.close()
     return bad, port, snap
 
 
@@ -134,14 +136,13 @@ def test_gpu_matches_port_on_mesh_scenes(family, seed, tmp_path):
 @pytest.mark.gpu
 @pytest.mark.parametrize("sched,cta,no_flat", [(s, c, False) for s in schedenv.SCHEDS for c in schedenv.CTAS] + [("free", "768", True)])
 def test_mesh_scenes_under_every_scheduler_variant(sched, cta, no_flat, tmp_path):
-    with schedenv.sched_env(sched, cta, no_flat=no_flat):
-        for family, seed in MATRIX_CASES:
-            path = str(tmp_path / ("%s%d.tsnap" % (family, seed)))
-            what = fuzzscene.make_mesh_scene(seed, path, family, width=96, height=64)
-            bad, port, snap = _gpu_vs_port(path, pipelines=("wavefront",), frames=(3, 4))
-            assert not bad, "%s: samples differ %s" % (what, bad)
-            port.close()
-            snap.close()
+    for family, seed in MATRIX_CASES:
+        path = str(tmp_path / ("%s%d.tsnap" % (family, seed)))
+        what = fuzzscene.make_mesh_scene(seed, path, family, width=96, height=64)
+        bad, port, snap = _gpu_vs_port(path, {sched: schedenv.sched_knobs(sched, cta, no_flat)}, frames=(3, 4))
+        assert not bad, "%s: samples differ %s" % (what, bad)
+        port.close()
+        snap.close()
 
 
 @pytest.mark.gpu

@@ -11,8 +11,15 @@ import pytest
 import tinsel_b200 as tb
 from tinsel_b200 import abi, sharding
 import refdrv
+import schedenv
 
 pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(autouse=True)
+def default_knobs():
+    with schedenv.knobs():
+        yield
 
 
 def _gpus():
@@ -23,7 +30,6 @@ def _gpus():
 def _scene(name, size):
     if not os.path.exists(tb.scene_path(name)):
         pytest.skip("snapshot scenes/%s.tsnap not present" % name)
-    os.environ["TINSEL_B200_PIPELINE"] = "wavefront"
     snap = tb.Snapshot(tb.scene_path(name))
     cam, opt = snap.camera, snap.options
     opt.width, opt.height = size
@@ -123,12 +129,9 @@ def _check_group(devices, name="cornell", size=(256, 192)):
 def test_group_of_renderers_sharing_one_device():
     """The whole multi-device host path (worker threads, slabs, per-member streamed read-back, gather)
     on a one-GPU box: a group whose three members all sit on device 0 (test hook)."""
-    os.environ["TINSEL_B200_TEST_DUP_DEVICES"] = "1"
-    try:
+    with schedenv.knobs(TEST_DUP_DEVICES="1"):
         _check_group([0, 0, 0])
         _check_group([0, 0], name="veach", size=(200, 110))
-    finally:
-        del os.environ["TINSEL_B200_TEST_DUP_DEVICES"]
 
 
 def test_multi_device_renderer_equals_single_device():

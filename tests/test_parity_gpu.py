@@ -17,6 +17,13 @@ import schedenv
 
 pytestmark = pytest.mark.gpu
 
+
+@pytest.fixture(autouse=True)
+def default_knobs():
+    with schedenv.knobs():
+        yield
+
+
 # scene -> (width, height) used for the per-sample tests (None keeps the .tin's size)
 SCENES = {
     "cornell": (256, 256),
@@ -53,11 +60,10 @@ def _oracle(name, flavour):
     return refdrv.PortScene.from_snapshot(tb.scene_path(name))
 
 
-def _setup(name, pipeline, size=None, flavour="detmath"):
+def _setup(name, size=None, flavour="detmath"):
     if not _available(name):
         pytest.skip("snapshot scenes/%s.tsnap not present" % name)
     ref = _oracle(name, flavour)
-    os.environ["TINSEL_B200_PIPELINE"] = pipeline
     snap = tb.Snapshot(tb.scene_path(name))
     cam, opt = snap.camera, snap.options
     w, h = size or SCENES[name]
@@ -78,7 +84,8 @@ def test_sample_seed_matches_host():
 @pytest.mark.parametrize("pipeline", ["mega", "wavefront"])
 @pytest.mark.parametrize("name", list(SCENES))
 def test_per_sample_radiance_bit_exact(name, pipeline):
-    snap, cam, opt, ref, r = _setup(name, pipeline)
+    with schedenv.knobs(**schedenv.ROUTES[pipeline]):
+        snap, cam, opt, ref, r = _setup(name)
     for frame in (0, 5):
         rad, ras = r.trace_frame(cam, opt, frame)
         rrad, rras = ref.trace_frame(frame, nthreads=8)
@@ -96,7 +103,8 @@ def test_per_sample_radiance_bit_exact(name, pipeline):
 @pytest.mark.parametrize("name", ["cornell", "veach", "glass", "ajax", "env", "envmini"])
 def test_render_matches_seeded_oracle(name, pipeline):
     """Renderer.Render x spp vs oracle B at matched spp and seeds: rel-L2 <= 1e-4 (BASELINE.json)."""
-    snap, cam, opt, ref, r = _setup(name, pipeline)
+    with schedenv.knobs(**schedenv.ROUTES[pipeline]):
+        snap, cam, opt, ref, r = _setup(name)
     spp = 4
     out = np.zeros((opt.height, opt.width, 4), np.float32)
     for _ in range(spp):
@@ -118,7 +126,7 @@ def test_normals_mode_bit_exact_vs_literal_reference(name):
     """eNormals (render.cpp:494-515) has no RNG and no libm: exact match against the literal reference
     (or the CPU restatement, whose normals images equal the literal reference's in tests/golden)."""
     literal = refdrv.have_ref("literal")
-    snap, cam, opt, ref, r = _setup(name, "wavefront", flavour="literal" if literal else "port")
+    snap, cam, opt, ref, r = _setup(name, flavour="literal" if literal else "port")
     opt.mode = abi.MODE_NORMALS
     ref.set_mode(abi.MODE_NORMALS)
     out = np.zeros((opt.height, opt.width, 4), np.float32)
@@ -143,11 +151,11 @@ def test_matches_reference_golden_vectors(name, pipeline):
     if not _available(name):
         pytest.skip("snapshot scenes/%s.tsnap not present" % name)
     g = np.load(os.path.join(GOLD, "scene_%s.npz" % name))
-    os.environ["TINSEL_B200_PIPELINE"] = pipeline
     snap = tb.Snapshot(tb.scene_path(name))
     cam, opt = snap.camera, snap.options
     opt.width, opt.height = w, h = int(g["width"]), int(g["height"])
-    r = tb.Renderer(snap.scene)
+    with schedenv.knobs(**schedenv.ROUTES[pipeline]):
+        r = tb.Renderer(snap.scene)
     r.Init(w, h)
     for f in g["frames"]:
         rad, ras = r.trace_frame(cam, opt, int(f))
@@ -172,7 +180,7 @@ def test_matches_reference_golden_vectors(name, pipeline):
 
 
 def test_batched_render_equals_repeated_render():
-    snap, cam, opt, ref, r = _setup("cornell", "wavefront", size=(128, 128))
+    snap, cam, opt, ref, r = _setup("cornell", size=(128, 128))
     out = np.zeros((opt.height, opt.width, 4), np.float32)
     for _ in range(3):
         r.Render(cam, opt, out)
@@ -198,7 +206,7 @@ def test_batched_render_equals_repeated_render():
 def test_literal_reference_statistical_agreement():
     """Against the reference as shipped (glibc libm): no per-sample exactness is possible in
     principle (libm rounding), but at matched seeds the images must agree to ~1e-6."""
-    snap, cam, opt, ref, r = _setup("cornell", "wavefront", size=(128, 128), flavour="literal")
+    snap, cam, opt, ref, r = _setup("cornell", size=(128, 128), flavour="literal")
     out = np.zeros((opt.height, opt.width, 4), np.float32)
     for _ in range(8):
         r.Render(cam, opt, out)
@@ -212,7 +220,7 @@ def test_literal_reference_statistical_agreement():
 
 def test_interleaved_shards_sum_to_full_image():
     """Image-plane sharding (tb200_set_shard): the shard accumulators sum to the unsharded image."""
-    snap, cam, opt, ref, r = _setup("cornell", "wavefront", size=(100, 70))
+    snap, cam, opt, ref, r = _setup("cornell", size=(100, 70))
     r.render_device(cam, opt, 3)
     full = r.read_accumulator()
     total = np.zeros_like(full)
@@ -235,7 +243,7 @@ def test_interleaved_shards_sum_to_full_image():
 @pytest.mark.parametrize("size", [(1, 1), (3, 100), (37, 23), (8, 4), (129, 65)])
 def test_ragged_image_sizes(size):
     """Image sizes that are not multiples of the 8x4 sample tiles (and the degenerate 1x1)."""
-    snap, cam, opt, ref, r = _setup("cornell", "wavefront", size=size)
+    snap, cam, opt, ref, r = _setup("cornell", size=size)
     rad, ras = r.trace_frame(cam, opt, 2)
     rrad, rras = ref.trace_frame(2, nthreads=2)
     assert np.array_equal(ras, rras)
@@ -255,7 +263,8 @@ def test_ragged_image_sizes(size):
 @pytest.mark.parametrize("depth", [0, 1, 2, 7])
 def test_max_depth_edge_cases(depth, pipeline):
     """maxDepth 0 (no trace at all), 1 (camera ray + NEE only), deeper than the default 4."""
-    snap, cam, opt, ref, r = _setup("glass", pipeline, size=(64, 48))
+    with schedenv.knobs(**schedenv.ROUTES[pipeline]):
+        snap, cam, opt, ref, r = _setup("glass", size=(64, 48))
     opt.maxDepth = depth
     ref.set_max_depth(depth)
     rad, _ = r.trace_frame(cam, opt, 1)
@@ -279,7 +288,7 @@ def test_both_scheduling_modes_bit_exact(sched, cta):
         for name in ("veach", "meshlight", "many", "envmini", "glass", "table", "ajax", "motionblur"):
             if not _available(name):
                 continue
-            snap, cam, opt, ref, r = _setup(name, "wavefront")
+            snap, cam, opt, ref, r = _setup(name)
             for frame in (3, 4):   # two launches of one renderer: the second starts from the device buffers the first left
                 rad, _ = r.trace_frame(cam, opt, frame)
                 rrad, _ = ref.trace_frame(frame, nthreads=8)
@@ -291,7 +300,7 @@ def test_both_scheduling_modes_bit_exact(sched, cta):
 
 def test_box_filter_and_clamp():
     """eFilterBox (render.cpp:405-423) and a tight radiance clamp (ClampLength, maths.h:1577-1589)."""
-    snap, cam, opt, ref, r = _setup("cornell", "wavefront", size=(64, 64))
+    snap, cam, opt, ref, r = _setup("cornell", size=(64, 64))
     opt.filterType = abi.FILTER_BOX
     opt.clamp = 0.75
     o = ref.options
@@ -313,7 +322,7 @@ def test_box_filter_and_clamp():
 
 
 def test_rotated_camera_and_fov():
-    snap, cam, opt, ref, r = _setup("cornell", "wavefront", size=(80, 60))
+    snap, cam, opt, ref, r = _setup("cornell", size=(80, 60))
     q = np.array([0.05, 0.2, -0.03, 0.97], np.float32)
     q /= np.linalg.norm(q)
     port = refdrv.PortScene.from_snapshot(tb.scene_path("cornell"))
@@ -340,13 +349,15 @@ def test_rotated_camera_and_fov():
     ("cornell", (300, 900), 1, 3.5),      # wide box filter: rows stay open 4-5 rows behind the frontier
     ("cornell", (5, 3), 1, 0.0),          # fewer rows than one tile
 ])
-def test_streamed_readback_delivers_final_rows(case):
+def test_streamed_readback_delivers_final_rows(case, queues=None):
     """tb200_render copies finished pixel rows to the host while the kernel is still running
     (api.cu render_streamed / wf2_common.cuh wf2_band_report).  Whatever the timing, the host
     buffer must equal the device accumulator bit for bit after every call, and must equal what
-    the plain launch-then-copy path delivers up to the accumulation order."""
+    the plain launch-then-copy path delivers up to the accumulation order.  queues: the QUEUES knob both renderers
+    are created with."""
     name, size, shards, boxw = case
-    snap, cam, opt, ref, r = _setup(name, "wavefront", size=size)
+    with schedenv.knobs(QUEUES=queues):
+        snap, cam, opt, ref, r = _setup(name, size=size)
     if boxw > 0.0:
         opt.filterType = abi.FILTER_BOX
         opt.filterWidth = boxw
@@ -356,11 +367,8 @@ def test_streamed_readback_delivers_final_rows(case):
         r.Render(cam, opt, out)
         dev = r.read_accumulator()
         assert (out.view(np.uint32) == dev.view(np.uint32)).all(), "frame %d: stale rows in the host buffer" % frame
-    os.environ["TINSEL_B200_READBACK"] = "plain"
-    try:
+    with schedenv.knobs(QUEUES=queues, READBACK="plain"):
         rp = tb.Renderer(snap.scene)
-    finally:
-        del os.environ["TINSEL_B200_READBACK"]
     rp.Init(opt.width, opt.height)
     rp.set_shard(shards - 1 if shards > 1 else 0, shards)
     outp = np.zeros_like(out)
@@ -374,18 +382,18 @@ def test_streamed_readback_delivers_final_rows(case):
     snap.close()
 
 
-def test_lane_queue_layout_on_small_frames(monkeypatch):
+def test_lane_queue_layout_on_small_frames():
     """Launches of fewer than six samples per slot run the ring queues by default (kernels.cu:
     launch_wavefront2), so the small-frame feature tests above never see the lane-owned layout: force it
     (TINSEL_B200_QUEUES=lanes) and repeat the ones that exercise ragged tiles, tile padding, the band counters
     of the streamed read-back, interleaved shards and batched frames."""
-    monkeypatch.setenv("TINSEL_B200_QUEUES", "lanes")
-    for size in [(1, 1), (37, 23), (129, 65)]:
-        test_ragged_image_sizes(size)
-    test_batched_render_equals_repeated_render()
-    test_interleaved_shards_sum_to_full_image()
+    with schedenv.knobs(QUEUES="lanes"):
+        for size in [(1, 1), (37, 23), (129, 65)]:
+            test_ragged_image_sizes(size)
+        test_batched_render_equals_repeated_render()
+        test_interleaved_shards_sum_to_full_image()
     for case in [("cornell", (1021, 515), 1, 0.0), ("cornell", (512, 512), 3, 0.0), ("cornell", (300, 900), 1, 3.5), ("cornell", (5, 3), 1, 0.0)]:
-        test_streamed_readback_delivers_final_rows(case)
+        test_streamed_readback_delivers_final_rows(case, queues="lanes")
 
 
 # BASELINE.json configs at their full image sizes (C2 cornell 1024^2, C3 ajax 1024^2, C4 veach
@@ -395,7 +403,7 @@ def test_lane_queue_layout_on_small_frames(monkeypatch):
 @pytest.mark.parametrize("name,size", [("cornell", (1024, 1024)), ("ajax", (1024, 1024)), ("veach", (1920, 1080)),
                                        ("env", (2048, 2048))])
 def test_baseline_configs_full_size(name, size):
-    snap, cam, opt, ref, r = _setup(name, "wavefront", size=size)
+    snap, cam, opt, ref, r = _setup(name, size=size)
     threads = min(os.cpu_count() or 8, 32)   # more threads than a cgroup CPU quota allows only thrash
     frame = 3
     rad, ras = r.trace_frame(cam, opt, frame)
@@ -433,7 +441,7 @@ def test_baseline_configs_full_size(name, size):
                                                ("veach", (1920, 1080), 8, 1e-4), ("env", (2048, 2048), 32, 1e-4),
                                                ("glass", (512, 512), 8, 5e-3)])
 def test_literal_reference_rel_l2_at_baseline_sizes(name, size, spp, tol):
-    snap, cam, opt, ref, r = _setup(name, "wavefront", size=size, flavour="literal")
+    snap, cam, opt, ref, r = _setup(name, size=size, flavour="literal")
     threads = min(os.cpu_count() or 8, 32)
     out = np.zeros((opt.height, opt.width, 4), np.float32)
     r.render_n(cam, opt, spp, out)

@@ -9,8 +9,15 @@ import pytest
 
 import tinsel_b200 as tb
 import refdrv
+import schedenv
 
 PLUGIN = os.path.join(tb.ROOT, "tinsel_b200", "plugin", "libtinsel_b200_plugin.so")
+
+
+@pytest.fixture(autouse=True)
+def default_knobs():
+    with schedenv.knobs():
+        yield
 
 
 def test_plugin_exports_reference_factory_symbol():
@@ -25,7 +32,6 @@ def test_plugin_exports_reference_factory_symbol():
 def test_plugin_render_matches_seeded_oracle(name):
     if not os.path.exists(PLUGIN) or not refdrv.have_ref("detmath"):
         pytest.skip("plugin or oracle/_ref not built")
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
     ref = refdrv.RefScene.from_snapshot(tb.scene_path(name), "detmath")
     ref.set_size(96, 80)
     lib = C.CDLL(PLUGIN)
@@ -49,11 +55,9 @@ def test_plugin_multi_gpu_factory(monkeypatch):
     import torch
     if not os.path.exists(PLUGIN) or not refdrv.have_ref("detmath"):
         pytest.skip("plugin or oracle/_ref not built")
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
-    n = min(torch.cuda.device_count(), 4)
+    n, dup = min(torch.cuda.device_count(), 4), None
     if n < 2:
-        n = 3
-        monkeypatch.setenv("TINSEL_B200_TEST_DUP_DEVICES", "1")
+        n, dup = 3, "1"
     monkeypatch.setenv("TINSEL_GPUS", str(n))
     ref = refdrv.RefScene.from_snapshot(tb.scene_path("cornell"), "detmath")
     ref.set_size(128, 100)
@@ -61,8 +65,9 @@ def test_plugin_multi_gpu_factory(monkeypatch):
     lib.tb200_plugin_render.restype = C.c_int
     lib.tb200_plugin_render.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_float)]
     out = np.full((100, 128, 4), -3.0, np.float32)
-    rc = lib.tb200_plugin_render(ref.lib.ref_native_scene(ref.h), ref.lib.ref_native_camera(ref.h),
-                                 ref.lib.ref_native_options(ref.h), 5, out.ctypes.data_as(C.POINTER(C.c_float)))
+    with schedenv.knobs(TEST_DUP_DEVICES=dup):
+        rc = lib.tb200_plugin_render(ref.lib.ref_native_scene(ref.h), ref.lib.ref_native_camera(ref.h),
+                                     ref.lib.ref_native_options(ref.h), 5, out.ctypes.data_as(C.POINTER(C.c_float)))
     assert rc == 0
     oracle = ref.render_seeded(0, 5, 4)
     rel = np.linalg.norm((out - oracle).astype(np.float64)) / np.linalg.norm(oracle.astype(np.float64))
@@ -77,7 +82,6 @@ def test_plugin_fast_paths_render_n_and_finish(tmp_path):
     reference's own finish loop and PNG writer applied to the sums the call returned."""
     if not os.path.exists(PLUGIN) or not refdrv.have_ref("detmath"):
         pytest.skip("plugin or oracle/_ref not built")
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
     ref = refdrv.RefScene.from_snapshot(tb.scene_path("veach"), "detmath")
     ref.set_size(96, 80)
     lib = C.CDLL(PLUGIN)
@@ -119,7 +123,6 @@ def test_unmodified_tinsel_app_renders_through_the_plugin(tmp_path):
     import subprocess
     if not (os.path.exists(HEADLESS) and os.path.exists(HEADLESS_CPU)):
         pytest.skip("headless tinsel app not built (build container only)")
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
     imgs = {}
     for name, exe in (("gpu", HEADLESS), ("cpu", HEADLESS_CPU)):
         d = tmp_path / name

@@ -17,6 +17,7 @@ import fuzzscene
 import rayoracle
 import raysets
 import refdrv
+import schedenv
 
 pytestmark = pytest.mark.gpu
 
@@ -143,7 +144,7 @@ def test_mesh_with_device_built_bvh_matches_port():
 
 @pytest.mark.parametrize("variant", ["no_flat", "cached", "group"])
 @pytest.mark.parametrize("name", ["cornell", "meshlight", "fuzz_instanced"])
-def test_variants_give_the_same_bits(variant, name, monkeypatch, tmp_path):
+def test_variants_give_the_same_bits(variant, name, tmp_path):
     if name.startswith("fuzz_"):
         path = str(tmp_path / "s.tsnap")
         fuzzscene.make_mesh_scene(2, path, name[5:])
@@ -154,15 +155,15 @@ def test_variants_give_the_same_bits(variant, name, monkeypatch, tmp_path):
     rng = np.random.RandomState(5)
     rays = np.concatenate(list(_ray_sets(snap.scene.contents, snap.camera, port, rng).values()))
     if variant == "no_flat":
-        monkeypatch.setenv("TINSEL_B200_NO_FLAT", "1")
-        r = tb.Renderer(snap.scene)
+        with schedenv.knobs(**schedenv.ROUTES["no-flat"]):
+            r = tb.Renderer(snap.scene)
     elif variant == "cached":
         cache = str(tmp_path / "s.tcache")
         tb.scene_cache_save(snap.scene, cache)
         r = tb.Renderer(None, cache=cache)
     else:
-        monkeypatch.setenv("TINSEL_B200_TEST_DUP_DEVICES", "1")
-        r = tb.Renderer(snap.scene, devices=[0, 0])
+        with schedenv.knobs(TEST_DUP_DEVICES="1"):
+            r = tb.Renderer(snap.scene, devices=[0, 0])
         assert r.num_devices() == 2
     _check(r, port, rays, "%s/%s" % (name, variant))
     r.close()

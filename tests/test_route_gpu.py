@@ -2,9 +2,7 @@
 name through tb200_last_kernel.  Every kernel gives the same bits, so no image test notices a scene sent to the
 wrong one: this test restates the rule and checks the kernel that ran against it, under the default knobs and
 every scheduler variant of schedenv, at a small launch and at one of at least six samples per slot."""
-import contextlib
 import math
-import os
 
 import pytest
 import torch
@@ -16,16 +14,15 @@ import schedenv
 
 pytestmark = pytest.mark.gpu
 
-KNOBS = schedenv.KEYS + ("TINSEL_B200_SPECIALIZE", "TINSEL_B200_PIPELINE", "TINSEL_B200_TEST_LAUNCH_SAMPLES")
 SMALL = (64, 64)   # one frame of these is a small launch
 TUNE_SIZE = (256, 256)   # 4 frames of these are the 2^18 image samples a launch needs to advance the tuner
 SETTINGS = [None] + [(s, c) for s in schedenv.SCHEDS for c in schedenv.CTAS]
 
 
 @pytest.fixture(autouse=True)
-def clean_env(monkeypatch):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
+def default_knobs():
+    with schedenv.knobs():
+        yield
 
 
 @pytest.fixture(scope="module")
@@ -62,10 +59,9 @@ def facts(path):
     return out
 
 
-def route(f):
-    """The per-scene part of the rule, from the scene's facts and the knobs in the environment."""
-    knob = os.environ.get
-    sched, split, cta, queues, spec = (knob("TINSEL_B200_" + k) for k in ("SCHED", "SPLIT", "CTA", "QUEUES", "SPECIALIZE"))
+def route(f, knobs):
+    """The per-scene part of the rule, from the scene's facts and the knob settings schedenv.knobs applied."""
+    sched, split, cta, queues, spec = (knobs.get(k) for k in ("SCHED", "SPLIT", "CTA", "QUEUES", "SPECIALIZE"))
     hard = {"hard": True, "free": False}.get(sched, f["numNee"] > 1 and f["maxTris"] <= 4096)
     wide = {"768": True, "512": False}.get(cta, not hard and f["maxTris"] > 4096)
     in_use = f["box"] and (f["maxTris"] > 4096 or split == "1") and split != "0"
@@ -119,38 +115,38 @@ def test_defaults(scenes, num_sms):
 def test_route_matches_rule(name, setting, scenes, num_sms):
     f = facts(scenes[name])
     for spp in (1, large_spp(SMALL, num_sms)):
-        with schedenv.sched_env(*setting) if setting else contextlib.nullcontext():
-            want = kernel(route(f), SMALL[0] * SMALL[1] * spp, num_sms)
+        with schedenv.sched_env(*setting) if setting else schedenv.knobs() as knobs:
+            want = kernel(route(f, knobs), SMALL[0] * SMALL[1] * spp, num_sms)
             ran = run(scenes[name], SMALL, [spp])[0]
         assert ran == want, "%s %s, %d spp: ran %s, the rule says %s (facts %s)" % (name, setting, spp, ran, want, f)
 
 
-def test_tuner_default(scenes, monkeypatch):
+def test_tuner_default(scenes):
     """The tuner times phase 1 with the split queue and phase 2 without it, then keeps the faster."""
-    assert route(facts(scenes["big"]))["tune"]
+    assert route(facts(scenes["big"]), {})["tune"]
     ran = run(scenes["big"], TUNE_SIZE, [4] * 6)
     assert ran[:3] == ["wf2_l2.split", "wf2_l2.split", "wf2_l2.generic"], ran
     assert ran[3] in ("wf2_l2.split", "wf2_l2.generic") and ran[3:] == [ran[3]] * 3, ran
 
 
 @pytest.mark.parametrize("split,name", [("0", "wf2_l2.generic"), ("1", "wf2_l2.split")])
-def test_tuner_off_when_split_is_set(split, name, scenes, monkeypatch):
-    monkeypatch.setenv("TINSEL_B200_SPLIT", split)
-    assert run(scenes["big"], TUNE_SIZE, [4] * 6) == [name] * 6
+def test_tuner_off_when_split_is_set(split, name, scenes):
+    with schedenv.knobs(SPLIT=split):
+        assert run(scenes["big"], TUNE_SIZE, [4] * 6) == [name] * 6
 
 
 @pytest.mark.parametrize("size", ["small", "large"])
-def test_tuner_phase2_takes_rule_2(size, scenes, num_sms, monkeypatch):
+def test_tuner_phase2_takes_rule_2(size, scenes, num_sms):
     """With 512-thread CTAs the split queue runs on wf2_smem; phase 2 turns it off, so rule 2 applies: a launch of
     at least six samples per slot runs the lane-owned kernel, a smaller one the generic ring kernel."""
     spp = 4 if size == "small" else large_spp(TUNE_SIZE, num_sms)
     samples = TUNE_SIZE[0] * TUNE_SIZE[1] * spp
     assert samples >= 1 << 18 and (samples < 6 * num_sms * 1024) == (size == "small")
     f = facts(scenes["big"])
-    monkeypatch.setenv("TINSEL_B200_CTA", "512")
-    without = kernel(dict(route(f), split=False), samples, num_sms)
+    with schedenv.knobs(CTA="512") as knobs:
+        without = kernel(dict(route(f, knobs), split=False), samples, num_sms)
+        ran = run(scenes["big"], TUNE_SIZE, [spp] * 6)
     assert without == ("wf2_smem.generic" if size == "small" else
                        "wf2_lq.generic" if f["features"] else "wf2_lq.specialized")
-    ran = run(scenes["big"], TUNE_SIZE, [spp] * 6)
     assert ran[:3] == ["wf2_smem.split", "wf2_smem.split", without], ran
     assert ran[3] in ("wf2_smem.split", without) and ran[3:] == [ran[3]] * 3, ran

@@ -9,6 +9,13 @@ import numpy as np
 import pytest
 
 import tinsel_b200 as tb
+import schedenv
+
+
+@pytest.fixture(autouse=True)
+def default_knobs():
+    with schedenv.knobs():
+        yield
 
 
 def _cache(tmp_path, name):
@@ -76,7 +83,6 @@ def test_damaged_cache_files_are_refused(tmp_path):
                                        ("env", (256, 256))])
 def test_renderer_from_cache_is_bit_identical(tmp_path, name, size):
     snap, path = _cache(tmp_path, name)
-    os.environ["TINSEL_B200_PIPELINE"] = "wavefront"
     cam, opt = snap.camera, snap.options
     opt.width, opt.height = size
     a = tb.Renderer(snap.scene)

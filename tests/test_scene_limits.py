@@ -24,6 +24,12 @@ SMALL_CASES = [c for c in CASES if not c.startswith("prims")]      # 8 primitive
 NTHREADS = os.cpu_count() or 8
 
 
+@pytest.fixture(autouse=True)
+def default_knobs():
+    with schedenv.knobs():
+        yield
+
+
 def _size(case):
     return (24, 16) if case == "prims4095" else (48, 32)
 
@@ -202,25 +208,23 @@ def test_port_matches_reference_on_limit_scenes(case, scenes, port_frames):
 
 # ---- GPU ---------------------------------------------------------------------------------------------
 
-def _gpu_vs_port(path, port_frames, case, pipelines=(None,), frames=(0, 3)):
-    """{(pipeline, frame): samples that differ from the port}; pipeline None: the default routing."""
+def _gpu_vs_port(path, port_frames, case, routes, frames=(0, 3)):
+    """{(route, frame): samples that differ from the port}; routes: {route: its knob settings}."""
     snap = tb.Snapshot(path)
     cam, opt = snap.camera, snap.options
     bad = {}
     try:
-        for pipeline in pipelines:
-            if pipeline:
-                os.environ["TINSEL_B200_PIPELINE"] = pipeline
-            r = tb.Renderer(snap.scene)
+        for route, settings in routes.items():
+            with schedenv.knobs(**settings):
+                r = tb.Renderer(snap.scene)
             r.Init(opt.width, opt.height)
             for frame in frames:
                 rad, ras = r.trace_frame(cam, opt, frame)
                 n = _bad_samples(rad, ras, *port_frames(case, frame))
                 if n:
-                    bad[(pipeline, frame)] = n
+                    bad[(route, frame)] = n
             r.close()
     finally:
-        os.environ.pop("TINSEL_B200_PIPELINE", None)
         snap.close()
     return bad
 
@@ -230,9 +234,8 @@ def _gpu_vs_port(path, port_frames, case, pipelines=(None,), frames=(0, 3)):
 def test_gpu_matches_port_at_the_limits(case, scenes, port_frames):
     """Both pipelines as the default routing picks their kernels (for the many-shadow-ray scenes: hard phases and
     the ring queues, which store the NEE cursor between the shade and shadow stages)."""
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
     path, info = scenes(case)
-    bad = _gpu_vs_port(path, port_frames, case, pipelines=("mega", "wavefront"))
+    bad = _gpu_vs_port(path, port_frames, case, {p: schedenv.ROUTES[p] for p in ("mega", "wavefront")})
     assert not bad, "%s: samples differ %s" % (info["case"], bad)
 
 
@@ -241,18 +244,16 @@ def test_gpu_matches_port_at_the_limits(case, scenes, port_frames):
 @pytest.mark.parametrize("case", CASES)
 def test_limit_scenes_under_every_scheduler_variant(case, sched, cta, scenes, port_frames):
     path, info = scenes(case)
-    with schedenv.sched_env(sched, cta):
-        bad = _gpu_vs_port(path, port_frames, case)
+    bad = _gpu_vs_port(path, port_frames, case, {sched: schedenv.sched_knobs(sched, cta)})
     assert not bad, "%s %s/%s: samples differ %s" % (case, sched, cta, bad)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", SMALL_CASES)
-def test_small_limit_scenes_without_the_flat_program(case, scenes, port_frames, monkeypatch):
+def test_small_limit_scenes_without_the_flat_program(case, scenes, port_frames):
     """The scene level runs the reference-order walk instead of the flat program (default routing otherwise)."""
-    monkeypatch.setenv("TINSEL_B200_NO_FLAT", "1")
     path, info = scenes(case)
-    bad = _gpu_vs_port(path, port_frames, case)
+    bad = _gpu_vs_port(path, port_frames, case, {"no-flat": schedenv.ROUTES["no-flat"]})
     assert not bad, "%s: samples differ %s" % (case, bad)
 
 
@@ -261,7 +262,6 @@ def test_small_limit_scenes_without_the_flat_program(case, scenes, port_frames, 
 def test_limit_scene_images_match_port(case, scenes):
     """The 4-spp image against the port's seeded render (rel-L2 <= 1e-4: the framebuffer sums run in another
     order, NaN on the same pixels), and for the prims* scenes the normals image bit for bit."""
-    os.environ.pop("TINSEL_B200_PIPELINE", None)
     path, info = scenes(case)
     port = refdrv.PortScene.from_snapshot(path)
     snap = tb.Snapshot(path)

@@ -18,6 +18,7 @@ import occlusionsets
 import rayoracle
 import raysets
 import refdrv
+import schedenv
 
 pytestmark = pytest.mark.gpu
 
@@ -103,22 +104,19 @@ def test_small_meshes_per_sample(variant, tmp_path):
     snap = tb.Snapshot(path)
     cam, opt = snap.camera, snap.options
     lit = 0.0
-    try:
-        for pipeline in ("mega", "wavefront"):
-            os.environ["TINSEL_B200_PIPELINE"] = pipeline
+    for pipeline in ("mega", "wavefront"):
+        with schedenv.knobs(**schedenv.ROUTES[pipeline]):
             r = tb.Renderer(snap.scene)
-            r.Init(opt.width, opt.height)
-            for frame in (0, 3):
-                rad, ras = r.trace_frame(cam, opt, frame)
-                prad, pras = port.trace_frame(frame, 8)
-                assert np.array_equal(ras, pras)
-                same = (rad.view(np.uint32) == prad.view(np.uint32)) | (np.isnan(rad) & np.isnan(prad))
-                bad = int((~same.all(-1)).sum())
-                assert bad == 0, "%s/%s frame %d: %d of %d samples differ" % (variant, pipeline, frame, bad, rad.shape[0] * rad.shape[1])
-                lit += float(np.nan_to_num(rad).sum())
-            r.close()
-    finally:
-        os.environ.pop("TINSEL_B200_PIPELINE", None)
+        r.Init(opt.width, opt.height)
+        for frame in (0, 3):
+            rad, ras = r.trace_frame(cam, opt, frame)
+            prad, pras = port.trace_frame(frame, 8)
+            assert np.array_equal(ras, pras)
+            same = (rad.view(np.uint32) == prad.view(np.uint32)) | (np.isnan(rad) & np.isnan(prad))
+            bad = int((~same.all(-1)).sum())
+            assert bad == 0, "%s/%s frame %d: %d of %d samples differ" % (variant, pipeline, frame, bad, rad.shape[0] * rad.shape[1])
+            lit += float(np.nan_to_num(rad).sum())
+        r.close()
     assert lit > 0.0
     port.close()
     snap.close()

@@ -292,7 +292,6 @@ struct tb200_renderer {
     unsigned int* dBandFlags = nullptr;
     cudaStream_t copyStream = nullptr;
     unsigned int bandTag = 0;
-    int streamedReadback = 1;             // TINSEL_B200_READBACK=plain turns it off
 
     // host read-back: a caller-owned buffer pinned on request (tb200_pin_output), never implicitly
     void* registered = nullptr;
@@ -308,7 +307,7 @@ struct tb200_renderer {
     std::string workerError;              // a peer's failure message, handed to the calling thread
     bool peerAccess = false;
 
-    int pipeline = 2;             // 0 = mega (validation), 2 = wavefront (product)
+    Knobs knobs = {};             // read once, at the start of tb200_create* (read_knobs)
     Wf2Route route = {};          // the wavefront kernel's scheduling, decided at upload (kernels.cu: wavefront2_route)
     const char* lastKernel = "";  // the kernel the last path-tracing launch ran (tb200_last_kernel)
     // Split trace queue on/off is decided by measurement when route.tune (every variant produces the same bits):
@@ -317,7 +316,7 @@ struct tb200_renderer {
     double tuneRate[2] = {0.0, 0.0};   // samples per ms with / without the split queue
     unsigned long long launchSamples = 0;   // samples of the launch whose time is in stats.gpuMs
     // most samples (tile padding included) per launch: slot records keep a 32-bit sample index.
-    // TINSEL_B200_TEST_LAUNCH_SAMPLES lowers it, so that tests reach the split at small sizes.
+    // knobs.launchSamples lowers it, so that tests reach the split at small sizes.
     unsigned long long maxLaunchSamples = 0x7fffffffull;
     tb200_stats stats;
 };
@@ -495,7 +494,7 @@ bool upload(tb200_renderer* r, const std::vector<T>& host, const T** dev, size_t
     return true;
 }
 
-// device upload of a scene image + the per-scene scheduling decisions (which read the environment)
+// device upload of a scene image + the per-scene scheduling decisions (from r->knobs)
 bool upload_image(tb200_renderer* r, const SceneImage& img)
 {
     memset(&r->scene, 0, sizeof(r->scene));
@@ -513,7 +512,7 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
     sc.splitValid = img.splitBoxValid;
     sc.splitLo = img.splitLo;
     sc.splitHi = img.splitHi;
-    r->route = wavefront2_route(img.numNee, img.maxTris, img.splitBoxValid, scene_features(img));
+    r->route = wavefront2_route(img.numNee, img.maxTris, img.splitBoxValid, scene_features(img), r->knobs);
     r->tunePhase = r->route.tune ? 0 : 3;
     // one element of padding each: the kernels' bulk copies round their length up to 16 bytes
     if (!upload(r, img.prims, &sc.prims, 1)) return false;
@@ -521,7 +520,7 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
     sc.numPrims = (int)img.prims.size();
     sc.numPairs = (int)img.scenePairs.size();
     static const std::vector<ProgOp> noFlat;
-    const std::vector<ProgOp>& flat = getenv("TINSEL_B200_NO_FLAT") ? noFlat : img.flat;
+    const std::vector<ProgOp>& flat = r->knobs.noFlat ? noFlat : img.flat;
     if (!upload(r, flat, &sc.flat, 1)) return false;
     sc.numFlat = (int)flat.size();
     // treelet: the top of the largest mesh's BVH staged in the shared memory the slot arrays leave, for the
@@ -531,11 +530,10 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
     sc.treeletMesh = -1;
     sc.treeletPairs = 0;
     {
-        const char* tl = getenv("TINSEL_B200_TREELET");
         int big = -1;
         for (size_t m = 0; m < img.meshes.size(); ++m)
             if (img.meshes[m].numTris > 1024 && (big < 0 || img.meshes[m].numTris > img.meshes[big].numTris)) big = (int)m;
-        if (big >= 0 && tl && atoi(tl) == 1) {
+        if (big >= 0 && r->knobs.treelet) {
             sc.treeletMesh = big;
             sc.treeletPairs = (int)img.meshes[big].pairs.size();
         }
@@ -792,7 +790,7 @@ bool launch_frames(tb200_renderer* r, LaunchParams& P, bool recordStart = true)
         for (int f = 0; f < frames; f += framesPerLaunch) {
             P.frame0 = frame0 + f;
             P.numFrames = std::min(framesPerLaunch, frames - f);
-            const char* name = r->pipeline == 0 ? launch_mega(P, r->stream, &launches) : launch_wavefront2(P, r->route, r->numSMs, r->stream, &launches);
+            const char* name = r->knobs.mega ? launch_mega(P, r->stream, &launches) : launch_wavefront2(P, r->route, r->numSMs, r->stream, &launches);
             if (name) r->lastKernel = name;
         }
         P.frame0 = frame0;
@@ -937,7 +935,7 @@ bool render_streamed(tb200_renderer* r, LaunchParams& P, float* output, bool rec
 // else copied after the frames.  The frame counters advance only when all of this succeeded.
 bool run_frames(tb200_renderer* r, LaunchParams& P, int n, float* output)
 {
-    const bool streamed = output && r->streamedReadback && r->pipeline != 0 && P.samplesPerFrame > 0 && P.samplesPerFrame < 0x7fffffffull;
+    const bool streamed = output && !r->knobs.plainReadback && !r->knobs.mega &&P.samplesPerFrame > 0 && P.samplesPerFrame < 0x7fffffffull;
     const int head = streamed ? n - 1 : n;   // frames launched before the streamed one
     P.frame0 = r->frame;
     P.numFrames = head;
@@ -1183,8 +1181,36 @@ tb200_renderer* tb200_create_cached(const char* path, int device)
     return create_with(device, [img](tb200_renderer* r) { return upload_image(r, *img); });
 }
 
+// The library's one reader of the environment (tb_kernels.cuh: Knobs lists each variable and its parsing)
+static Knobs read_knobs()
+{
+    const auto is = [](const char* value, const char* word) { return value && strcmp(value, word) == 0; };
+    const char* cap = getenv("TINSEL_B200_TEST_LAUNCH_SAMPLES");
+    const char* sched = getenv("TINSEL_B200_SCHED");
+    const char* split = getenv("TINSEL_B200_SPLIT");
+    const char* cta = getenv("TINSEL_B200_CTA");
+    const char* queues = getenv("TINSEL_B200_QUEUES");
+    const char* spec = getenv("TINSEL_B200_SPECIALIZE");
+    const char* treelet = getenv("TINSEL_B200_TREELET");
+    Knobs k;
+    k.mega = is(getenv("TINSEL_B200_PIPELINE"), "mega");
+    k.plainReadback = is(getenv("TINSEL_B200_READBACK"), "plain");
+    k.launchSamples = cap ? strtoull(cap, nullptr, 10) : 0;
+    k.dupDevices = getenv("TINSEL_B200_TEST_DUP_DEVICES") != nullptr;
+    k.sched = is(sched, "hard") ? 1 : is(sched, "free") ? 0 : -1;
+    k.splitSet = split != nullptr;
+    k.split = split ? atoi(split) : 0;
+    k.cta = cta ? atoi(cta) : 0;
+    k.laneQueues = is(queues, "ring") ? 0 : is(queues, "lanes") ? 2 : 1;
+    k.specialize = !(spec && atoi(spec) == 0);
+    k.noFlat = getenv("TINSEL_B200_NO_FLAT") != nullptr;
+    k.treelet = treelet && atoi(treelet) == 1;
+    return k;
+}
+
 static tb200_renderer* create_with(int device, const std::function<bool(tb200_renderer*)>& build)
 {
+    const Knobs knobs = read_knobs();
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
         cudaGetLastError();
@@ -1198,6 +1224,8 @@ static tb200_renderer* create_with(int device, const std::function<bool(tb200_re
     tb200_renderer* r = new tb200_renderer();
     memset(&r->stats, 0, sizeof(r->stats));
     r->device = device;
+    r->knobs = knobs;
+    if (knobs.launchSamples > 0) r->maxLaunchSamples = std::min(knobs.launchSamples, r->maxLaunchSamples);   // test hook: lowers the cap, never raises it
     bool ok = cudaSetDevice(device) == cudaSuccess;
     cudaDeviceProp prop;
     ok = ok && cudaGetDeviceProperties(&prop, device) == cudaSuccess;
@@ -1209,14 +1237,6 @@ static tb200_renderer* create_with(int device, const std::function<bool(tb200_re
         set_error(std::string("tb200_create: device setup failed: ") + cudaGetErrorString(cudaGetLastError()));
         delete r;
         return nullptr;
-    }
-    const char* pipe = getenv("TINSEL_B200_PIPELINE");
-    if (pipe && strcmp(pipe, "mega") == 0) r->pipeline = 0;
-    const char* rb = getenv("TINSEL_B200_READBACK");
-    if (rb && strcmp(rb, "plain") == 0) r->streamedReadback = 0;
-    if (const char* cap = getenv("TINSEL_B200_TEST_LAUNCH_SAMPLES")) {   // test hook: lowers the cap, never raises it
-        const unsigned long long n = strtoull(cap, nullptr, 10);
-        if (n > 0) r->maxLaunchSamples = std::min(n, r->maxLaunchSamples);
     }
     unsigned int* hostFlags = nullptr;
     // cold slot state for every CTA a launch can have (one or two per SM, see launch_wavefront2): 8 float4 per slot
@@ -1244,9 +1264,10 @@ tb200_renderer* tb200_create_multi(const tb200_scene* scene, const int* devices,
         set_error("tb200_create_multi: bad device list");
         return nullptr;
     }
+    const bool dupDevices = read_knobs().dupDevices;   // test hook: a one-GPU box
     for (int a = 0; a < numDevices; ++a)
         for (int b = 0; b < a; ++b)
-            if (devices[a] == devices[b] && !getenv("TINSEL_B200_TEST_DUP_DEVICES")) {   // test hook: a one-GPU box
+            if (devices[a] == devices[b] && !dupDevices) {
                 set_error("tb200_create_multi: a device is listed twice");
                 return nullptr;
             }

@@ -373,7 +373,7 @@ static const struct {
 enum { WF2_L2_SPLIT, WF2_L2_GENERIC, WF2_LQ_NONE, WF2_LQ_ALL, WF2_SMEM_HARD, WF2_SMEM_SPLIT, WF2_SMEM_GENERIC };
 
 // Which of the seven kernels runs: every one produces the same bits, so the choice is speed alone.
-// Per scene (wavefront2_route, at upload in tb200_create / tb200_create_cached, reading the knobs then):
+// Per scene (wavefront2_route, at upload in tb200_create / tb200_create_cached, from the knobs read at its start):
 //  * hardPhases = numNee > 1 && maxTris <= 4096 (TINSEL_B200_SCHED=hard|free overrides).  Block-synchronous stages
 //    win when every hit spawns several shadow rays (the barrier keeps all warps on one stage's code); free-running
 //    warps win otherwise, by a wide margin when ray cost varies (deep mesh BVHs).
@@ -392,25 +392,20 @@ enum { WF2_L2_SPLIT, WF2_L2_GENERIC, WF2_LQ_NONE, WF2_LQ_ALL, WF2_SMEM_HARD, WF2
 //     round 2).  The specialised kernel has 512-thread CTAs too: at 640 (20 warps, 96 registers) it spills 128
 //     bytes and measured no faster on cornell.
 //  3. Otherwise wf2_smem.hard when hardPhases, else wf2_smem.split when split, else wf2_smem.generic.
-Wf2Route wavefront2_route(int numNee, int maxTris, bool splitBox, uint32_t features)
+Wf2Route wavefront2_route(int numNee, int maxTris, bool splitBox, uint32_t features, const Knobs& knobs)
 {
-    const char* sched = getenv("TINSEL_B200_SCHED");
-    const char* split = getenv("TINSEL_B200_SPLIT");
-    const char* cta = getenv("TINSEL_B200_CTA");
-    const char* queues = getenv("TINSEL_B200_QUEUES");
-    const char* spec = getenv("TINSEL_B200_SPECIALIZE");
     Wf2Route r;
     r.hardPhases = numNee > 1 && maxTris <= 4096;
-    if (sched && strcmp(sched, "hard") == 0) r.hardPhases = true;
-    if (sched && strcmp(sched, "free") == 0) r.hardPhases = false;
+    if (knobs.sched == 1) r.hardPhases = true;
+    if (knobs.sched == 0) r.hardPhases = false;
     r.wideCta = !r.hardPhases && maxTris > 4096;
-    if (cta && atoi(cta) == 768) r.wideCta = true;
-    if (cta && atoi(cta) == 512) r.wideCta = false;
-    const bool splitQueue = splitBox && (maxTris > 4096 || (split && atoi(split) == 1)) && !(split && atoi(split) == 0);
+    if (knobs.cta == 768) r.wideCta = true;
+    if (knobs.cta == 512) r.wideCta = false;
+    const bool splitQueue = splitBox && (maxTris > 4096 || (knobs.splitSet && knobs.split == 1)) && !(knobs.splitSet && knobs.split == 0);
     r.split = !r.hardPhases && splitQueue;
-    r.tune = r.split && !split;
-    r.laneQueues = !queues ? 1 : strcmp(queues, "ring") == 0 ? 0 : strcmp(queues, "lanes") == 0 ? 2 : 1;
-    r.specialized = features == TB_FEAT_NONE && !(spec && atoi(spec) == 0);
+    r.tune = r.split && !knobs.splitSet;
+    r.laneQueues = knobs.laneQueues;
+    r.specialized = features == TB_FEAT_NONE && knobs.specialize;
     return r;
 }
 

@@ -51,6 +51,38 @@ struct Wf2Route {
     int laneQueues;     // lane-owned slots with bit-set queues: 0 never, 1 for launches that are not small, 2 always
 };
 
+// The run-time knobs (README, "Run-time knobs"): environment variables that choose between variants which all give
+// the same bits.  api.cu: read_knobs is the library's only reader of them; each tb200_create* call reads them once,
+// at its start.  Each variable, how its value is read, and what it does:
+//   TINSEL_B200_PIPELINE=mega          mega: the validation kernel k_mega (one thread per path) instead of the wavefront kernel
+//   TINSEL_B200_READBACK=plain         plainReadback: tb200_render copies after the launch instead of streaming rows under it
+//   TINSEL_B200_TEST_LAUNCH_SAMPLES=n  launchSamples (strtoull): test hook, n > 0 lowers the 2^31-1 samples per launch
+//   TINSEL_B200_TEST_DUP_DEVICES       dupDevices (set at all): test hook, tb200_create_multi accepts a device twice
+//   TINSEL_B200_SCHED=hard|free        sched (1, 0; -1 for any other value): forces Wf2Route::hardPhases
+//   TINSEL_B200_SPLIT=1|0              splitSet, split (atoi): 1 forces the split trace queue on, 0 off; set to any
+//                                      value at all, it turns off the tuner (Wf2Route::tune)
+//   TINSEL_B200_CTA=768|512            cta (atoi): forces Wf2Route::wideCta on or off; other values leave the rule's
+//   TINSEL_B200_QUEUES=ring|lanes      laneQueues: Wf2Route::laneQueues 0 or 2; unset or any other value gives 1
+//   TINSEL_B200_SPECIALIZE=0           specialize (false when atoi is 0, non-numeric text included): featureless
+//                                      scenes run the generic lane-owned kernel
+//   TINSEL_B200_NO_FLAT                noFlat (set at all, even to 0): the scene level runs the reference-order BVH
+//                                      walk instead of the flat scene program
+//   TINSEL_B200_TREELET=1              treelet (atoi is 1): stage the top of the biggest mesh's BVH in shared memory
+struct Knobs {
+    bool mega;
+    bool plainReadback;
+    unsigned long long launchSamples;   // 0 when unset
+    bool dupDevices;
+    int sched;
+    bool splitSet;
+    int split;
+    int cta;
+    int laneQueues;
+    bool specialize;
+    bool noFlat;
+    bool treelet;
+};
+
 #define TB_MAX_BANDS 64
 
 // fills tilesX / tileRows / samplesPerFrame and their division multipliers from the row range and shard
@@ -62,8 +94,9 @@ void divisor_magic(uint32_t d, uint32_t* mul, uint32_t* shift);
 // one thread per (pixel, frame): the whole path in registers.  Validation / fallback pipeline.
 const char* launch_mega(const LaunchParams& p, cudaStream_t stream, unsigned long long* launchCount);
 // persistent CTA-resident wavefront pipeline with a dedicated traversal stage (the product path), and its route for
-// a scene of numNee shadow rays per hit, largest mesh maxTris triangles (splitBox: its box in DScene), features
-Wf2Route wavefront2_route(int numNee, int maxTris, bool splitBox, uint32_t features);
+// a scene of numNee shadow rays per hit, largest mesh maxTris triangles (splitBox: its box in DScene), features,
+// under the renderer's knobs
+Wf2Route wavefront2_route(int numNee, int maxTris, bool splitBox, uint32_t features, const Knobs& knobs);
 const char* launch_wavefront2(const LaunchParams& p, const Wf2Route& route, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds: the per-stage cycle counters of the lane-owned wavefront layout (wf2_lanes.cuh), summed
