@@ -332,6 +332,25 @@ int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, 
  * numRays == 0 launches nothing.  Returns 0 on success. */
 int tb200_occluded_rays(tb200_renderer* r, const tb200_ray* rays, uint8_t* occluded, int64_t numRays);
 
+/* ---- batched closest-hit ray query with the hit triangle -----------------------------------
+ * hits[i] and prims[i] are bit for bit what tb200_trace_rays writes for the same ray.  When prims[i] is
+ * a mesh primitive, tris[i] describes the triangle whose hit Trace kept:
+ *   tri      its index in that primitive's mesh: its vertices are indices[3*tri .. 3*tri+2] of the
+ *            tb200_mesh the scene was created from
+ *   u, v, w  IntersectRayTriTwoSided's barycentric weights (intersection.h:117-145): v weights
+ *            indices[3*tri+1], w weights indices[3*tri+2], and u = 1 - v - w as the reference rounds it
+ * so u*N[i0] + v*N[i1] + w*N[i2] is the smooth normal before its flip, transform and normalisation
+ * (intersection.h:994-1013).  The weights are in the mesh's own space: an instance transform, motion
+ * included, does not change them.  Ties are Trace's: the first primitive in the reference's order wins,
+ * and inside a mesh the first triangle in walk order.  A sphere hit, a plane hit or a miss gives
+ * tri = -1 and u = v = w = 0.  tris (numRays records, 16-byte aligned) is DEVICE memory like the other
+ * arrays; the refusals, stream, synchronisation and side effects are tb200_trace_rays': it adds 1 to
+ * stats.kernelLaunches, sets stats.gpuMs to its kernel's time, and touches nothing else.  numRays == 0
+ * launches nothing.  `pad` is ignored.  Returns 0 on success. */
+typedef struct tb200_tri_hit { int32_t tri; float u, v, w; } tb200_tri_hit;   /* 16 B */
+int tb200_trace_rays_tri(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims,
+                         tb200_tri_hit* tris, int64_t numRays);
+
 /* Sets the frame counter (frame k seeds sample k of every pixel). */
 void tb200_set_frame(tb200_renderer* r, int frame);
 

@@ -84,6 +84,8 @@ def load_library():
     lib.tb200_trace_frame.argtypes = [C.c_void_p, C.POINTER(Camera), C.POINTER(Options), C.c_int, f32p, f32p]
     lib.tb200_trace_rays.restype = C.c_int
     lib.tb200_trace_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_trace_rays_tri.restype = C.c_int
+    lib.tb200_trace_rays_tri.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_occluded_rays.restype = C.c_int
     lib.tb200_occluded_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_set_frame.restype = None
@@ -347,6 +349,30 @@ class Renderer:
         self._wait_for_torch()
         self._check(self.lib.tb200_trace_rays(self.h, rays.data_ptr(), hits.data_ptr(), prims.data_ptr(), n), "tb200_trace_rays")
         return hits, prims
+
+    def trace_rays_tri(self, rays, hits=None, prims=None, tris=None):
+        """trace_rays, plus the triangle each mesh hit lies on (tb200_trace_rays_tri).  Returns (hits, prims) as
+        trace_rays does, bit for bit, and (tri (N,) int32, uvw (N, 3) float32): the hit triangle's index in its mesh
+        and its barycentric weights, u*N[i0] + v*N[i1] + w*N[i2] over the triangle's vertices i0, i1, i2 in the mesh's
+        own space; tri = -1 and uvw = 0 for a sphere hit, a plane hit or a miss.  Both are views of one (N, 4) int32
+        tensor, the tb200_tri_hit records, which `tris` gives when it is passed.  Stream behaviour as for trace_rays."""
+        import torch
+        n = self._check_rays(rays)
+        dev = torch.device("cuda", self.device)
+        if hits is None:
+            hits = torch.empty((n, 4), dtype=torch.float32, device=dev)
+        if prims is None:
+            prims = torch.empty((n,), dtype=torch.int32, device=dev)
+        if tris is None:
+            tris = torch.empty((n, 4), dtype=torch.int32, device=dev)
+        self._check_tensor(hits, "hits", (n, 4), torch.float32)
+        self._check_tensor(prims, "prims", (n,), torch.int32)
+        self._check_tensor(tris, "tris", (n, 4), torch.int32)
+        if n > 0:
+            self._wait_for_torch()
+            self._check(self.lib.tb200_trace_rays_tri(self.h, rays.data_ptr(), hits.data_ptr(), prims.data_ptr(),
+                                                      tris.data_ptr(), n), "tb200_trace_rays_tri")
+        return hits, prims, tris[:, 0], tris[:, 1:].view(torch.float32)
 
     def occluded(self, rays, out=None):
         """Whether anything blocks each ray before its tmax (tb200_occluded_rays): exactly `Trace (src/render.cpp:17-62)

@@ -150,6 +150,11 @@ class Hit(C.Structure):
     _fields_ = [("t", C.c_float), ("normal", C.c_float * 3)]
 
 
+class TriHit(C.Structure):
+    """tb200_tri_hit: the hit triangle and its barycentric weights, from tb200_trace_rays_tri (16 bytes)."""
+    _fields_ = [("tri", C.c_int32), ("u", C.c_float), ("v", C.c_float), ("w", C.c_float)]
+
+
 class BvhBuildInfo(C.Structure):
     _fields_ = [("numNodes", C.c_int32), ("rounds", C.c_int32), ("kernelLaunches", C.c_uint64), ("buildMs", C.c_double)]
 
@@ -191,6 +196,7 @@ EXPORTS = [
     "tb200_nlm",
     "tb200_trace_frame",
     "tb200_trace_rays",
+    "tb200_trace_rays_tri",
     "tb200_occluded_rays",
     "tb200_set_frame",
     "tb200_get_stats",

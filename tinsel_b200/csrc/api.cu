@@ -1907,6 +1907,29 @@ int tb200_occluded_rays(tb200_renderer* r, const tb200_ray* rays, uint8_t* occlu
     return query_run(entry, r, [&](unsigned long long* launches) { launch_occluded_rays(Q, r->numSMs, r->stream, launches); });
 }
 
+int tb200_trace_rays_tri(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, tb200_tri_hit* tris, int64_t numRays)
+{
+    const char* entry = "tb200_trace_rays_tri";
+    const int begin = query_begin(entry, r, numRays);
+    if (begin != 0) return begin < 0 ? -1 : 0;
+    const size_t n = (size_t)numRays;
+    if (!check_device_span(entry, r, rays, n * sizeof(tb200_ray), 16, "rays") ||
+        !check_device_span(entry, r, hits, n * sizeof(tb200_hit), 16, "hits") ||
+        !check_device_span(entry, r, prims, n * sizeof(int32_t), 4, "prims") ||
+        !check_device_span(entry, r, tris, n * sizeof(tb200_tri_hit), 16, "tris"))
+        return -1;
+    static_assert(sizeof(tb200_tri_hit) == 16, "the query kernel writes one int4 per triangle record");
+    TriQueryParams Q;
+    Q.scene = r->scene;
+    Q.rays = reinterpret_cast<const float4*>(rays);
+    Q.hits = reinterpret_cast<float4*>(hits);
+    Q.prims = prims;
+    Q.tris = reinterpret_cast<int4*>(tris);
+    Q.numRays = numRays;
+    Q.counter = r->mem.counter.get();
+    return query_run(entry, r, [&](unsigned long long* launches) { launch_trace_rays_tri(Q, r->numSMs, r->stream, launches); });
+}
+
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds only (-DTB_WF2_STAGE_CLOCKS, tools/stage_clocks.py): copies the lane-owned wavefront
 // layout's per-stage cycle counters of the current device into out[0..n) (n >= 15 words, see wf2_lanes.cuh:

@@ -148,3 +148,16 @@ struct OcclusionParams {
     unsigned long long* counter;   // work counter, cleared by the launch
 };
 const char* launch_occluded_rays(const OcclusionParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
+
+// Batched closest-hit query that also reports the triangle (tb200_trace_rays_tri, tb_query.cuh): tb200_trace_rays'
+// outputs plus the winner's triangle and barycentric weights.  Its own struct, so that k_trace_rays keeps its code.
+struct TriQueryParams {
+    DScene scene;
+    const float4* rays;   // 2 per ray: origin.xyz, time; dir.xyz, pad
+    float4* hits;         // 1 per ray: t, normal.xyz
+    int* prims;           // 1 per ray: closest primitive, -1 on a miss
+    int4* tris;           // 1 per ray: triangle, then the bits of u, v, w; -1, 0, 0, 0 unless a mesh was hit
+    long long numRays;
+    unsigned long long* counter;   // work counter, cleared by the launch
+};
+const char* launch_trace_rays_tri(const TriQueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);

@@ -16,6 +16,7 @@
 #pragma once
 
 #include <algorithm>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -481,6 +482,16 @@ struct PrimHit {
     V3 gn;     // MeshQuery::closestNormal (n*sign, unnormalised)
 };
 
+// What trace_ordered() and trace_closest() return: Hit, and with REC also the winner's PrimHit (the closest-hit query
+// that reports the triangle, tb200_trace_rays_tri).  The record is the winner's only when the winner is a mesh.  REC
+// is a template parameter rather than an output pointer, so that the instantiations without it -- every caller but
+// that query's kernel -- keep their code.
+struct HitRec : Hit {
+    PrimHit rec;
+};
+template <bool REC>
+using TraceHit = typename std::conditional<REC, HitRec, Hit>::type;
+
 template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV bool prim_test(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, PrimHit& ph)
 {
@@ -549,8 +560,8 @@ TB_DEV V3 prim_normal(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, 
 // Trace + QueryBVH, render.cpp:17-62 + intersection.h:751-799: near-first DFS over the scene
 // BVH with NO closest-t culling; the callback keeps `t < minT && t > 0` (first found wins ties).
 // This is the reference's visit order, bit for bit.
-template <uint32_t FEAT = TB_FEAT_ALL>
-TB_ORDERED_ATTR Hit trace_ordered(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
+template <uint32_t FEAT = TB_FEAT_ALL, bool REC = false>
+TB_ORDERED_ATTR TraceHit<REC> trace_ordered(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
 {
     const V3 rcp = ray_rcp(d);
     uint32_t stack[TB_STACK];
@@ -590,12 +601,13 @@ TB_ORDERED_ATTR Hit trace_ordered(const DScene& sc, V3 o, V3 d, float time, bool
             if (hitRight) stack[count++] = right;
         }
     }
-    Hit h;
+    TraceHit<REC> h;
     h.t = minT;
     h.prim = closest;
     V3 n = v3s(0.0f);
     if (wantNormal && closest >= 0) n = prim_normal<FEAT>(sc, sc.prims[closest], o, d, time, best);
     h.n = face_forward(n, -d);
+    if constexpr (REC) h.rec = best;
     return h;
 }
 
@@ -632,11 +644,11 @@ TB_DEV bool flat_guard(const V3& o, const V3& d)
 
 // `flat` is sc.flat, or the same program where the caller can name it in shared memory (the lane-owned wavefront
 // kernel: Wf2Shared::flat), so that the op loads compile to shared-memory loads instead of generic ones.
-template <uint32_t FEAT = TB_FEAT_ALL>
-TB_DEV Hit trace_closest(const DScene& sc, const ProgOp* flat, V3 o, V3 d, float time, bool wantNormal)
+template <uint32_t FEAT = TB_FEAT_ALL, bool REC = false>
+TB_DEV TraceHit<REC> trace_closest(const DScene& sc, const ProgOp* flat, V3 o, V3 d, float time, bool wantNormal)
 {
     const int n = sc.numFlat;
-    if (n == 0 || !flat_guard(o, d)) return trace_ordered<FEAT>(sc, o, d, time, wantNormal);
+    if (n == 0 || !flat_guard(o, d)) return trace_ordered<FEAT, REC>(sc, o, d, time, wantNormal);
 
     const V3 rcp = ray_rcp(d);
 
@@ -688,8 +700,8 @@ TB_DEV Hit trace_closest(const DScene& sc, const ProgOp* flat, V3 o, V3 d, float
             }
         }
     }
-    if (tie) return trace_ordered<FEAT>(sc, o, d, time, wantNormal);
-    Hit h;
+    if (tie) return trace_ordered<FEAT, REC>(sc, o, d, time, wantNormal);
+    TraceHit<REC> h;
     h.t = minT;
     h.prim = closest;
     V3 nrm = v3s(0.0f);
@@ -698,13 +710,14 @@ TB_DEV Hit trace_closest(const DScene& sc, const ProgOp* flat, V3 o, V3 d, float
         nrm = prim_normal<FEAT>(sc, sc.prims[closest], o, d, time, rec[ri]);
     }
     h.n = face_forward(nrm, -d);
+    if constexpr (REC) h.rec = rec[ri];
     return h;
 }
 
-template <uint32_t FEAT = TB_FEAT_ALL>
-TB_DEV Hit trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
+template <uint32_t FEAT = TB_FEAT_ALL, bool REC = false>
+TB_DEV TraceHit<REC> trace_closest(const DScene& sc, V3 o, V3 d, float time, bool wantNormal)
 {
-    return trace_closest<FEAT>(sc, sc.flat, o, d, time, wantNormal);
+    return trace_closest<FEAT, REC>(sc, sc.flat, o, d, time, wantNormal);
 }
 
 // ---- occlusion (any-hit) query: trace_occluded() answers `Trace(o, d, time) hits a primitive with t < tmax`

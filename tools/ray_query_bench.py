@@ -1,13 +1,18 @@
 #!/usr/bin/env python
-"""Throughput of the batched closest-hit and occlusion queries (Renderer.trace_rays / tb200_trace_rays and
-Renderer.occluded / tb200_occluded_rays), one JSON line per scene:
+"""Throughput of the batched closest-hit and occlusion queries (Renderer.trace_rays / tb200_trace_rays,
+Renderer.trace_rays_tri / tb200_trace_rays_tri and Renderer.occluded / tb200_occluded_rays), one JSON line per scene:
     python tools/ray_query_bench.py [--scenes cornell,veach,meshlight,ajax,env] [--calls 10] [--warmup 3]
 
 Closest hit, per scene: Mrays/s for 2^24 coherent camera rays (a raster-order 4096 x 4096 grid, jittered) and 2^24
 random rays (origins in and around the scene bounds, uniform directions), from CUDA events around `--calls` timed
 calls after the warm-up; the bytes each ray moves (32 in, 20 out) against the H100 SXM's 3.35 TB/s; the CPU
 restatement's rate on every host core (tests/rayoracle.py); a bit-exact check of 2^16 rays against it; and the GPU's
-name and power limit, read in the same run.
+name, power limit and maximum SM clock, read in the same run.
+
+Closest hit with the hit triangle (key "tri"), on the same camera and random batches: the same rates (68 bytes per
+ray: 32 in, 16 + 4 + 16 out), the kernel time against trace_rays' on the same rays, the fraction of rays that hit a
+mesh, and a bit-exact check of 2^16 rays (hits, primitives, triangles and weights) against the restatement
+(tests/trioracle.py).
 
 Occlusion (key "occluded"), on the same batches: the camera rays with tmax = +inf, the random rays with tmax uniform
 in [0, the scene's diagonal), and point-to-point segments built on the device from the camera rays' hit points to
@@ -32,21 +37,24 @@ import tinsel_b200 as tb  # noqa: E402
 import occlusionsets  # noqa: E402
 import rayoracle  # noqa: E402
 import raysets  # noqa: E402
+import trioracle  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
 BYTES_PER_RAY = 32 + 16 + 4
 OCC_BYTES_PER_RAY = 32 + 1
+TRI_BYTES_PER_RAY = 32 + 16 + 4 + 16
 
 
 def gpu_info():
     try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = [x.strip() for x in out.split(",")]
-        return name, power
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, power, clock = [x.strip() for x in out.split(",")]
+        return name, power, clock
     except Exception as e:   # the rates are still measured; the line says what could not be read
         import torch
-        return torch.cuda.get_device_name(0), "unknown (%s)" % type(e).__name__
+        unknown = "unknown (%s)" % type(e).__name__
+        return torch.cuda.get_device_name(0), unknown, unknown
 
 
 def camera_rays_device(torch, camera, side, seed):
@@ -144,6 +152,23 @@ def occlusion_arm(torch, r, port, rays, occ, trace_kms, args):
     return out
 
 
+def tri_arm(torch, r, port, rays, hits, prims, tris, trace_kms, args):
+    """The closest-hit query with the hit triangle on `rays`: rates, kernel time against trace_rays' (trace_kms, on the
+    same rays), the mesh-hit fraction and a bit-exact check of the first 2^16 rays against the restatement."""
+    n = len(rays)
+    ms, kms = time_calls(torch, r, lambda: r.trace_rays_tri(rays, hits, prims, tris), args.warmup, args.calls)
+    out = rates(n, ms, kms, TRI_BYTES_PER_RAY)
+    out["trace_rays_kernel_ms"] = round(trace_kms, 4)
+    out["kernel_ms_over_trace_rays"] = round(kms / trace_kms, 4) if trace_kms > 0 else None
+    out["mesh_hit_fraction"] = round(float((tris[:, 0] >= 0).float().mean()), 4)
+    k = min(n, 1 << 16)
+    want_h, want_p, want_tri, want_uvw = port.trace_rays_tri(rays[:k].cpu().numpy())
+    got = tris[:k].cpu().numpy()
+    out["bit_exact_2^16"] = (len(raysets.mismatches(hits[:k].cpu().numpy(), prims[:k].cpu().numpy(), want_h, want_p)) == 0 and
+                             bool((got[:, 0] == want_tri).all()) and bool((got[:, 1:] == want_uvw.view(np.int32)).all()))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--scenes", default="cornell,veach,meshlight,ajax,env")
@@ -155,7 +180,8 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("ray_query_bench: no CUDA device (the rates are GPU measurements)")
     rayoracle.load()
-    gpu, power = gpu_info()
+    trioracle.load()
+    gpu, power, clock = gpu_info()
     n = 1 << args.log2_rays
     side = 1 << (args.log2_rays // 2)
     for name in args.scenes.split(","):
@@ -166,14 +192,17 @@ def main():
         scene = snap.scene.contents
         r = tb.Renderer(snap.scene)
         port = rayoracle.RayOracle.from_snapshot(path)
-        line = {"scene": name, "rays": n, "gpu": gpu, "power_limit": power,
+        tri_port = trioracle.TriOracle.from_snapshot(path)
+        line = {"scene": name, "rays": n, "gpu": gpu, "power_limit": power, "max_sm_clock": clock,
                 "library": os.path.basename(os.environ.get("TINSEL_B200_LIB", tb.LIB_PATH))}
         hits = torch.empty((n, 4), device="cuda")
         prims = torch.empty((n,), device="cuda", dtype=torch.int32)
         occ = torch.empty((n,), device="cuda", dtype=torch.bool)
+        tris = torch.empty((n, 4), device="cuda", dtype=torch.int32)
         lo, hi = raysets.scene_bounds(scene)
         diagonal = float(np.linalg.norm(hi - lo))
         line["occluded"] = {}
+        line["tri"] = {}
         for kind in ("camera", "random"):
             rays = camera_rays_device(torch, snap.camera, side, 1) if kind == "camera" else random_rays_device(torch, scene, n, 2)
             ms, kms = time_calls(torch, r, lambda: r.trace_rays(rays, hits, prims), args.warmup, args.calls)
@@ -187,6 +216,8 @@ def main():
             got_h, got_p = hits[:k].cpu().numpy(), prims[:k].cpu().numpy()
             line[kind]["bit_exact_2^16"] = len(raysets.mismatches(got_h, got_p, want_h[:k], want_p[:k])) == 0
             line[kind]["hit_fraction"] = round(float((prims >= 0).float().mean()), 4)
+            # the query with the hit triangle on the same rays (it writes the same hits and prims)
+            line["tri"][kind] = tri_arm(torch, r, tri_port, rays, hits, prims, tris, kms, args)
             # the occlusion query on the same rays
             if kind == "camera":
                 rays[:, 7] = float("inf")
@@ -205,6 +236,7 @@ def main():
         print(json.dumps(line), flush=True)
         r.close()
         port.close()
+        tri_port.close()
         snap.close()
 
 
