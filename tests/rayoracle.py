@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE: the CPU restatement's Trace over a whole batch of rays (tests/trace_rays_oracle.cpp), the arm
-the device's closest-hit query is checked against.  The library is compiled on first use, with oracle/Makefile's
+the device's closest-hit queries are checked against.  The library is compiled on first use, with oracle/Makefile's
 flags, from the restatement's unchanged source, into a temporary directory keyed by the sources' hash (the
 repository tree may be read-only)."""
 import ctypes as C
@@ -46,13 +46,17 @@ def load():
     lib.oracle_destroy.argtypes = [C.c_void_p]
     lib.oracle_trace_rays.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_longlong, C.POINTER(C.c_float),
                                       C.POINTER(C.c_int32), C.c_int]
+    lib.oracle_trace_rays_tri.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_longlong, C.POINTER(C.c_float),
+                                          C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]
     abi.declare_snapshot_api(lib)
     _lib = lib
     return lib
 
 
 class RayOracle:
-    """The restatement over a tb200_scene; trace_rays(rays (N, 8) float32) -> (hits (N, 4), prims (N,))."""
+    """The restatement over a tb200_scene; trace_rays(rays (N, 8) float32) -> (hits (N, 4), prims (N,)), and
+    trace_rays_tri(rays) -> (hits, prims, tri (N,), uvw (N, 3) float32), the shapes and meaning of
+    Renderer.trace_rays_tri."""
 
     def __init__(self, scene_ptr, keepalive=None):
         self.lib = load()
@@ -81,6 +85,16 @@ class RayOracle:
                                    hits.ctypes.data_as(C.POINTER(C.c_float)), prims.ctypes.data_as(C.POINTER(C.c_int32)),
                                    nthreads or os.cpu_count() or 1)
         return hits, prims
+
+    def trace_rays_tri(self, rays, nthreads=None):
+        rays = np.ascontiguousarray(rays, np.float32).reshape(-1, 8)
+        hits = np.zeros((len(rays), 4), np.float32)
+        prims = np.zeros(len(rays), np.int32)
+        tris = np.zeros((len(rays), 4), np.int32)
+        self.lib.oracle_trace_rays_tri(self.h, rays.ctypes.data_as(C.POINTER(C.c_float)), len(rays),
+                                       hits.ctypes.data_as(C.POINTER(C.c_float)), prims.ctypes.data_as(C.POINTER(C.c_int32)),
+                                       tris.ctypes.data_as(C.POINTER(C.c_int32)), nthreads or os.cpu_count() or 1)
+        return hits, prims, tris[:, 0], tris[:, 1:].view(np.float32)
 
     def close(self):
         if self.h:

@@ -13,19 +13,16 @@ import numpy as np
 import pytest
 
 import tinsel_b200 as tb
-from tinsel_b200 import abi
-import fuzzscene
+from queryscenes import FUZZ, N, SNAPSHOTS
 import occlusionsets
+import queryscenes
 import rayoracle
 import raysets
 import refdrv
-import schedenv
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SNAPSHOTS = sorted(f[:-6] for f in os.listdir(os.path.join(ROOT, "scenes")) if f.endswith(".tsnap"))
-N = 1 << 15
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -62,13 +59,6 @@ def _check(r, port, rays, rng, what=""):
     return hits, prims
 
 
-def _ray_sets(scene, camera, port, rng):
-    cam = raysets.camera_rays(camera, N, rng)
-    h, p = port.trace_rays(cam)
-    return {"camera": cam, "random": raysets.random_rays(scene, N, rng), "secondary": raysets.secondary_rays(cam, h, p, rng),
-            "fallback": raysets.fallback_rays(scene, rng)}
-
-
 def _check_point_to_point(r, port, camera, rng, what):
     """Segments between the hit points of two camera batches (the shadow-ray use), with tmax 1 - 1e-4 and 1."""
     a = raysets.camera_rays(camera, N, rng)
@@ -91,7 +81,7 @@ def test_snapshot_occlusion_matches_port(name):
     port = rayoracle.RayOracle.from_snapshot(tb.scene_path(name))
     r = tb.Renderer(snap.scene)
     rng = np.random.RandomState(zlib.crc32(name.encode()) & 0xffff)
-    sets = _ray_sets(snap.scene.contents, snap.camera, port, rng)
+    sets = queryscenes.ray_sets(snap.scene.contents, snap.camera, port, rng)
     if name == "motionblur":   # times outside the shutter too
         sets["motion"] = raysets.camera_rays(snap.camera, N, rng, time=rng.uniform(-0.5, 1.5, N))
         sets["motion_random"] = raysets.random_rays(snap.scene.contents, N, rng, (-0.5, 1.5))
@@ -117,23 +107,15 @@ def test_snapshot_occlusion_matches_port(name):
     snap.close()
 
 
-FUZZ = [("ties", 0, False), ("ties", 0, True), ("ties", 3, True), ("many", 1, False), ("big", 0, False),
-        ("caterpillar", 0, False), ("instanced", 0, False), ("instanced", 1, False), ("instanced", 2, False), ("probe", 0, False)]
-
-
 @pytest.mark.parametrize("family,seed,swap", FUZZ)
 def test_fuzz_scenes_occlusion_matches_port(family, seed, swap, tmp_path):
     path = str(tmp_path / "s.tsnap")
-    info = fuzzscene.make_mesh_scene(seed, path, family, swap_ties=swap, levels=30 if family == "caterpillar" else None)
-    if family == "caterpillar":
-        assert info["levels"] == 30
-    if family == "big":
-        assert max(info["tris"]) > 4096
+    queryscenes.fuzz_scene(family, seed, swap, path)
     snap = tb.Snapshot(path)
     port = rayoracle.RayOracle.from_snapshot(path)
     r = tb.Renderer(snap.scene)
     rng = np.random.RandomState(seed + 17)
-    sets = _ray_sets(snap.scene.contents, snap.camera, port, rng)
+    sets = queryscenes.ray_sets(snap.scene.contents, snap.camera, port, rng)
     sets["times"] = raysets.random_rays(snap.scene.contents, N, rng, (-0.5, 1.5))
     for what, rays in sets.items():
         _check(r, port, rays, rng, "%s/%d/%s" % (family, seed, what))
@@ -144,56 +126,25 @@ def test_fuzz_scenes_occlusion_matches_port(family, seed, swap, tmp_path):
 
 
 def test_mesh_with_device_built_bvh_occlusion_matches_port():
-    p, n, f = fuzzscene._icosphere(4, np.random.RandomState(3), bump=0.05)
-    mesh = fuzzscene.MeshData(p, n, f)
-    nodes = np.zeros((2 * len(mesh.idx) - 1) * 8, np.float32)
-    tb.bvh_build(mesh.pos, mesh.idx, nodes)
-    rng = np.random.RandomState(4)
-    prims = (abi.Primitive * 3)()
-    bounds = [fuzzscene._floor(prims[0], rng)]
-    prims[1].material = fuzzscene._material(rng, False)
-    bounds.append(fuzzscene._instance(prims[1], 0, mesh, (0.0, 1.0, 0.0), fuzzscene._quat(rng), 0.8, (0.2, 1.1, 0.0)))
-    bounds.append(fuzzscene._sphere(prims[2], (0.0, 3.0, 1.0), 0.3, fuzzscene._material(rng, True), 1))
-    scene, keep = fuzzscene.make_scene_struct(prims, fuzzscene._build_bvh(bounds), [mesh])
-    scene.meshes[0].nodes = nodes.ctypes.data_as(C.POINTER(abi.BvhNode))
-    scene.meshes[0].numNodes = 2 * len(mesh.idx) - 1
-    base = tb.Snapshot(tb.scene_path("cornell"))
-    cam = abi.copy_struct(base.camera)
-    cam.position[:] = [0.0, 1.2, 6.0]
-    cam.rotation[:] = [0.0, 0.0, 0.0, 1.0]
-    port = rayoracle.RayOracle(C.byref(scene), keepalive=(keep, nodes))
+    scene, keep, cam, rng = queryscenes.bvh_build_scene()
+    port = rayoracle.RayOracle(C.byref(scene), keepalive=keep)
     r = tb.Renderer(C.byref(scene))
-    for what, rays in _ray_sets(scene, cam, port, rng).items():
+    for what, rays in queryscenes.ray_sets(scene, cam, port, rng).items():
         _check(r, port, rays, rng, "bvh_build/" + what)
     assert _check_point_to_point(r, port, cam, rng, "bvh_build") > 0
     r.close()
     port.close()
-    base.close()
 
 
 @pytest.mark.parametrize("variant", ["no_flat", "cached", "group"])
 @pytest.mark.parametrize("name", ["cornell", "meshlight", "fuzz_instanced"])
 def test_occlusion_variants_give_the_same_answers(variant, name, tmp_path):
-    if name.startswith("fuzz_"):
-        path = str(tmp_path / "s.tsnap")
-        fuzzscene.make_mesh_scene(2, path, name[5:])
-    else:
-        path = tb.scene_path(name)
+    path = queryscenes.variant_path(name, tmp_path)
     snap = tb.Snapshot(path)
     port = rayoracle.RayOracle.from_snapshot(path)
     rng = np.random.RandomState(5)
-    rays = np.concatenate(list(_ray_sets(snap.scene.contents, snap.camera, port, rng).values()))
-    if variant == "no_flat":
-        with schedenv.knobs(**schedenv.ROUTES["no-flat"]):
-            r = tb.Renderer(snap.scene)
-    elif variant == "cached":
-        cache = str(tmp_path / "s.tcache")
-        tb.scene_cache_save(snap.scene, cache)
-        r = tb.Renderer(None, cache=cache)
-    else:
-        with schedenv.knobs(TEST_DUP_DEVICES="1"):
-            r = tb.Renderer(snap.scene, devices=[0, 0])
-        assert r.num_devices() == 2
+    rays = np.concatenate(list(queryscenes.ray_sets(snap.scene.contents, snap.camera, port, rng).values()))
+    r = queryscenes.variant_renderer(variant, snap, tmp_path)
     _check(r, port, rays, rng, "%s/%s" % (name, variant))
     _check_point_to_point(r, port, snap.camera, rng, "%s/%s" % (name, variant))
     r.close()

@@ -1,7 +1,7 @@
-"""The closest-hit query with the hit triangle, CPU side: the restatement's batch form (tests/trioracle.py, the arm
-tb200_trace_rays_tri is checked against) returns tb200_trace_rays' arm's hits and primitives bit for bit, and a triangle
-record that passes the checks that need no restatement (trioracle.check_semantics); and the ctypes mirror of
-tb200_tri_hit has the header's layout."""
+"""The closest-hit query with the hit triangle, CPU side: the restatement's batch form (RayOracle.trace_rays_tri in
+tests/rayoracle.py, the arm tb200_trace_rays_tri is checked against) returns tb200_trace_rays' arm's hits and
+primitives bit for bit, and a triangle record that passes the checks that need no restatement
+(trioracle.check_semantics); and the ctypes mirror of tb200_tri_hit has the header's layout."""
 import ctypes as C
 import os
 import re
@@ -25,20 +25,18 @@ def _check(path, rng, time=(0.0, 1.0)):
     snap = tb.Snapshot(path)
     scene = snap.scene.contents
     plain = rayoracle.RayOracle.from_snapshot(path)
-    tri_oracle = trioracle.TriOracle.from_snapshot(path)
     cam = raysets.camera_rays(snap.camera, N, rng)
     h, p = plain.trace_rays(cam)
     rays = np.concatenate([cam, raysets.random_rays(scene, N, rng, time), raysets.secondary_rays(cam, h, p, rng),
                            raysets.fallback_rays(scene, rng)])
     want_h, want_p = plain.trace_rays(rays)
-    hits, prims, tri, uvw = tri_oracle.trace_rays_tri(rays, nthreads=3)
+    hits, prims, tri, uvw = plain.trace_rays_tri(rays, nthreads=3)
     bad = raysets.mismatches(hits, prims, want_h, want_p)
     assert len(bad) == 0, "%d of %d rays differ from oracle_trace_rays, first %s" % (len(bad), len(rays), rays[bad[0]])
     counts = trioracle.check_semantics(scene, rays, hits, prims, tri, uvw, os.path.basename(path))
     types = {p.type for p in C.cast(scene.primitives, C.POINTER(abi.Primitive * scene.numPrimitives)).contents}
     assert counts[0] > 0 or abi.MESH not in types, "no mesh hit in a scene with meshes"
     assert counts[1] > 0 or not types & {abi.SPHERE, abi.PLANE}, "no sphere or plane hit in a scene with them"
-    tri_oracle.close()
     plain.close()
     snap.close()
     return counts

@@ -1,27 +1,23 @@
 """The closest-hit query with the hit triangle on the device (tb200_trace_rays_tri / Renderer.trace_rays_tri) against
-the CPU restatement (tests/trioracle.py), per ray and bit for bit: the primitive, the bits of t and of the normal, the
-triangle and the bits of u, v, w.  Its hits and primitives are also tb200_trace_rays' own, bit for bit, and its
-triangle records pass trioracle.check_semantics.  Every snapshot with camera, random, secondary and fallback rays;
-motion blur; every fuzzscene family; a mesh BVH from tb200_bvh_build; the upload and multi-device variants; ray
-counts; streams; side effects; and the refusals of bad arguments."""
+the CPU restatement (RayOracle.trace_rays_tri in tests/rayoracle.py), per ray and bit for bit: the primitive, the bits
+of t and of the normal, the triangle and the bits of u, v, w.  Its hits and primitives are also tb200_trace_rays'
+own, bit for bit, and its triangle records pass trioracle.check_semantics.  Every snapshot with camera, random,
+secondary and fallback rays; motion blur; every fuzzscene family; a mesh BVH from tb200_bvh_build; the upload and
+multi-device variants; ray counts; streams; side effects; and the refusals of bad arguments."""
 import ctypes as C
-import os
 import zlib
 
 import numpy as np
 import pytest
 
 import tinsel_b200 as tb
-from tinsel_b200 import abi
-import fuzzscene
+from queryscenes import FUZZ, N, SNAPSHOTS
+import queryscenes
+import rayoracle
 import raysets
-import schedenv
 import trioracle
 
 pytestmark = pytest.mark.gpu
-
-SNAPSHOTS = sorted(f[:-6] for f in os.listdir(tb.SCENE_DIR) if f.endswith(".tsnap"))
-N = 1 << 15
 
 
 def _torch():
@@ -54,21 +50,12 @@ def _check(r, oracle, scene, rays, what=""):
     return trioracle.check_semantics(scene, rays, hits, prims, tri, uvw, what)
 
 
-def _ray_sets(scene, camera, oracle, rng):
-    """test_ray_query_gpu's sets: camera rays through jittered raster positions, random rays in and around the scene,
-    secondary rays from the camera rays' hit points, and rays that reach the ordered fallback."""
-    cam = raysets.camera_rays(camera, N, rng)
-    h, p = oracle.trace_rays(cam)
-    return {"camera": cam, "random": raysets.random_rays(scene, N, rng), "secondary": raysets.secondary_rays(cam, h, p, rng),
-            "fallback": raysets.fallback_rays(scene, rng)}
-
-
 def test_snapshots_hit_meshes_and_other_primitives():
     """The snapshot test below must see both kinds of hit: it checks that records are set on one and cleared on the other."""
     seen = np.zeros(2, np.int64)
     for name in SNAPSHOTS:
         snap = tb.Snapshot(tb.scene_path(name))
-        oracle = trioracle.TriOracle.from_snapshot(tb.scene_path(name))
+        oracle = rayoracle.RayOracle.from_snapshot(tb.scene_path(name))
         r = tb.Renderer(snap.scene)
         seen += _check(r, oracle, snap.scene.contents, raysets.camera_rays(snap.camera, 4096, np.random.RandomState(2)), name)
         r.close()
@@ -80,11 +67,11 @@ def test_snapshots_hit_meshes_and_other_primitives():
 @pytest.mark.parametrize("name", SNAPSHOTS)
 def test_snapshot_rays_match_port(name):
     snap = tb.Snapshot(tb.scene_path(name))
-    oracle = trioracle.TriOracle.from_snapshot(tb.scene_path(name))
+    oracle = rayoracle.RayOracle.from_snapshot(tb.scene_path(name))
     r = tb.Renderer(snap.scene)
     scene = snap.scene.contents
     rng = np.random.RandomState(zlib.crc32(name.encode()) & 0xffff)
-    sets = _ray_sets(scene, snap.camera, oracle, rng)
+    sets = queryscenes.ray_sets(scene, snap.camera, oracle, rng)
     if name == "motionblur":   # times in and outside the shutter
         sets["motion"] = raysets.camera_rays(snap.camera, N, rng, time=rng.uniform(-0.5, 1.5, N))
         sets["motion_random"] = raysets.random_rays(scene, N, rng, (-0.5, 1.5))
@@ -95,24 +82,16 @@ def test_snapshot_rays_match_port(name):
     snap.close()
 
 
-FUZZ = [("ties", 0, False), ("ties", 0, True), ("ties", 3, True), ("many", 1, False), ("big", 0, False),
-        ("caterpillar", 0, False), ("instanced", 0, False), ("instanced", 1, False), ("instanced", 2, False), ("probe", 0, False)]
-
-
 @pytest.mark.parametrize("family,seed,swap", FUZZ)
 def test_fuzz_scenes_match_port(family, seed, swap, tmp_path):
     path = str(tmp_path / "s.tsnap")
-    info = fuzzscene.make_mesh_scene(seed, path, family, swap_ties=swap, levels=30 if family == "caterpillar" else None)
-    if family == "caterpillar":
-        assert info["levels"] == 30
-    if family == "big":
-        assert max(info["tris"]) > 4096
+    queryscenes.fuzz_scene(family, seed, swap, path)
     snap = tb.Snapshot(path)
-    oracle = trioracle.TriOracle.from_snapshot(path)
+    oracle = rayoracle.RayOracle.from_snapshot(path)
     r = tb.Renderer(snap.scene)
     scene = snap.scene.contents
     rng = np.random.RandomState(seed + 17)
-    sets = _ray_sets(scene, snap.camera, oracle, rng)
+    sets = queryscenes.ray_sets(scene, snap.camera, oracle, rng)
     sets["times"] = raysets.random_rays(scene, N, rng, (-0.5, 1.5))
     mesh_hits = 0
     for what, rays in sets.items():
@@ -124,57 +103,26 @@ def test_fuzz_scenes_match_port(family, seed, swap, tmp_path):
 
 
 def test_mesh_with_device_built_bvh_matches_port():
-    p, n, f = fuzzscene._icosphere(4, np.random.RandomState(3), bump=0.05)
-    mesh = fuzzscene.MeshData(p, n, f)
-    nodes = np.zeros((2 * len(mesh.idx) - 1) * 8, np.float32)
-    tb.bvh_build(mesh.pos, mesh.idx, nodes)
-    rng = np.random.RandomState(4)
-    prims = (abi.Primitive * 3)()
-    bounds = [fuzzscene._floor(prims[0], rng)]
-    prims[1].material = fuzzscene._material(rng, False)
-    bounds.append(fuzzscene._instance(prims[1], 0, mesh, (0.0, 1.0, 0.0), fuzzscene._quat(rng), 0.8, (0.2, 1.1, 0.0)))
-    bounds.append(fuzzscene._sphere(prims[2], (0.0, 3.0, 1.0), 0.3, fuzzscene._material(rng, True), 1))
-    scene, keep = fuzzscene.make_scene_struct(prims, fuzzscene._build_bvh(bounds), [mesh])
-    scene.meshes[0].nodes = nodes.ctypes.data_as(C.POINTER(abi.BvhNode))
-    scene.meshes[0].numNodes = 2 * len(mesh.idx) - 1
-    base = tb.Snapshot(tb.scene_path("cornell"))
-    cam = abi.copy_struct(base.camera)
-    cam.position[:] = [0.0, 1.2, 6.0]
-    cam.rotation[:] = [0.0, 0.0, 0.0, 1.0]
-    oracle = trioracle.TriOracle(C.byref(scene), keepalive=(keep, nodes))
+    scene, keep, cam, rng = queryscenes.bvh_build_scene()
+    oracle = rayoracle.RayOracle(C.byref(scene), keepalive=keep)
     r = tb.Renderer(C.byref(scene))
     mesh_hits = 0
-    for what, rays in _ray_sets(scene, cam, oracle, rng).items():
+    for what, rays in queryscenes.ray_sets(scene, cam, oracle, rng).items():
         mesh_hits += _check(r, oracle, scene, rays, "bvh_build/" + what)[0]
     assert mesh_hits > 0
     r.close()
     oracle.close()
-    base.close()
 
 
 @pytest.mark.parametrize("variant", ["no_flat", "cached", "group"])
 @pytest.mark.parametrize("name", ["cornell", "meshlight", "fuzz_instanced"])
 def test_variants_give_the_same_bits(variant, name, tmp_path):
-    if name.startswith("fuzz_"):
-        path = str(tmp_path / "s.tsnap")
-        fuzzscene.make_mesh_scene(2, path, name[5:])
-    else:
-        path = tb.scene_path(name)
+    path = queryscenes.variant_path(name, tmp_path)
     snap = tb.Snapshot(path)
-    oracle = trioracle.TriOracle.from_snapshot(path)
+    oracle = rayoracle.RayOracle.from_snapshot(path)
     rng = np.random.RandomState(5)
-    rays = np.concatenate(list(_ray_sets(snap.scene.contents, snap.camera, oracle, rng).values()))
-    if variant == "no_flat":
-        with schedenv.knobs(**schedenv.ROUTES["no-flat"]):
-            r = tb.Renderer(snap.scene)
-    elif variant == "cached":
-        cache = str(tmp_path / "s.tcache")
-        tb.scene_cache_save(snap.scene, cache)
-        r = tb.Renderer(None, cache=cache)
-    else:
-        with schedenv.knobs(TEST_DUP_DEVICES="1"):
-            r = tb.Renderer(snap.scene, devices=[0, 0])
-        assert r.num_devices() == 2
+    rays = np.concatenate(list(queryscenes.ray_sets(snap.scene.contents, snap.camera, oracle, rng).values()))
+    r = queryscenes.variant_renderer(variant, snap, tmp_path)
     _check(r, oracle, snap.scene.contents, rays, "%s/%s" % (name, variant))
     r.close()
     oracle.close()
@@ -184,7 +132,7 @@ def test_variants_give_the_same_bits(variant, name, tmp_path):
 @pytest.mark.parametrize("count", [1, 31, 33, 10 ** 6 + 7])
 def test_ray_counts(count):
     snap = tb.Snapshot(tb.scene_path("meshlight"))
-    oracle = trioracle.TriOracle.from_snapshot(tb.scene_path("meshlight"))
+    oracle = rayoracle.RayOracle.from_snapshot(tb.scene_path("meshlight"))
     r = tb.Renderer(snap.scene)
     rays = raysets.random_rays(snap.scene.contents, count, np.random.RandomState(count % 1000))
     _check(r, oracle, snap.scene.contents, rays, "count %d" % count)
@@ -196,7 +144,7 @@ def test_ray_counts(count):
 def test_rays_written_on_the_callers_stream():
     torch = _torch()
     snap = tb.Snapshot(tb.scene_path("meshlight"))
-    oracle = trioracle.TriOracle.from_snapshot(tb.scene_path("meshlight"))
+    oracle = rayoracle.RayOracle.from_snapshot(tb.scene_path("meshlight"))
     r = tb.Renderer(snap.scene)
     rays = raysets.random_rays(snap.scene.contents, N, np.random.RandomState(9))
     src = torch.from_numpy(rays).cuda()
@@ -222,7 +170,7 @@ def test_query_has_no_side_effects():
     snap = tb.Snapshot(tb.scene_path("meshlight"))
     cam, opt = snap.camera, snap.options
     opt.width, opt.height = 64, 48
-    oracle = trioracle.TriOracle.from_snapshot(tb.scene_path("meshlight"))
+    oracle = rayoracle.RayOracle.from_snapshot(tb.scene_path("meshlight"))
     scene = snap.scene.contents
     rays = raysets.random_rays(scene, 4096, np.random.RandomState(11))
     fresh = tb.Renderer(snap.scene)

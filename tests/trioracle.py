@@ -1,88 +1,10 @@
-"""TEST INFRASTRUCTURE: the CPU restatement's closest hit with the hit triangle over a whole batch of rays
-(tests/trace_rays_tri_oracle.cpp), the arm the device's tb200_trace_rays_tri is checked against.  Built like
-tests/rayoracle.py, with the same flags, into a temporary directory keyed by the sources' hash; the library also
-holds rayoracle's entry points, so TriOracle is a RayOracle over it."""
+"""TEST INFRASTRUCTURE: checks of tb200_trace_rays_tri's triangle records that need no restatement (the restatement's
+own records come from rayoracle.RayOracle.trace_rays_tri)."""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from tinsel_b200 import abi
-import rayoracle
-
-ROOT = rayoracle.ROOT
-SOURCES = [os.path.join(ROOT, "tests", "trace_rays_tri_oracle.cpp"), os.path.join(ROOT, "tinsel_b200", "csrc", "snapshot.cpp")]
-DEPS = SOURCES + rayoracle.DEPS
-
-_lib = None
-
-
-def library_path():
-    h = hashlib.sha1(" ".join([rayoracle.CXX] + rayoracle.FLAGS).encode())
-    for p in DEPS:
-        with open(p, "rb") as f:
-            h.update(f.read())
-    return os.path.join(tempfile.gettempdir(), "tinsel_b200_trioracle_%s.so" % h.hexdigest()[:16])
-
-
-def load():
-    global _lib
-    if _lib is not None:
-        return _lib
-    path = library_path()
-    if not os.path.exists(path):
-        tmp = "%s.%d.tmp" % (path, os.getpid())
-        subprocess.check_call([rayoracle.CXX, *rayoracle.FLAGS, "-I", ROOT, "-I", os.path.join(ROOT, "include"), "-o", tmp,
-                               *SOURCES])
-        os.replace(tmp, path)
-    lib = C.CDLL(path)
-    lib.oracle_create.restype = C.c_void_p
-    lib.oracle_create.argtypes = [C.POINTER(abi.Scene)]
-    lib.oracle_destroy.argtypes = [C.c_void_p]
-    lib.oracle_trace_rays.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_longlong, C.POINTER(C.c_float),
-                                      C.POINTER(C.c_int32), C.c_int]
-    lib.oracle_trace_rays_tri.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_longlong, C.POINTER(C.c_float),
-                                          C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]
-    abi.declare_snapshot_api(lib)
-    _lib = lib
-    return lib
-
-
-class TriOracle(rayoracle.RayOracle):
-    """RayOracle over this library, plus trace_rays_tri(rays (N, 8) float32) -> (hits (N, 4), prims (N,), tri (N,),
-    uvw (N, 3) float32), the shapes and meaning of Renderer.trace_rays_tri."""
-
-    def __init__(self, scene_ptr, keepalive=None):
-        self.lib = load()
-        h = self.lib.oracle_create(scene_ptr)
-        if not h:
-            raise RuntimeError("the CPU restatement refused the scene: a BVH is not a tree or is too deep for its stack")
-        self.h = C.c_void_p(h)
-        self._keep = keepalive
-        self._snap = None
-
-    @classmethod
-    def from_snapshot(cls, path):
-        lib = load()
-        snap = lib.tb200_snapshot_load(path.encode())
-        if not snap:
-            raise RuntimeError("cannot load " + path)
-        o = cls(lib.tb200_snapshot_scene(snap))
-        o._snap = snap
-        return o
-
-    def trace_rays_tri(self, rays, nthreads=None):
-        rays = np.ascontiguousarray(rays, np.float32).reshape(-1, 8)
-        hits = np.zeros((len(rays), 4), np.float32)
-        prims = np.zeros(len(rays), np.int32)
-        tris = np.zeros((len(rays), 4), np.int32)
-        self.lib.oracle_trace_rays_tri(self.h, rays.ctypes.data_as(C.POINTER(C.c_float)), len(rays),
-                                       hits.ctypes.data_as(C.POINTER(C.c_float)), prims.ctypes.data_as(C.POINTER(C.c_int32)),
-                                       tris.ctypes.data_as(C.POINTER(C.c_int32)), nthreads or os.cpu_count() or 1)
-        return hits, prims, tris[:, 0], tris[:, 1:].view(np.float32)
 
 
 def _rotate(q, v):

@@ -329,6 +329,23 @@ class Renderer:
         if not self._external_stream:
             torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()
 
+    def _query(self, entry, rays, outputs):
+        """What the ray queries share: checks `rays` (N rays) and each output (tensor or None, name, shape after N,
+        dtype), allocating on the head device those not given; when N > 0, waits for torch and calls the library's
+        `entry` on the rays and the outputs, raising on a refusal.  Returns the output tensors."""
+        import torch
+        n = self._check_rays(rays)
+        out = []
+        for x, name, shape, dtype in outputs:
+            if x is None:
+                x = torch.empty((n,) + shape, dtype=dtype, device=torch.device("cuda", self.device))
+            self._check_tensor(x, name, (n,) + shape, dtype)
+            out.append(x)
+        if n > 0:
+            self._wait_for_torch()
+            self._check(getattr(self.lib, entry)(self.h, rays.data_ptr(), *[x.data_ptr() for x in out], n), entry)
+        return out
+
     def trace_rays(self, rays, hits=None, prims=None):
         """Closest hit of every ray (tb200_trace_rays): Trace (src/render.cpp:17-62) bit for bit.
         rays: contiguous float32 CUDA tensor (N, 8) on the head device -- origin.xyz, time, dir.xyz, pad.
@@ -336,18 +353,7 @@ class Renderer:
         `hits` / `prims` when given.  On the renderer's private stream the call first waits for torch's current
         stream, so that tensors written there are complete; after set_stream the work is ordered on that stream."""
         import torch
-        n = self._check_rays(rays)
-        dev = torch.device("cuda", self.device)
-        if hits is None:
-            hits = torch.empty((n, 4), dtype=torch.float32, device=dev)
-        if prims is None:
-            prims = torch.empty((n,), dtype=torch.int32, device=dev)
-        self._check_tensor(hits, "hits", (n, 4), torch.float32)
-        self._check_tensor(prims, "prims", (n,), torch.int32)
-        if n == 0:
-            return hits, prims
-        self._wait_for_torch()
-        self._check(self.lib.tb200_trace_rays(self.h, rays.data_ptr(), hits.data_ptr(), prims.data_ptr(), n), "tb200_trace_rays")
+        hits, prims = self._query("tb200_trace_rays", rays, [(hits, "hits", (4,), torch.float32), (prims, "prims", (), torch.int32)])
         return hits, prims
 
     def trace_rays_tri(self, rays, hits=None, prims=None, tris=None):
@@ -357,21 +363,9 @@ class Renderer:
         own space; tri = -1 and uvw = 0 for a sphere hit, a plane hit or a miss.  Both are views of one (N, 4) int32
         tensor, the tb200_tri_hit records, which `tris` gives when it is passed.  Stream behaviour as for trace_rays."""
         import torch
-        n = self._check_rays(rays)
-        dev = torch.device("cuda", self.device)
-        if hits is None:
-            hits = torch.empty((n, 4), dtype=torch.float32, device=dev)
-        if prims is None:
-            prims = torch.empty((n,), dtype=torch.int32, device=dev)
-        if tris is None:
-            tris = torch.empty((n, 4), dtype=torch.int32, device=dev)
-        self._check_tensor(hits, "hits", (n, 4), torch.float32)
-        self._check_tensor(prims, "prims", (n,), torch.int32)
-        self._check_tensor(tris, "tris", (n, 4), torch.int32)
-        if n > 0:
-            self._wait_for_torch()
-            self._check(self.lib.tb200_trace_rays_tri(self.h, rays.data_ptr(), hits.data_ptr(), prims.data_ptr(),
-                                                      tris.data_ptr(), n), "tb200_trace_rays_tri")
+        hits, prims, tris = self._query("tb200_trace_rays_tri", rays, [(hits, "hits", (4,), torch.float32),
+                                                                        (prims, "prims", (), torch.int32),
+                                                                        (tris, "tris", (4,), torch.int32)])
         return hits, prims, tris[:, 0], tris[:, 1:].view(torch.float32)
 
     def occluded(self, rays, out=None):
@@ -380,14 +374,7 @@ class Renderer:
         dir = target - origin, tmax = 1 asks about the segment between two points).  Returns a (N,) torch.bool
         tensor, `out` when given.  Stream behaviour as for trace_rays."""
         import torch
-        n = self._check_rays(rays)
-        if out is None:
-            out = torch.empty((n,), dtype=torch.bool, device=torch.device("cuda", self.device))
-        self._check_tensor(out, "out", (n,), torch.bool)
-        if n == 0:
-            return out
-        self._wait_for_torch()
-        self._check(self.lib.tb200_occluded_rays(self.h, rays.data_ptr(), out.data_ptr(), n), "tb200_occluded_rays")
+        out, = self._query("tb200_occluded_rays", rays, [(out, "out", (), torch.bool)])
         return out
 
     def set_frame(self, frame):

@@ -1831,103 +1831,77 @@ static bool check_device_span(const char* entry, const tb200_renderer* r, const 
     return true;
 }
 
-// The checks of a query's renderer and ray count: 0 when there are rays to trace (the renderer's device is then
-// current), 1 when there are none, -1 (error set) when either is refused
-static int query_begin(const char* entry, tb200_renderer* r, int64_t numRays)
-{
-    if (!r) {
-        set_error(std::string(entry) + ": null renderer");
-        return -1;
-    }
-    if (numRays < 0 || numRays > (int64_t)(SIZE_MAX / sizeof(tb200_ray))) {
-        set_error(std::string(entry) + ": numRays " + std::to_string((long long)numRays) + " is out of range");
-        return -1;
-    }
-    if (numRays == 0) return 1;
-    cudaSetDevice(r->device);   // a multi-device renderer answers on its head, which holds a full copy of the scene
-    return 0;
-}
+// One output of a ray query, as the caller passed it: checked by check_device_span for numRays records
+struct QuerySpan {
+    const void* ptr;
+    size_t bytesPerRay;
+    size_t align;
+    const char* what;   // its name in refusals
+};
 
-// Runs launch(&launches) -- one query kernel -- on r's stream, waits for it and sets stats.gpuMs to its time
-static int query_run(const char* entry, tb200_renderer* r, const std::function<void(unsigned long long*)>& launch)
+// Every ray query: checks the renderer, the ray count, the rays and then the outputs in the order given (the first
+// refusal sets the error), makes the renderer's device current, runs the query's kernel on r's stream with Q's
+// outputs, waits for it and sets stats.gpuMs to its time.  No rays: returns 0 before the pointers are checked.
+static int run_query(const char* entry, tb200_renderer* r, QueryKind kind, const tb200_ray* rays, int64_t numRays,
+                     std::initializer_list<QuerySpan> outputs, QueryParams Q)
 {
-    unsigned long long launches = 0;
-    if (cudaEventRecord(r->evStart, r->stream) != cudaSuccess) {
-        set_error(std::string(entry) + ": " + cudaGetErrorString(cudaGetLastError()));
+    auto fail = [&](const std::string& why) {
+        set_error(std::string(entry) + ": " + why);
         return -1;
-    }
-    launch(&launches);
+    };
+    if (!r) return fail("null renderer");
+    if (numRays < 0 || numRays > (int64_t)(SIZE_MAX / sizeof(tb200_ray)))
+        return fail("numRays " + std::to_string((long long)numRays) + " is out of range");
+    if (numRays == 0) return 0;
+    cudaSetDevice(r->device);   // a multi-device renderer answers on its head, which holds a full copy of the scene
+    const size_t n = (size_t)numRays;
+    if (!check_device_span(entry, r, rays, n * sizeof(tb200_ray), 16, "rays")) return -1;
+    for (const QuerySpan& s : outputs)
+        if (!check_device_span(entry, r, s.ptr, n * s.bytesPerRay, s.align, s.what)) return -1;
+    Q.scene = r->scene;
+    Q.rays = reinterpret_cast<const float4*>(rays);
+    Q.numRays = numRays;
+    Q.counter = r->mem.counter.get();   // the wavefront's work counter: free between launches on this stream
+
+    unsigned long long launches = 0;
+    if (cudaEventRecord(r->evStart, r->stream) != cudaSuccess) return fail(cudaGetErrorString(cudaGetLastError()));
+    launch_query(kind, Q, r->numSMs, r->stream, &launches);
     r->stats.kernelLaunches += launches;
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaEventRecord(r->evStop, r->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
-    if (e != cudaSuccess) {
-        set_error(std::string(entry) + ": " + cudaGetErrorString(e));
-        return -1;
-    }
+    if (e != cudaSuccess) return fail(cudaGetErrorString(e));
     return sync_gpu_ms(r) ? 0 : -1;
 }
 
+static_assert(sizeof(tb200_ray) == 32 && sizeof(tb200_hit) == 16, "the query kernels read two float4 per ray and write one hit");
+static_assert(sizeof(tb200_tri_hit) == 16, "the query kernel writes one int4 per triangle record");
+
 int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, int64_t numRays)
 {
-    const char* entry = "tb200_trace_rays";
-    const int begin = query_begin(entry, r, numRays);
-    if (begin != 0) return begin < 0 ? -1 : 0;
-    const size_t n = (size_t)numRays;
-    if (!check_device_span(entry, r, rays, n * sizeof(tb200_ray), 16, "rays") ||
-        !check_device_span(entry, r, hits, n * sizeof(tb200_hit), 16, "hits") ||
-        !check_device_span(entry, r, prims, n * sizeof(int32_t), 4, "prims"))
-        return -1;
-    static_assert(sizeof(tb200_ray) == 32 && sizeof(tb200_hit) == 16, "the query kernel reads two float4 per ray and writes one");
-    QueryParams Q;
-    Q.scene = r->scene;
-    Q.rays = reinterpret_cast<const float4*>(rays);
+    QueryParams Q = {};
     Q.hits = reinterpret_cast<float4*>(hits);
     Q.prims = prims;
-    Q.numRays = numRays;
-    Q.counter = r->mem.counter.get();   // the wavefront's work counter: free between launches on this stream
-    return query_run(entry, r, [&](unsigned long long* launches) { launch_trace_rays(Q, r->numSMs, r->stream, launches); });
+    return run_query("tb200_trace_rays", r, QueryKind::Closest, rays, numRays,
+                     {{hits, sizeof(tb200_hit), 16, "hits"}, {prims, sizeof(int32_t), 4, "prims"}}, Q);
 }
 
 int tb200_occluded_rays(tb200_renderer* r, const tb200_ray* rays, uint8_t* occluded, int64_t numRays)
 {
-    const char* entry = "tb200_occluded_rays";
-    const int begin = query_begin(entry, r, numRays);
-    if (begin != 0) return begin < 0 ? -1 : 0;
-    const size_t n = (size_t)numRays;
-    if (!check_device_span(entry, r, rays, n * sizeof(tb200_ray), 16, "rays") ||
-        !check_device_span(entry, r, occluded, n, 1, "occluded"))
-        return -1;
-    OcclusionParams Q;
-    Q.scene = r->scene;
-    Q.rays = reinterpret_cast<const float4*>(rays);
+    QueryParams Q = {};
     Q.occluded = occluded;
-    Q.numRays = numRays;
-    Q.counter = r->mem.counter.get();
-    return query_run(entry, r, [&](unsigned long long* launches) { launch_occluded_rays(Q, r->numSMs, r->stream, launches); });
+    return run_query("tb200_occluded_rays", r, QueryKind::Occluded, rays, numRays, {{occluded, 1, 1, "occluded"}}, Q);
 }
 
 int tb200_trace_rays_tri(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, tb200_tri_hit* tris, int64_t numRays)
 {
-    const char* entry = "tb200_trace_rays_tri";
-    const int begin = query_begin(entry, r, numRays);
-    if (begin != 0) return begin < 0 ? -1 : 0;
-    const size_t n = (size_t)numRays;
-    if (!check_device_span(entry, r, rays, n * sizeof(tb200_ray), 16, "rays") ||
-        !check_device_span(entry, r, hits, n * sizeof(tb200_hit), 16, "hits") ||
-        !check_device_span(entry, r, prims, n * sizeof(int32_t), 4, "prims") ||
-        !check_device_span(entry, r, tris, n * sizeof(tb200_tri_hit), 16, "tris"))
-        return -1;
-    static_assert(sizeof(tb200_tri_hit) == 16, "the query kernel writes one int4 per triangle record");
-    TriQueryParams Q;
-    Q.scene = r->scene;
-    Q.rays = reinterpret_cast<const float4*>(rays);
+    QueryParams Q = {};
     Q.hits = reinterpret_cast<float4*>(hits);
     Q.prims = prims;
     Q.tris = reinterpret_cast<int4*>(tris);
-    Q.numRays = numRays;
-    Q.counter = r->mem.counter.get();
-    return query_run(entry, r, [&](unsigned long long* launches) { launch_trace_rays_tri(Q, r->numSMs, r->stream, launches); });
+    return run_query("tb200_trace_rays_tri", r, QueryKind::ClosestTri, rays, numRays,
+                     {{hits, sizeof(tb200_hit), 16, "hits"}, {prims, sizeof(int32_t), 4, "prims"},
+                      {tris, sizeof(tb200_tri_hit), 16, "tris"}}, Q);
 }
 
 #ifdef TB_WF2_STAGE_CLOCKS

@@ -128,36 +128,22 @@ struct NlmParams {
 };
 void launch_nlm(const NlmParams& p, cudaStream_t stream, unsigned long long* launchCount);
 
-// Batched closest-hit query (tb200_trace_rays, tb_query.cuh): Trace (render.cpp:17-62) of every ray.
+// The batched ray queries (tb_query.cuh), each Trace (render.cpp:17-62) of every ray of a caller's batch:
+enum class QueryKind {
+    Closest,      // tb200_trace_rays: the closest hit
+    ClosestTri,   // tb200_trace_rays_tri: the closest hit and the winner's triangle and barycentric weights
+    Occluded,     // tb200_occluded_rays: whether Trace hits something before the ray's tmax
+};
+// Every query's parameters.  The output pointers a query does not write stay null.
 struct QueryParams {
     DScene scene;
-    const float4* rays;   // 2 per ray: origin.xyz, time; dir.xyz, pad
-    float4* hits;         // 1 per ray: t, normal.xyz
-    int* prims;           // 1 per ray: closest primitive, -1 on a miss
+    const float4* rays;   // 2 per ray: origin.xyz, time; dir.xyz, pad (Occluded: tmax)
+    float4* hits;         // Closest, ClosestTri: 1 per ray: t, normal.xyz
+    int* prims;           // Closest, ClosestTri: 1 per ray: closest primitive, -1 on a miss
+    int4* tris;           // ClosestTri: 1 per ray: triangle, then the bits of u, v, w; -1, 0, 0, 0 unless a mesh was hit
+    unsigned char* occluded;   // Occluded: 1 per ray: 1 when occluded, else 0
     long long numRays;
     unsigned long long* counter;   // work counter, cleared by the launch
 };
-const char* launch_trace_rays(const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
-
-// Batched occlusion query (tb200_occluded_rays, tb_query.cuh): whether Trace of every ray hits something before its tmax.
-struct OcclusionParams {
-    DScene scene;
-    const float4* rays;   // 2 per ray: origin.xyz, time; dir.xyz, tmax
-    unsigned char* occluded;   // 1 per ray: 1 when occluded, else 0
-    long long numRays;
-    unsigned long long* counter;   // work counter, cleared by the launch
-};
-const char* launch_occluded_rays(const OcclusionParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
-
-// Batched closest-hit query that also reports the triangle (tb200_trace_rays_tri, tb_query.cuh): tb200_trace_rays'
-// outputs plus the winner's triangle and barycentric weights.  Its own struct, so that k_trace_rays keeps its code.
-struct TriQueryParams {
-    DScene scene;
-    const float4* rays;   // 2 per ray: origin.xyz, time; dir.xyz, pad
-    float4* hits;         // 1 per ray: t, normal.xyz
-    int* prims;           // 1 per ray: closest primitive, -1 on a miss
-    int4* tris;           // 1 per ray: triangle, then the bits of u, v, w; -1, 0, 0, 0 unless a mesh was hit
-    long long numRays;
-    unsigned long long* counter;   // work counter, cleared by the launch
-};
-const char* launch_trace_rays_tri(const TriQueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
+// Unlike the launches above, it leaves tb200_last_kernel alone and so returns no kernel name.
+void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);

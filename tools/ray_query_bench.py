@@ -11,8 +11,7 @@ name, power limit and maximum SM clock, read in the same run.
 
 Closest hit with the hit triangle (key "tri"), on the same camera and random batches: the same rates (68 bytes per
 ray: 32 in, 16 + 4 + 16 out), the kernel time against trace_rays' on the same rays, the fraction of rays that hit a
-mesh, and a bit-exact check of 2^16 rays (hits, primitives, triangles and weights) against the restatement
-(tests/trioracle.py).
+mesh, and a bit-exact check of 2^16 rays (hits, primitives, triangles and weights) against the restatement.
 
 Occlusion (key "occluded"), on the same batches: the camera rays with tmax = +inf, the random rays with tmax uniform
 in [0, the scene's diagonal), and point-to-point segments built on the device from the camera rays' hit points to
@@ -37,7 +36,6 @@ import tinsel_b200 as tb  # noqa: E402
 import occlusionsets  # noqa: E402
 import rayoracle  # noqa: E402
 import raysets  # noqa: E402
-import trioracle  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
 BYTES_PER_RAY = 32 + 16 + 4
@@ -180,7 +178,6 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("ray_query_bench: no CUDA device (the rates are GPU measurements)")
     rayoracle.load()
-    trioracle.load()
     gpu, power, clock = gpu_info()
     n = 1 << args.log2_rays
     side = 1 << (args.log2_rays // 2)
@@ -192,7 +189,6 @@ def main():
         scene = snap.scene.contents
         r = tb.Renderer(snap.scene)
         port = rayoracle.RayOracle.from_snapshot(path)
-        tri_port = trioracle.TriOracle.from_snapshot(path)
         line = {"scene": name, "rays": n, "gpu": gpu, "power_limit": power, "max_sm_clock": clock,
                 "library": os.path.basename(os.environ.get("TINSEL_B200_LIB", tb.LIB_PATH))}
         hits = torch.empty((n, 4), device="cuda")
@@ -217,7 +213,7 @@ def main():
             line[kind]["bit_exact_2^16"] = len(raysets.mismatches(got_h, got_p, want_h[:k], want_p[:k])) == 0
             line[kind]["hit_fraction"] = round(float((prims >= 0).float().mean()), 4)
             # the query with the hit triangle on the same rays (it writes the same hits and prims)
-            line["tri"][kind] = tri_arm(torch, r, tri_port, rays, hits, prims, tris, kms, args)
+            line["tri"][kind] = tri_arm(torch, r, port, rays, hits, prims, tris, kms, args)
             # the occlusion query on the same rays
             if kind == "camera":
                 rays[:, 7] = float("inf")
@@ -236,7 +232,6 @@ def main():
         print(json.dumps(line), flush=True)
         r.close()
         port.close()
-        tri_port.close()
         snap.close()
 
 
