@@ -101,7 +101,7 @@ const char* launch_wavefront2(const LaunchParams& p, const Wf2Route& route, int 
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds: the per-stage cycle counters of the lane-owned wavefront layout (wf2_lanes.cuh), summed
 // over every launch since the last reset
-#define TB_WF2_STAGE_CLOCK_WORDS 18
+#define TB_WF2_STAGE_CLOCK_WORDS 23
 void read_stage_clocks(unsigned long long* out, bool reset);
 #endif
 // eNormals mode (render.cpp:494-515)

@@ -419,8 +419,10 @@ static __device__ __noinline__ MeshHit ray_mesh(const DMesh& m, const unsigned c
 // the reference pops them; a reference without TB_LEAF ends the list.  The reference pops the root, pushes each
 // child whose box passes `tChild < tmax` (tmax is still FLT_MAX), the nearer one last when both do, then pops and
 // tests the triangles in turn; no box test follows, so the truncation of the ray changes nothing and the walk needs
-// no stack.  Returns false for any other tree.
-TB_DEV bool small_mesh_leaves(const DMesh& m, const V3& origin, const V3& dir, uint32_t& first, uint32_t& second)
+// no stack.  Returns false for any other tree.  haveRcp: rcp is ray_rcp(dir), which the caller already has (passed by
+// value, not through a pointer that may be null: that would keep the caller's copy in local memory).
+TB_DEV bool small_mesh_leaves(const DMesh& m, const V3& origin, const V3& dir, uint32_t& first, uint32_t& second, bool haveRcp = false,
+                              const V3& rcp = V3{})
 {
     first = m.rootRef;
     second = 0u;
@@ -429,10 +431,10 @@ TB_DEV bool small_mesh_leaves(const DMesh& m, const V3& origin, const V3& dir, u
     const uint2 kids = *reinterpret_cast<const uint2*>(&pr->left);
     if (!(kids.x & kids.y & TB_LEAF)) return false;
     const float4 a = pr->a, b = pr->b, c = pr->c;
-    const V3 rcp = ray_rcp(dir);
+    const V3 r = haveRcp ? rcp : ray_rcp(dir);
     float tLeft, tRight;
-    const bool hitLeft = ray_aabb(origin, rcp, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < FLT_MAX;
-    const bool hitRight = ray_aabb(origin, rcp, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < FLT_MAX;
+    const bool hitLeft = ray_aabb(origin, r, a.x, a.y, a.z, a.w, b.x, b.y, tLeft) && tLeft < FLT_MAX;
+    const bool hitRight = ray_aabb(origin, r, b.z, b.w, c.x, c.y, c.z, c.w, tRight) && tRight < FLT_MAX;
     const bool both = hitLeft && hitRight;
     const bool swap = both && (tLeft < tRight);   // left pushed last: it pops first
     first = hitRight ? (swap ? kids.x : kids.y) : (hitLeft ? kids.x : 0u);
@@ -441,11 +443,11 @@ TB_DEV bool small_mesh_leaves(const DMesh& m, const V3& origin, const V3& dir, u
 }
 
 // ray_mesh() for small_mesh_leaves()' trees, inline and without the stack.  Returns false, having done nothing, for
-// any other tree.
-TB_DEV bool ray_mesh_small(const DMesh& m, V3 origin, V3 dir, MeshHit& out)
+// any other tree.  haveRcp, rcp: as for small_mesh_leaves().
+TB_DEV bool ray_mesh_small(const DMesh& m, V3 origin, V3 dir, MeshHit& out, bool haveRcp = false, const V3& rcp = V3{})
 {
     uint32_t first, second;
-    if (!small_mesh_leaves(m, origin, dir, first, second)) return false;
+    if (!small_mesh_leaves(m, origin, dir, first, second, haveRcp, rcp)) return false;
     float closestT = FLT_MAX;
     out.tri = -1;
     out.u = out.v = out.w = 0.0f;
@@ -492,8 +494,11 @@ struct HitRec : Hit {
 template <bool REC>
 using TraceHit = typename std::conditional<REC, HitRec, Hit>::type;
 
+// rcp: ray_rcp(d) where the caller already has it (a pointer known when the call is compiled: null or the caller's).  A mesh walk that starts with the bits of d (a primitive without
+// rotation or scale: rotate_xf and inverse_scale leave d as d + 0, which differs only where a -0 becomes +0) reuses
+// it: ray_rcp is a function of the direction's bits alone.
 template <uint32_t FEAT = TB_FEAT_ALL>
-TB_DEV bool prim_test(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, PrimHit& ph)
+TB_DEV bool prim_test(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, PrimHit& ph, const V3* rcp = nullptr)
 {
     if (p.type == TB200_PLANE) {
         // IntersectRayPlane, intersection.h:85-99; Dot(Vec4,Vec4) adds plane.w*0 resp. plane.w*1
@@ -527,7 +532,9 @@ TB_DEV bool prim_test(const DScene& sc, const DPrim& p, V3 o, V3 d, float time, 
     const V3 ld = inverse_transform_vector(xf, d);
     const DMesh& m = sc.meshes[p.mesh];
     MeshHit mh;
-    if (!ray_mesh_small(m, lo, ld, mh)) {
+    const bool sameDir = rcp && tb_float_bits(ld.x) == tb_float_bits(d.x) && tb_float_bits(ld.y) == tb_float_bits(d.y) &&
+                         tb_float_bits(ld.z) == tb_float_bits(d.z);
+    if (!ray_mesh_small(m, lo, ld, mh, sameDir, rcp ? *rcp : ld)) {
         const bool staged = p.mesh == sc.treeletMesh && sc.treelet != nullptr;
         mh = ray_mesh(m, sc.treelet, staged ? (uint32_t)sc.treeletPairs : 0u, lo, ld);
     }
@@ -644,7 +651,9 @@ TB_DEV bool flat_guard(const V3& o, const V3& d)
 
 // `flat` is sc.flat, or the same program where the caller can name it in shared memory (the lane-owned wavefront
 // kernel: Wf2Shared::flat), so that the op loads compile to shared-memory loads instead of generic ones.
-template <uint32_t FEAT = TB_FEAT_ALL, bool REC = false>
+// SHARE_RCP: small meshes whose walk starts with the ray's own direction reuse the ray's reciprocals (prim_test).
+// A template switch, so that the callers without it -- all but the lane-owned kernel -- keep their code.
+template <uint32_t FEAT = TB_FEAT_ALL, bool REC = false, bool SHARE_RCP = false>
 TB_DEV TraceHit<REC> trace_closest(const DScene& sc, const ProgOp* flat, V3 o, V3 d, float time, bool wantNormal)
 {
     const int n = sc.numFlat;
@@ -687,7 +696,7 @@ TB_DEV TraceHit<REC> trace_closest(const DScene& sc, const ProgOp* flat, V3 o, V
                 }
             }
             PrimHit* ph = &rec[ri ^ 1];
-            if (!prim_test<FEAT>(sc, sc.prims[kindPrim >> 8], o, d, time, *ph)) continue;
+            if (!prim_test<FEAT>(sc, sc.prims[kindPrim >> 8], o, d, time, *ph, SHARE_RCP ? &rcp : nullptr)) continue;
             t = ph->t;
             if (t > 0.0f && t < minT) ri ^= 1;   // the record just written becomes the best one
         }

@@ -172,6 +172,108 @@ TB_NOINLINE BsdfValue bsdf_eval_pdf(const DMaterial& mat, float etaI, float etaO
     return r;
 }
 
+// The terms of BSDFEval that depend on the view alone: the same for every light direction of one surface point, so a
+// bounce computes them once for its NEE connections and its BSDF sample (bsdf_view) instead of once per call.
+struct BsdfView {
+    float NDotV;
+    float FV;    // schlick_fresnel(NDotV)
+    float GsV;   // smith_ggx(NDotV, mat.alpha)
+    float GrV;   // smith_ggx(NDotV, .25f): the clearcoat lobe's, only where that lobe is compiled in
+};
+
+template <uint32_t FEAT = TB_FEAT_ALL>
+TB_DEV BsdfView bsdf_view(const DMaterial& mat, V3 N, V3 V)
+{
+    BsdfView w;
+    w.NDotV = dot(N, V);
+    w.FV = schlick_fresnel(w.NDotV);
+    w.GsV = smith_ggx(w.NDotV, mat.alpha);
+    w.GrV = ((FEAT & TB_FEAT_CLEARCOAT) && !(mat.flags & TB_MAT_NO_CLEARCOAT)) ? smith_ggx(w.NDotV, .25f) : 0.0f;
+    return w;
+}
+
+// bsdf_eval_pdf() given bsdf_view(mat, N, V), bit for bit: the same expressions as bsdf_pdf() and bsdf_eval(), with
+// what the two share computed once.  Both take the half vector of L + V: bsdf_pdf's safe_normalize and bsdf_eval's
+// normalize are the same a * (1 / sqrtf(m)) when m = |L + V|^2 > 0, and dot() is commutative bit for bit, so NDotH,
+// LDotH and GTR2 are each evaluated once (GTR2 reads its argument only as NDotH * NDotH, so |NDotH| gives the same).
+// For !(m > 0) bsdf_pdf keeps its zero fallback and bsdf_eval keeps normalize's inf / NaN.  Both branch on
+// dot(L, N) <= 0 first, also the same bits.
+template <uint32_t FEAT = TB_FEAT_ALL>
+TB_NOINLINE BsdfValue bsdf_eval_pdf(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3 L, BsdfView view)
+{
+    BsdfValue r;
+    const float NDotL = dot(N, L);
+    const float NDotV = view.NDotV;
+    const float a = mat.alpha;
+    V3 bsdf = v3s(0.0f);
+    V3 brdf = v3s(0.0f);
+    if (NDotL <= 0.0f) {
+        // bsdf_pdf's early return
+        r.pdf = tb_lerp(TB_INV_2PI * mat.subsurface * 0.5f, 0.0f, mat.transmission);
+        if ((FEAT & TB_FEAT_TRANSMISSION) && mat.transmission > 0.0f) {
+            const float F = fresnel_dielectric(NDotV, etaI, etaO);
+            bsdf = v3s(mat.transmission * (1.0f - F) / tb_abs(NDotL) * (1.0f - mat.metallic));
+        }
+        if ((FEAT & TB_FEAT_SUBSURFACE) && (!(FEAT & TB_FEAT_TRANSMISSION) || mat.transmission < 1.0f) && mat.subsurface > 0.0f) {
+            const float FL = schlick_fresnel(tb_abs(NDotL));
+            const float Fd = (1.0f - 0.5f * FL) * (1.0f - 0.5f * view.FV);
+            brdf = TB_INV_PI * mat.sqrtColor * mat.subsurface * Fd * (1.0f - mat.metallic);
+        }
+        r.f = tb_lerp(brdf, bsdf, mat.transmission);
+        return r;
+    }
+    const V3 LV = L + V;
+    const float m = length_sq(LV);
+    const V3 H = LV * (1.0f / sqrtf(m));   // normalize(L + V)
+    const float NDotH = dot(N, H);
+    const float LDotH = dot(L, H);
+    const float Ds = gtr2(NDotH, a);
+
+    // bsdf_pdf
+    float cosThetaHalf = tb_abs(NDotH), Dh = Ds, LDotHalf = LDotH;
+    if (!(m > 0.0f)) {
+        const V3 half = v3s(0.0f);   // safe_normalize's fallback
+        cosThetaHalf = tb_abs(dot(half, N));
+        Dh = gtr2(cosThetaHalf, a);
+        LDotHalf = dot(L, half);
+    }
+    const float pdfHalf = Dh * cosThetaHalf;
+    const float pdfSpec = 0.25f * pdfHalf / tb_max(1.e-6f, LDotHalf);
+    const float pdfDiff = tb_abs(NDotL) * TB_INV_PI * (1.0f - mat.subsurface);
+    const float brdfPdf = tb_lerp(pdfDiff, pdfSpec, 0.5f);
+    if ((!(FEAT & TB_FEAT_TRANSMISSION) || (mat.flags & TB_MAT_NO_FRESNEL)) && NDotV > 0.0f) {
+        r.pdf = brdfPdf;
+    } else {
+        const float F = fresnel_dielectric(NDotV, etaI, etaO);
+        r.pdf = tb_lerp(brdfPdf, pdfSpec * F, mat.transmission);
+    }
+
+    // bsdf_eval
+    if ((FEAT & TB_FEAT_TRANSMISSION) && mat.transmission > 0.0f) {
+        const float FH = fresnel_dielectric(LDotH, etaI, etaO);
+        const V3 Fs = tb_lerp(mat.cspec0, v3s(1.0f), FH);
+        const float Gs = view.GsV * smith_ggx(NDotL, a);
+        bsdf = Gs * Fs * Ds;
+    }
+    if (!(FEAT & TB_FEAT_TRANSMISSION) || mat.transmission < 1.0f) {
+        const float FH = schlick_fresnel(LDotH);
+        const V3 Fs = tb_lerp(mat.cspec0, v3s(1.0f), FH);
+        const float Gs = view.GsV * smith_ggx(NDotL, a);
+        const float FL = schlick_fresnel(NDotL);
+        const float Fd90 = 0.5f + 2.0f * LDotH * LDotH * mat.roughness;
+        const float Fd = tb_lerp(1.0f, Fd90, FL) * tb_lerp(1.0f, Fd90, view.FV);
+        brdf = TB_INV_PI * Fd * mat.color * (1.0f - mat.metallic) * (1.0f - mat.subsurface) + Gs * Fs * Ds;
+        if ((FEAT & TB_FEAT_CLEARCOAT) && !(mat.flags & TB_MAT_NO_CLEARCOAT)) {
+            const float Dr = gtr1_clearcoat(mat, NDotH);
+            const float Fc = tb_lerp(.04f, 1.0f, FH);
+            const float Gr = smith_ggx(NDotL, .25f) * view.GrV;
+            brdf = brdf + v3s(mat.clearcoat * Gr * Fc * Dr);
+        }
+    }
+    r.f = tb_lerp(brdf, bsdf, mat.transmission);
+    return r;
+}
+
 // the GGX half-vector lobe shared by both branches of BSDFSample, disney.h:183-205 / 256-279;
 // sinPhiHalf / cosPhiHalf = sinf / cosf(r1*k2Pi) are computed by the caller
 TB_DEV V3 sample_ggx_reflection(const DMaterial& mat, float r2, float sinPhiHalf, float cosPhiHalf, V3 U, V3 Vt, V3 N, V3 view)
@@ -547,9 +649,10 @@ TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCur
 }
 
 // Consumes the traced shadow ray of the slot generated last; accumulates into the cursor in the
-// reference's order (render.cpp:122-143 for the probe, :176-224 for area lights).
+// reference's order (render.cpp:122-143 for the probe, :176-224 for area lights).  view: bsdf_view() of the surface,
+// where the caller keeps it for the whole bounce (nullptr: each BSDF evaluation computes its own).
 template <uint32_t FEAT = TB_FEAT_ALL>
-TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr, const Hit& sh, NeeCursor& c)
+TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr, const Hit& sh, NeeCursor& c, const BsdfView* view = nullptr)
 {
     const DMaterial& mat = sc.prims[sf.prim].mat;
     const bool isProbe = (FEAT & TB_FEAT_PROBE) && sr.light < 0;   // only the probe sample has no light
@@ -569,7 +672,8 @@ TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr
     V3 f = v3s(0.0f);
     float bsdfPdf = 0.0f;
     if (need) {
-        const BsdfValue b = bsdf_eval_pdf<FEAT>(mat, sf.etaI, sf.etaO, sf.n, sf.wo, sr.d);
+        const BsdfValue b = view ? bsdf_eval_pdf<FEAT>(mat, sf.etaI, sf.etaO, sf.n, sf.wo, sr.d, *view)
+                                 : bsdf_eval_pdf<FEAT>(mat, sf.etaI, sf.etaO, sf.n, sf.wo, sr.d);
         f = b.f;
         bsdfPdf = b.pdf;
     }
@@ -603,9 +707,9 @@ TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr
 }
 
 // After NEE: light-hit termination, BSDF sampling, throughput and medium update, next ray
-// (render.cpp:314-363).  Returns false when the path ends here.
+// (render.cpp:314-363).  Returns false when the path ends here.  view: as for nee_connect().
 template <uint32_t FEAT = TB_FEAT_ALL>
-TB_DEV bool path_scatter(const DScene& sc, PathState& ps, const Surface& sf, V3 neeSum)
+TB_DEV bool path_scatter(const DScene& sc, PathState& ps, const Surface& sf, V3 neeSum, const BsdfView* view = nullptr)
 {
     ps.L = ps.L + ps.T * neeSum;
 
@@ -621,7 +725,8 @@ TB_DEV bool path_scatter(const DScene& sc, PathState& ps, const Surface& sf, V3 
     V3 f = v3s(0.0f);
     if (pdfFromBsdf || pdf > 0.0f) {
         // pdf = BSDFPdf(dir) (disney.h:291) and f = BSDFEval(dir) (render.cpp:341) share one call
-        const BsdfValue b = bsdf_eval_pdf<FEAT>(prim.mat, sf.etaI, sf.etaO, sf.n, sf.wo, bsdfDir);
+        const BsdfValue b = view ? bsdf_eval_pdf<FEAT>(prim.mat, sf.etaI, sf.etaO, sf.n, sf.wo, bsdfDir, *view)
+                                 : bsdf_eval_pdf<FEAT>(prim.mat, sf.etaI, sf.etaO, sf.n, sf.wo, bsdfDir);
         f = b.f;
         if (pdfFromBsdf) pdf = b.pdf;
     }

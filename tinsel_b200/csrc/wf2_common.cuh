@@ -183,10 +183,11 @@ TB_DEV bool wf2_hit(const Wf2SharedBase& S, float4* rec, const DScene& sc, int s
 }
 
 // finish the shading of a surface hit once all NEE samples are folded: BSDF sample, next ray
-// (path_scatter) or termination.  Returns true when the slot continues with a new extension ray.
+// (path_scatter) or termination.  Returns true when the slot continues with a new extension ray.  view: the surface's
+// bsdf_view(), or nullptr (see nee_connect).
 template <uint32_t FEAT = TB_FEAT_ALL>
 TB_DEV bool wf2_scatter(Wf2SharedBase& S, float4* rec, const DScene& sc, int s, const Surface& sf, V3 T, V3 L, Rng rng, float time, V3 neeSum,
-                        int bounce, int maxDepth, V3 absorb, float bsdfPdf, uint32_t sample)
+                        int bounce, int maxDepth, V3 absorb, float bsdfPdf, uint32_t sample, const BsdfView* view = nullptr)
 {
     PathState ps;
     ps.o = v3s(0.0f);
@@ -205,7 +206,7 @@ TB_DEV bool wf2_scatter(Wf2SharedBase& S, float4* rec, const DScene& sc, int s, 
         ps.L = ps.L + ps.T * neeSum;
         go = false;
     } else {
-        go = path_scatter<FEAT>(sc, ps, sf, neeSum);
+        go = path_scatter<FEAT>(sc, ps, sf, neeSum, view);
     }
     cold_st(rec, CC_L, ps.L.x, ps.L.y, ps.L.z, ps.bsdfPdf);
     if (!go) return false;

@@ -98,6 +98,17 @@ TB_DEV unsigned wf2_claim_fullest(Wf2Shared& S, int stick, int& slot, int& stage
     }
 }
 
+// stage A's parts, timed separately in the clock build (tools/stage_clocks.py): the hit prologue (wf2_hit), the light
+// samples (nee_generate), the shadow traces, the connections (wf2_surface, nee_connect) and the BSDF sample
+// (wf2_scatter).  The lanes of a chunk leave the NEE loop at different times, so no lane can wait for the others
+// inside it: each lane reads the clock on its own (wf2_lane_now), and the chunk counts the longest any lane spent.
+enum { WF2_A_HIT = 0, WF2_A_LIGHT = 1, WF2_A_SHADOW = 2, WF2_A_CONNECT = 3, WF2_A_SCATTER = 4, WF2_A_PARTS = 5 };
+#ifdef TB_WF2_STAGE_CLOCKS
+TB_DEV unsigned int wf2_lane_now() { return (unsigned int)clock64(); }
+#else
+TB_DEV unsigned int wf2_lane_now() { return 0u; }
+#endif
+
 #ifdef TB_WF2_STAGE_CLOCKS
 // Per-stage cycle accounting (development builds with -DTB_WF2_STAGE_CLOCKS, read by tb200_stage_clocks, see
 // tools/stage_clocks.py).  Every warp sums clock64() deltas in registers and adds its totals here when it exits.
@@ -105,8 +116,9 @@ TB_DEV unsigned wf2_claim_fullest(Wf2Shared& S, int stick, int& slot, int& stage
 //   [0] claims that got slots   [1] idle: empty claims and the back-off   [2 + k] cycles in stage k
 //   [6 + k] chunks of stage k   [10 + k] lanes active in those chunks      [14] warps
 //   [15 + p] stage R's cycles in part p: WF2_R_SPLAT, WF2_R_CLAIM, WF2_R_REGEN (see wf2_stage_r)
+//   [18 + p] stage A's cycles in part p: WF2_A_HIT ... WF2_A_SCATTER (see the kernel)
 enum { WF2_CLK_CLAIM = 0, WF2_CLK_IDLE = 1, WF2_CLK_CYCLES = 2, WF2_CLK_CHUNKS = 6, WF2_CLK_LANES = 10, WF2_CLK_WARPS = 14, WF2_CLK_R_PARTS = 15,
-       WF2_CLK_N = 18 };
+       WF2_CLK_A_PARTS = 18, WF2_CLK_N = 23 };
 static_assert(WF2_CLK_N == TB_WF2_STAGE_CLOCK_WORDS, "tb_kernels.cuh states the counter count");
 __device__ unsigned long long g_wf2StageClocks[WF2_CLK_N];
 
@@ -114,7 +126,14 @@ __device__ unsigned long long g_wf2StageClocks[WF2_CLK_N];
 // launch, and the tool's launches last far fewer than 2^32 cycles.
 struct Wf2Clocks {
     static constexpr int kinds = 3;   // R, T, A: this kernel has no stage B
-    unsigned int claim = 0, idle = 0, cyc[kinds] = {}, chunks[kinds] = {}, lanes[kinds] = {}, rparts[WF2_R_PARTS] = {};
+    unsigned int claim = 0, idle = 0, cyc[kinds] = {}, chunks[kinds] = {}, lanes[kinds] = {}, rparts[WF2_R_PARTS] = {}, aparts[WF2_A_PARTS] = {};
+
+    // a chunk of stage A: each part counts the longest any lane spent in it (lane_parts: per lane, see the kernel)
+    TB_DEV void add_a(const unsigned int (&lane_parts)[WF2_A_PARTS])
+    {
+#pragma unroll
+        for (int p = 0; p < WF2_A_PARTS; ++p) aparts[p] += __reduce_max_sync(0xffffffffu, lane_parts[p]);
+    }
 
     // the stage kind as a constant index, so the arrays stay in registers
     TB_DEV void add(int stage, unsigned int dt, unsigned act)
@@ -142,6 +161,8 @@ struct Wf2Clocks {
         }
 #pragma unroll
         for (int p = 0; p < WF2_R_PARTS; ++p) atomicAdd(&g_wf2StageClocks[WF2_CLK_R_PARTS + p], (unsigned long long)rparts[p]);
+#pragma unroll
+        for (int p = 0; p < WF2_A_PARTS; ++p) atomicAdd(&g_wf2StageClocks[WF2_CLK_A_PARTS + p], (unsigned long long)aparts[p]);
         atomicAdd(&g_wf2StageClocks[WF2_CLK_WARPS], 1ull);
     }
 };
@@ -236,7 +257,7 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                 if (maxDepth > 0) {
                     // S.flat, not sc.flat: shared-memory loads (wf2_stage_scene stages every flat program -- api.cu's
                     // build_program keeps them to the 32 ops S.flat holds -- and with numFlat == 0 no op is read)
-                    const Hit h = trace_closest<FEAT>(sc, S.flat, v3(S.ox[s], S.oy[s], S.oz[s]), v3(S.dx[s], S.dy[s], S.dz[s]), S.time[s], true);
+                    const Hit h = trace_closest<FEAT, false, true>(sc, S.flat, v3(S.ox[s], S.oy[s], S.oz[s]), v3(S.dx[s], S.dy[s], S.dz[s]), S.time[s], true);
                     S.ht[s] = h.t;
                     S.hnx[s] = h.n.x; S.hny[s] = h.n.y; S.hnz[s] = h.n.z;
                     S.hprim[s] = h.prim;
@@ -249,15 +270,19 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
         } else if (stage == WF2_Q_A) {
             // ===================== A: the whole bounce ============================================
             bool cont = false, fin = false;
+            unsigned int ap[WF2_A_PARTS] = {};   // this lane's cycles per part, in the clock build
             if (active) {
                 float4* rec = coldBase + (size_t)s * CC_CHUNKS;
                 const float4 ct = cold_ld(rec, CC_T), cl = cold_ld(rec, CC_L);
                 float4 ca;
                 PathState ps;
                 Surface sf;
+                unsigned int ta = wf2_lane_now();
                 if (!wf2_hit<FEAT>(S, rec, sc, s, ct, cl, ca, ps, sf)) {
+                    ap[WF2_A_HIT] += wf2_lane_now() - ta;
                     fin = true;
                 } else {
+                    ap[WF2_A_HIT] += wf2_lane_now() - ta;
                     NeeCursor c;
                     ShadowRay sr;
                     nee_begin(c, S.lightBegin);
@@ -267,26 +292,43 @@ __global__ void __launch_bounds__(THREADS, TB_WF2_CTAS_PER_SM) k_wavefront2(cons
                     // them instead of being held in registers across them: the throughput and radiance path_hit
                     // left, and the surface (wf2_surface rebuilds it bit for bit, as stage B of the ring kernel
                     // does).  s2 is s behind an empty asm, so the compiler cannot forward the stores to the reads.
-                    // (Measured on cornell: keeping it all in registers spills, 160 bytes.)
+                    // (Measured on cornell: keeping it all in registers spills, 160 bytes.)  The BSDF's view terms
+                    // (bsdf_view) are the exception: three floats (four with clearcoat), computed once here for every
+                    // BSDF evaluation of the bounce, fit in registers across the traces.
                     cold_st(rec, CC_T, ps.T.x, ps.T.y, ps.T.z, ct.w);
                     cold_st(rec, CC_L, ps.L.x, ps.L.y, ps.L.z, cl.w);
                     const float time = ps.time;
                     Rng rng = ps.rng;
+                    const BsdfView view = bsdf_view<FEAT>(sc.prims[sf.prim].mat, sf.n, sf.wo);
                     int s2 = s;
+                    ta = wf2_lane_now();
                     while (nee_generate<FEAT>(sc, sf, time, c, rng, sr, lightEnd)) {
-                        const Hit sh = trace_closest<FEAT>(sc, S.flat, sr.o, sr.d, time, false);
+                        unsigned int tb = wf2_lane_now();
+                        ap[WF2_A_LIGHT] += tb - ta;
+                        const Hit sh = trace_closest<FEAT, false, true>(sc, S.flat, sr.o, sr.d, time, false);
                         asm volatile("" : "+r"(s2) : "f"(sh.t));
+                        ta = wf2_lane_now();
+                        ap[WF2_A_SHADOW] += ta - tb;
                         sf = wf2_surface(S, sc, s2, ct.w);
-                        nee_connect<FEAT>(sc, sf, sr, sh, c);
+                        nee_connect<FEAT>(sc, sf, sr, sh, c, &view);
+                        tb = wf2_lane_now();
+                        ap[WF2_A_CONNECT] += tb - ta;
+                        ta = tb;
                     }
+                    ap[WF2_A_LIGHT] += wf2_lane_now() - ta;   // the call that found no further sample
                     asm volatile("" : "+r"(s2));
                     const float4* rec2 = coldBase + (size_t)s2 * CC_CHUNKS;
                     const float4 t2 = cold_ld(rec2, CC_T), l2 = cold_ld(rec2, CC_L), a2 = cold_ld(rec2, CC_A);
+                    ta = wf2_lane_now();
                     cont = wf2_scatter<FEAT>(S, rec, sc, s, sf, v3(t2.x, t2.y, t2.z), v3(l2.x, l2.y, l2.z), rng, time, c.sum, (int)(S.flags[s] >> 8), maxDepth,
-                                       v3(a2.x, a2.y, a2.z), l2.w, f2u(a2.w));
+                                       v3(a2.x, a2.y, a2.z), l2.w, f2u(a2.w), &view);
+                    ap[WF2_A_SCATTER] += wf2_lane_now() - ta;
                     fin = !cont;
                 }
             }
+#ifdef TB_WF2_STAGE_CLOCKS
+            clk.add_a(ap);
+#endif
             __threadfence_block();
             wf2_push(S, WF2_Q_T, cont, s);
             wf2_push(S, WF2_Q_R, fin, s);

@@ -8,7 +8,10 @@ product build) as tinsel_b200/libtinsel_b200_clocks.so, renders cornell in the b
 (1024x1024, 32 spp per render_device call, TINSEL_B200_LIB pointing at the variant) and prints per stage:
 SM cycles per camera sample, visits (warp chunks) per sample and the mean number of lanes active per chunk.
 Stage R is also split into its parts: the splat of the finished sample, the claim of new sample indices (from
-the vote to the index) and the regeneration (the camera rays).
+the vote to the index) and the regeneration (the camera rays).  So is stage A: the hit prologue, the light samples,
+the shadow traces, the connections and the BSDF sample.  A's lanes leave the NEE loop at different times, so each
+of its parts counts, per chunk, the longest any lane spent in it; the parts can add up to a little more than the
+stage where lanes run different parts side by side.
 
     python tools/stage_clocks.py [--steps N] [--lib PATH | --no-build]
 
@@ -24,10 +27,12 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 VARIANT = "libtinsel_b200_clocks.so"
-WORDS = 18                     # tb_kernels.cuh: TB_WF2_STAGE_CLOCK_WORDS
+WORDS = 23                     # tb_kernels.cuh: TB_WF2_STAGE_CLOCK_WORDS
 WARPS_PER_CTA = 512 // 32
 STAGES = ["R", "T", "A", "B"]  # counter order (wf2_lanes.cuh: Wf2Clocks)
 R_PARTS = ["splat", "claim", "regenerate"]   # wf2_common.cuh: WF2_R_*
+A_PARTS = ["hit", "light", "shadow", "connect", "scatter"]   # wf2_lanes.cuh: WF2_A_*
+PARTS = {"R": (15, R_PARTS), "A": (18, A_PARTS)}
 
 
 def main():
@@ -93,10 +98,12 @@ def main():
             continue
         print("%-10s %14.1f %7.1f%% %16.3f %12.2f" % (name, cyc[k] / per, 100.0 * cyc[k] / total, lanes[k] / samples,
                                                      lanes[k] / chunks[k]))
-        if name == "R":
-            # stage R's parts; what is left is the bookkeeping between them (flags, the claim loop's vote)
-            for p, part in enumerate(R_PARTS):
-                print("%-10s %14.1f %7.1f%%" % ("  " + part, c[15 + p] / per, 100.0 * c[15 + p] / total))
+        if name in PARTS:
+            # the stage's parts; what is left is the bookkeeping between them (flags, the claim loop's vote, the
+            # slot state's loads and stores)
+            first, parts = PARTS[name]
+            for p, part in enumerate(parts):
+                print("%-10s %14.1f %7.1f%%" % ("  " + part, c[first + p] / per, 100.0 * c[first + p] / total))
     print("%-10s %14.1f" % ("total", total / per))
 
 
