@@ -351,6 +351,42 @@ typedef struct tb200_tri_hit { int32_t tri; float u, v, w; } tb200_tri_hit;   /*
 int tb200_trace_rays_tri(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims,
                          tb200_tri_hit* tris, int64_t numRays);
 
+/* ---- batched BSDF queries --------------------------------------------------------------------
+ * The material half of a bounce, for a caller's batch: per query i, the Disney BSDF of src/disney.h
+ * bit for bit (a NaN may have another payload), with the material the path tracer shades primitive
+ * `prim` with (a mesh primitive has one material).  `n`, `v` (towards the viewer) and `l` (towards the
+ * light) are used as given, never normalised, as are the etas, which may take any value.  PathTrace's
+ * convention (src/render.cpp:259-269): a ray in air hitting a surface has etaI = 1, etaO = the
+ * material's ior (tb200_material eta, or Material::GetIndexOfRefraction's value from `specular` when
+ * eta == 0); a ray inside a medium of ior eta has etaI = eta, etaO = 1.
+ *   tb200_bsdf_eval:   out[i].f = BSDFEval(mat, etaI, etaO, n, v, l), out[i].pdf = BSDFPdf(same).
+ *   tb200_bsdf_sample: one step of PathTrace (src/render.cpp:327-341): BSDFSample with the basis
+ *                      BasisFromVector(n) and Random(seeds[i]) (src/maths.h:1040-1044) gives l, pdf
+ *                      and type; then f = BSDFEval(l) when pdf > 0, else f = 0.  q[i].l is ignored.
+ * A prim outside [0, numPrimitives) gives f = 0, pdf = 0 and, when sampling, l = 0, type = -1, so the
+ * prims of tb200_trace_rays can be passed straight through on misses (-1).
+ * `q`, `seeds` and `out` are DEVICE memory of the renderer's device (a multi-device renderer: its head);
+ * `q` and `out` 16-byte aligned, `seeds` 4-byte aligned.  The refusals, stream, synchronisation and side
+ * effects are tb200_trace_rays': null pointers, n < 0, host or foreign-device memory and spans past the
+ * end of their allocation are refused before any launch; needs no tb200_init; adds 1 to
+ * stats.kernelLaunches, sets stats.gpuMs to its kernel's time, and touches nothing else.  n == 0
+ * launches nothing.  Returns 0 on success. */
+typedef struct tb200_bsdf_query {   /* 48 B */
+    float n[3];
+    int32_t prim;
+    float v[3];
+    float etaI;
+    float l[3];
+    float etaO;
+} tb200_bsdf_query;
+typedef struct tb200_bsdf_value { float f[3]; float pdf; } tb200_bsdf_value;                              /* 16 B */
+typedef struct tb200_bsdf_sampled { float l[3]; float pdf; float f[3]; int32_t type; } tb200_bsdf_sampled;   /* 32 B */
+/* tb200_bsdf_sampled.type: BSDFType, src/disney.h:27-32 (-1 for a prim outside the scene) */
+enum { TB200_BSDF_REFLECTED = 0, TB200_BSDF_TRANSMITTED = 1, TB200_BSDF_SPECULAR = 2 };
+int tb200_bsdf_eval(tb200_renderer* r, const tb200_bsdf_query* q, tb200_bsdf_value* out, int64_t n);
+int tb200_bsdf_sample(tb200_renderer* r, const tb200_bsdf_query* q, const uint32_t* seeds, tb200_bsdf_sampled* out,
+                      int64_t n);
+
 /* Sets the frame counter (frame k seeds sample k of every pixel). */
 void tb200_set_frame(tb200_renderer* r, int frame);
 

@@ -88,6 +88,10 @@ def load_library():
     lib.tb200_trace_rays_tri.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_occluded_rays.restype = C.c_int
     lib.tb200_occluded_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_bsdf_eval.restype = C.c_int
+    lib.tb200_bsdf_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_bsdf_sample.restype = C.c_int
+    lib.tb200_bsdf_sample.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_set_frame.restype = None
     lib.tb200_set_frame.argtypes = [C.c_void_p, C.c_int]
     lib.tb200_get_stats.restype = None
@@ -119,6 +123,47 @@ def last_error():
 
 def sample_seed(pixel, frame):
     return load_library().tb200_sample_seed(pixel, frame)
+
+
+def material_ior(eta, specular):
+    """Material::GetIndexOfRefraction (src/scene.h:72-78) in float32, elementwise: `eta` where it is not 0, else
+    2 / (1 - sqrt(float(0.08 * specular))) - 1 with the product in double, as the reference rounds it.  The etaO of
+    a path entering a material (PathTrace's eta convention, include/tinsel_b200.h: tb200_bsdf_eval).  Returns a
+    float32 numpy array (a 0-d one for scalars)."""
+    eta = np.asarray(eta, np.float32)
+    specular = np.asarray(specular, np.float32)
+    with np.errstate(all="ignore"):
+        k = np.sqrt((0.08 * specular.astype(np.float64)).astype(np.float32))
+        from_specular = np.float32(2) / (np.float32(1) - k) - np.float32(1)
+    return np.where(eta == 0, from_specular, eta).astype(np.float32)
+
+
+def bsdf_queries(prims, n, v, eta_i, eta_o, l=None):
+    """Packs tb200_bsdf_query records for Renderer.bsdf_eval / bsdf_sample: an (N, 12) float32 tensor on `prims`'
+    device with n.xyz, the int32 primitive's bits, v.xyz, etaI, l.xyz, etaO per row.  prims: (N,) int32 tensor
+    (trace_rays' prims can be passed as they are); n, v, l: (N, 3) float32 tensors (l None: zeros, which sampling
+    ignores); eta_i, eta_o: (N,) float32 tensors or Python numbers."""
+    import torch
+    if not isinstance(prims, torch.Tensor) or prims.dtype != torch.int32 or prims.dim() != 1:
+        raise ValueError("prims must be an (N,) int32 tensor")
+    count, dev = prims.shape[0], prims.device
+    q = torch.empty((count, 12), dtype=torch.float32, device=dev)
+
+    def put(col, x, width, name):
+        if not isinstance(x, torch.Tensor):
+            q[:, col:col + width] = float(x)
+            return
+        if x.dtype != torch.float32 or tuple(x.shape) != ((count, width) if width > 1 else (count,)):
+            raise ValueError("%s must be a float32 tensor of shape %s" % (name, (count, width) if width > 1 else (count,)))
+        q[:, col:col + width] = x.to(dev).reshape(count, width)
+
+    put(0, n, 3, "n")
+    q[:, 3] = prims.view(torch.float32)
+    put(4, v, 3, "v")
+    put(7, eta_i, 1, "eta_i")
+    put(8, l if l is not None else 0.0, 3, "l")
+    put(11, eta_o, 1, "eta_o")
+    return q
 
 
 def scene_cache_save(scene, path):
@@ -314,13 +359,13 @@ class Renderer:
         if not x.is_contiguous():
             raise ValueError("%s must be contiguous" % name)
 
-    def _check_rays(self, rays):
-        """Checks a (N, 8) float32 ray tensor and returns N."""
+    def _check_records(self, x, name, width, dtype):
+        """Checks a (N, width) tensor of query records and returns N."""
         import torch
-        if not isinstance(rays, torch.Tensor) or rays.dim() != 2:
-            raise ValueError("rays must be a (N, 8) tensor")
-        n = rays.shape[0]
-        self._check_tensor(rays, "rays", (n, 8), torch.float32)
+        if not isinstance(x, torch.Tensor) or x.dim() != 2:
+            raise ValueError("%s must be a (N, %d) tensor" % (name, width))
+        n = x.shape[0]
+        self._check_tensor(x, name, (n, width), dtype)
         return n
 
     def _wait_for_torch(self):
@@ -329,21 +374,28 @@ class Renderer:
         if not self._external_stream:
             torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()
 
-    def _query(self, entry, rays, outputs):
-        """What the ray queries share: checks `rays` (N rays) and each output (tensor or None, name, shape after N,
-        dtype), allocating on the head device those not given; when N > 0, waits for torch and calls the library's
-        `entry` on the rays and the outputs, raising on a refusal.  Returns the output tensors."""
+    def _query(self, entry, records, inputs, outputs):
+        """What the batched queries share.  records: (tensor, name, width, dtype), the (N, width) records that set N;
+        inputs: further input arrays and outputs: output arrays, each (tensor or None, name, shape after N, dtype).
+        Checks them all, allocating on the head device the outputs not given (an input must be given); when N > 0,
+        waits for torch and calls the library's `entry` on the records, the inputs and the outputs, raising on a
+        refusal.  Returns the output tensors."""
         import torch
-        n = self._check_rays(rays)
+        x, name, width, dtype = records
+        n = self._check_records(x, name, width, dtype)
+        args = [x]
+        for y, yname, shape, ydtype in inputs:
+            self._check_tensor(y, yname, (n,) + shape, ydtype)
+            args.append(y)
         out = []
-        for x, name, shape, dtype in outputs:
-            if x is None:
-                x = torch.empty((n,) + shape, dtype=dtype, device=torch.device("cuda", self.device))
-            self._check_tensor(x, name, (n,) + shape, dtype)
-            out.append(x)
+        for y, yname, shape, ydtype in outputs:
+            if y is None:
+                y = torch.empty((n,) + shape, dtype=ydtype, device=torch.device("cuda", self.device))
+            self._check_tensor(y, yname, (n,) + shape, ydtype)
+            out.append(y)
         if n > 0:
             self._wait_for_torch()
-            self._check(getattr(self.lib, entry)(self.h, rays.data_ptr(), *[x.data_ptr() for x in out], n), entry)
+            self._check(getattr(self.lib, entry)(self.h, *[y.data_ptr() for y in args + out], n), entry)
         return out
 
     def trace_rays(self, rays, hits=None, prims=None):
@@ -353,7 +405,8 @@ class Renderer:
         `hits` / `prims` when given.  On the renderer's private stream the call first waits for torch's current
         stream, so that tensors written there are complete; after set_stream the work is ordered on that stream."""
         import torch
-        hits, prims = self._query("tb200_trace_rays", rays, [(hits, "hits", (4,), torch.float32), (prims, "prims", (), torch.int32)])
+        hits, prims = self._query("tb200_trace_rays", (rays, "rays", 8, torch.float32), [],
+                                  [(hits, "hits", (4,), torch.float32), (prims, "prims", (), torch.int32)])
         return hits, prims
 
     def trace_rays_tri(self, rays, hits=None, prims=None, tris=None):
@@ -363,9 +416,9 @@ class Renderer:
         own space; tri = -1 and uvw = 0 for a sphere hit, a plane hit or a miss.  Both are views of one (N, 4) int32
         tensor, the tb200_tri_hit records, which `tris` gives when it is passed.  Stream behaviour as for trace_rays."""
         import torch
-        hits, prims, tris = self._query("tb200_trace_rays_tri", rays, [(hits, "hits", (4,), torch.float32),
-                                                                        (prims, "prims", (), torch.int32),
-                                                                        (tris, "tris", (4,), torch.int32)])
+        hits, prims, tris = self._query("tb200_trace_rays_tri", (rays, "rays", 8, torch.float32), [],
+                                        [(hits, "hits", (4,), torch.float32), (prims, "prims", (), torch.int32),
+                                         (tris, "tris", (4,), torch.int32)])
         return hits, prims, tris[:, 0], tris[:, 1:].view(torch.float32)
 
     def occluded(self, rays, out=None):
@@ -374,8 +427,32 @@ class Renderer:
         dir = target - origin, tmax = 1 asks about the segment between two points).  Returns a (N,) torch.bool
         tensor, `out` when given.  Stream behaviour as for trace_rays."""
         import torch
-        out, = self._query("tb200_occluded_rays", rays, [(out, "out", (), torch.bool)])
+        out, = self._query("tb200_occluded_rays", (rays, "rays", 8, torch.float32), [], [(out, "out", (), torch.bool)])
         return out
+
+    def bsdf_eval(self, queries, out=None):
+        """The Disney BSDF of every query (tb200_bsdf_eval): BSDFEval and BSDFPdf (src/disney.h) bit for bit, with the
+        material the renderer shades primitive `prim` with.  queries: contiguous float32 CUDA tensor (N, 12) on the
+        head device, the tb200_bsdf_query records n.xyz, prim, v.xyz, etaI, l.xyz, etaO, with column 3 holding the
+        int32 primitive index's bits (bsdf_queries packs them).  n, v, l are used as given, never normalised.
+        Returns (N, 4) float32: f.rgb, pdf, in `out` when given; a prim outside the scene gives zeros.  Stream
+        behaviour as for trace_rays."""
+        import torch
+        out, = self._query("tb200_bsdf_eval", (queries, "queries", 12, torch.float32), [],
+                           [(out, "out", (4,), torch.float32)])
+        return out
+
+    def bsdf_sample(self, queries, seeds, out=None):
+        """One BSDF sampling step of PathTrace per query (tb200_bsdf_sample): BSDFSample with BasisFromVector(n) and
+        Random(seed), then f = BSDFEval of the sampled direction where its pdf > 0, else 0; bit for bit.  queries:
+        as for bsdf_eval (their l is ignored); seeds: (N,) int32 tensor whose bits are the uint32 seeds.  Returns
+        (l (N, 3) float32, pdf (N,) float32, f (N, 3) float32, type (N,) int32: abi.BSDF_*, -1 for a prim outside
+        the scene, whose other outputs are 0), views of one (N, 8) tensor of tb200_bsdf_sampled records, which `out`
+        (float32) gives when it is passed.  Stream behaviour as for trace_rays."""
+        import torch
+        out, = self._query("tb200_bsdf_sample", (queries, "queries", 12, torch.float32), [(seeds, "seeds", (), torch.int32)],
+                           [(out, "out", (8,), torch.float32)])
+        return out[:, 0:3], out[:, 3], out[:, 4:7], out[:, 7].view(torch.int32)
 
     def set_frame(self, frame):
         self.lib.tb200_set_frame(self.h, frame)

@@ -155,6 +155,27 @@ class TriHit(C.Structure):
     _fields_ = [("tri", C.c_int32), ("u", C.c_float), ("v", C.c_float), ("w", C.c_float)]
 
 
+class BsdfQuery(C.Structure):
+    """tb200_bsdf_query: one query of tb200_bsdf_eval and tb200_bsdf_sample (48 bytes; `l` is ignored when sampling)."""
+    _fields_ = [("n", C.c_float * 3), ("prim", C.c_int32), ("v", C.c_float * 3), ("etaI", C.c_float),
+                ("l", C.c_float * 3), ("etaO", C.c_float)]
+
+
+class BsdfValue(C.Structure):
+    """tb200_bsdf_value: BSDFEval and BSDFPdf of one query, from tb200_bsdf_eval (16 bytes)."""
+    _fields_ = [("f", C.c_float * 3), ("pdf", C.c_float)]
+
+
+class BsdfSampled(C.Structure):
+    """tb200_bsdf_sampled: the sampled direction, its pdf, BSDFEval of it and its BSDFType, from tb200_bsdf_sample
+    (32 bytes)."""
+    _fields_ = [("l", C.c_float * 3), ("pdf", C.c_float), ("f", C.c_float * 3), ("type", C.c_int32)]
+
+
+# BSDFType (src/disney.h:27-32), tb200_bsdf_sampled.type
+BSDF_REFLECTED, BSDF_TRANSMITTED, BSDF_SPECULAR = 0, 1, 2
+
+
 class BvhBuildInfo(C.Structure):
     _fields_ = [("numNodes", C.c_int32), ("rounds", C.c_int32), ("kernelLaunches", C.c_uint64), ("buildMs", C.c_double)]
 
@@ -198,6 +219,8 @@ EXPORTS = [
     "tb200_trace_rays",
     "tb200_trace_rays_tri",
     "tb200_occluded_rays",
+    "tb200_bsdf_eval",
+    "tb200_bsdf_sample",
     "tb200_set_frame",
     "tb200_get_stats",
     "tb200_last_kernel",

@@ -1831,36 +1831,37 @@ static bool check_device_span(const char* entry, const tb200_renderer* r, const 
     return true;
 }
 
-// One output of a ray query, as the caller passed it: checked by check_device_span for numRays records
+// One array of a query, as the caller passed it: checked by check_device_span for `count` records
 struct QuerySpan {
     const void* ptr;
-    size_t bytesPerRay;
+    size_t bytesPerItem;
     size_t align;
     const char* what;   // its name in refusals
 };
 
-// Every ray query: checks the renderer, the ray count, the rays and then the outputs in the order given (the first
-// refusal sets the error), makes the renderer's device current, runs the query's kernel on r's stream with Q's
-// outputs, waits for it and sets stats.gpuMs to its time.  No rays: returns 0 before the pointers are checked.
-static int run_query(const char* entry, tb200_renderer* r, QueryKind kind, const tb200_ray* rays, int64_t numRays,
-                     std::initializer_list<QuerySpan> outputs, QueryParams Q)
+// Every batched query: checks the renderer, the record count (named `countName` in refusals), then the input and
+// the outputs in the order given (the first refusal sets the error), makes the renderer's device current, runs the
+// query's kernel on r's stream with Q's pointers, waits for it and sets stats.gpuMs to its time.  No records:
+// returns 0 before the pointers are checked.
+static int run_query(const char* entry, tb200_renderer* r, QueryKind kind, const char* countName, int64_t count,
+                     std::initializer_list<QuerySpan> spans, QueryParams Q)
 {
     auto fail = [&](const std::string& why) {
         set_error(std::string(entry) + ": " + why);
         return -1;
     };
     if (!r) return fail("null renderer");
-    if (numRays < 0 || numRays > (int64_t)(SIZE_MAX / sizeof(tb200_ray)))
-        return fail("numRays " + std::to_string((long long)numRays) + " is out of range");
-    if (numRays == 0) return 0;
+    size_t widest = 1;
+    for (const QuerySpan& s : spans) widest = std::max(widest, s.bytesPerItem);
+    if (count < 0 || count > (int64_t)(SIZE_MAX / widest))
+        return fail(std::string(countName) + " " + std::to_string((long long)count) + " is out of range");
+    if (count == 0) return 0;
     cudaSetDevice(r->device);   // a multi-device renderer answers on its head, which holds a full copy of the scene
-    const size_t n = (size_t)numRays;
-    if (!check_device_span(entry, r, rays, n * sizeof(tb200_ray), 16, "rays")) return -1;
-    for (const QuerySpan& s : outputs)
-        if (!check_device_span(entry, r, s.ptr, n * s.bytesPerRay, s.align, s.what)) return -1;
+    const size_t n = (size_t)count;
+    for (const QuerySpan& s : spans)
+        if (!check_device_span(entry, r, s.ptr, n * s.bytesPerItem, s.align, s.what)) return -1;
     Q.scene = r->scene;
-    Q.rays = reinterpret_cast<const float4*>(rays);
-    Q.numRays = numRays;
+    Q.numRays = count;
     Q.counter = r->mem.counter.get();   // the wavefront's work counter: free between launches on this stream
 
     unsigned long long launches = 0;
@@ -1876,32 +1877,59 @@ static int run_query(const char* entry, tb200_renderer* r, QueryKind kind, const
 
 static_assert(sizeof(tb200_ray) == 32 && sizeof(tb200_hit) == 16, "the query kernels read two float4 per ray and write one hit");
 static_assert(sizeof(tb200_tri_hit) == 16, "the query kernel writes one int4 per triangle record");
+static_assert(sizeof(tb200_bsdf_query) == 48 && sizeof(tb200_bsdf_value) == 16 && sizeof(tb200_bsdf_sampled) == 32,
+              "the BSDF query kernels read three float4 per query and write one or two");
 
 int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, int64_t numRays)
 {
     QueryParams Q = {};
+    Q.rays = reinterpret_cast<const float4*>(rays);
     Q.hits = reinterpret_cast<float4*>(hits);
     Q.prims = prims;
-    return run_query("tb200_trace_rays", r, QueryKind::Closest, rays, numRays,
-                     {{hits, sizeof(tb200_hit), 16, "hits"}, {prims, sizeof(int32_t), 4, "prims"}}, Q);
+    return run_query("tb200_trace_rays", r, QueryKind::Closest, "numRays", numRays,
+                     {{rays, sizeof(tb200_ray), 16, "rays"}, {hits, sizeof(tb200_hit), 16, "hits"},
+                      {prims, sizeof(int32_t), 4, "prims"}}, Q);
 }
 
 int tb200_occluded_rays(tb200_renderer* r, const tb200_ray* rays, uint8_t* occluded, int64_t numRays)
 {
     QueryParams Q = {};
+    Q.rays = reinterpret_cast<const float4*>(rays);
     Q.occluded = occluded;
-    return run_query("tb200_occluded_rays", r, QueryKind::Occluded, rays, numRays, {{occluded, 1, 1, "occluded"}}, Q);
+    return run_query("tb200_occluded_rays", r, QueryKind::Occluded, "numRays", numRays,
+                     {{rays, sizeof(tb200_ray), 16, "rays"}, {occluded, 1, 1, "occluded"}}, Q);
 }
 
 int tb200_trace_rays_tri(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims, tb200_tri_hit* tris, int64_t numRays)
 {
     QueryParams Q = {};
+    Q.rays = reinterpret_cast<const float4*>(rays);
     Q.hits = reinterpret_cast<float4*>(hits);
     Q.prims = prims;
     Q.tris = reinterpret_cast<int4*>(tris);
-    return run_query("tb200_trace_rays_tri", r, QueryKind::ClosestTri, rays, numRays,
-                     {{hits, sizeof(tb200_hit), 16, "hits"}, {prims, sizeof(int32_t), 4, "prims"},
-                      {tris, sizeof(tb200_tri_hit), 16, "tris"}}, Q);
+    return run_query("tb200_trace_rays_tri", r, QueryKind::ClosestTri, "numRays", numRays,
+                     {{rays, sizeof(tb200_ray), 16, "rays"}, {hits, sizeof(tb200_hit), 16, "hits"},
+                      {prims, sizeof(int32_t), 4, "prims"}, {tris, sizeof(tb200_tri_hit), 16, "tris"}}, Q);
+}
+
+int tb200_bsdf_eval(tb200_renderer* r, const tb200_bsdf_query* q, tb200_bsdf_value* out, int64_t n)
+{
+    QueryParams Q = {};
+    Q.bsdfQueries = reinterpret_cast<const float4*>(q);
+    Q.bsdfValues = reinterpret_cast<float4*>(out);
+    return run_query("tb200_bsdf_eval", r, QueryKind::BsdfEval, "n", n,
+                     {{q, sizeof(tb200_bsdf_query), 16, "q"}, {out, sizeof(tb200_bsdf_value), 16, "out"}}, Q);
+}
+
+int tb200_bsdf_sample(tb200_renderer* r, const tb200_bsdf_query* q, const uint32_t* seeds, tb200_bsdf_sampled* out, int64_t n)
+{
+    QueryParams Q = {};
+    Q.bsdfQueries = reinterpret_cast<const float4*>(q);
+    Q.seeds = seeds;
+    Q.bsdfSamples = reinterpret_cast<float4*>(out);
+    return run_query("tb200_bsdf_sample", r, QueryKind::BsdfSample, "n", n,
+                     {{q, sizeof(tb200_bsdf_query), 16, "q"}, {seeds, sizeof(uint32_t), 4, "seeds"},
+                      {out, sizeof(tb200_bsdf_sampled), 16, "out"}}, Q);
 }
 
 #ifdef TB_WF2_STAGE_CLOCKS

@@ -128,22 +128,29 @@ struct NlmParams {
 };
 void launch_nlm(const NlmParams& p, cudaStream_t stream, unsigned long long* launchCount);
 
-// The batched ray queries (tb_query.cuh), each Trace (render.cpp:17-62) of every ray of a caller's batch:
+// The batched queries (tb_query.cuh): the ray queries, each Trace (render.cpp:17-62) of every ray of a caller's
+// batch, and the BSDF queries, one Disney BSDF call (disney.h) per query record:
 enum class QueryKind {
     Closest,      // tb200_trace_rays: the closest hit
     ClosestTri,   // tb200_trace_rays_tri: the closest hit and the winner's triangle and barycentric weights
     Occluded,     // tb200_occluded_rays: whether Trace hits something before the ray's tmax
+    BsdfEval,     // tb200_bsdf_eval: BSDFEval and BSDFPdf
+    BsdfSample,   // tb200_bsdf_sample: BSDFSample, then BSDFEval of the sampled direction
 };
-// Every query's parameters.  The output pointers a query does not write stay null.
+// Every query's parameters.  The input and output pointers a query does not use stay null.
 struct QueryParams {
     DScene scene;
-    const float4* rays;   // 2 per ray: origin.xyz, time; dir.xyz, pad (Occluded: tmax)
+    const float4* rays;   // Closest, ClosestTri, Occluded: 2 per ray: origin.xyz, time; dir.xyz, pad (Occluded: tmax)
     float4* hits;         // Closest, ClosestTri: 1 per ray: t, normal.xyz
     int* prims;           // Closest, ClosestTri: 1 per ray: closest primitive, -1 on a miss
     int4* tris;           // ClosestTri: 1 per ray: triangle, then the bits of u, v, w; -1, 0, 0, 0 unless a mesh was hit
     unsigned char* occluded;   // Occluded: 1 per ray: 1 when occluded, else 0
-    long long numRays;
-    unsigned long long* counter;   // work counter, cleared by the launch
+    const float4* bsdfQueries;  // BsdfEval, BsdfSample: 3 per query: n.xyz, prim bits; v.xyz, etaI; l.xyz, etaO
+    const uint32_t* seeds;      // BsdfSample: 1 per query: the Random seed
+    float4* bsdfValues;         // BsdfEval: 1 per query: f.rgb, pdf
+    float4* bsdfSamples;        // BsdfSample: 2 per query: l.xyz, pdf; f.rgb, type bits
+    long long numRays;    // records in the batch (rays or BSDF queries)
+    unsigned long long* counter;   // work counter of the ray queries, cleared by the launch
 };
 // Unlike the launches above, it leaves tb200_last_kernel alone and so returns no kernel name.
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);

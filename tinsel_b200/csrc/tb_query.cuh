@@ -1,11 +1,12 @@
 // tb_query.cuh -- batched closest-hit ray query (tb200_trace_rays): Trace(scene, Ray(origin, dir, time)) of
 // render.cpp:17-62 for every ray of a caller's batch, bit for bit, through the same trace_closest() the
 // renderer runs; the same query reporting the hit triangle and its barycentric weights (tb200_trace_rays_tri); and
-// the batched occlusion query (tb200_occluded_rays) over trace_occluded().  Included once, by kernels.cu.
+// the batched occlusion query (tb200_occluded_rays) over trace_occluded(); and the batched BSDF queries
+// (tb200_bsdf_eval, tb200_bsdf_sample) over the renderer's Disney BSDF functions.  Included once, by kernels.cu.
 //
-// A persistent kernel: as many CTAs as the SMs hold at once, for the whole batch.  Their warps claim chunks of 32
-// rays from a global counter: a static split would leave SMs idle, because a ray that hits a plane costs a few
-// dozen instructions and one that walks a deep mesh BVH more than ten times that.
+// The ray queries run a persistent kernel: as many CTAs as the SMs hold at once, for the whole batch.  Their warps
+// claim chunks of 32 rays from a global counter: a static split would leave SMs idle, because a ray that hits a plane
+// costs a few dozen instructions and one that walks a deep mesh BVH more than ten times that.
 
 #define TB_QUERY_THREADS 256
 
@@ -66,19 +67,93 @@ __global__ void __launch_bounds__(TB_QUERY_THREADS) k_occluded_rays(const __grid
     });
 }
 
+// bsdf_eval_pdf()'s body, inlined: that function is out of line and takes the material by reference, so the
+// kernel's copy of it, whose flags it changes, would live in a 112-byte local-memory frame (DESIGN §5.1); inlined,
+// the copy stays in registers.  bsdf_pdf() and bsdf_eval() are the functions bsdf_eval_pdf() calls.
+static __device__ __forceinline__ BsdfValue query_eval_pdf(const DMaterial& mat, float etaI, float etaO, V3 N, V3 V, V3 L)
+{
+    BsdfValue r;
+    r.pdf = bsdf_pdf<TB_FEAT_ALL>(mat, etaI, etaO, N, V, L);
+    r.f = bsdf_eval<TB_FEAT_ALL>(mat, etaI, etaO, N, V, L);
+    return r;
+}
+
+// The BSDF queries: BSDFEval + BSDFPdf (QueryKind::BsdfEval) or, with SAMPLE, one BSDFSample step of PathTrace
+// followed by BSDFEval of the sampled direction (QueryKind::BsdfSample), per query record, bit for bit.
+// Every query costs about the same (one BSDF call, no walk), so a grid-stride loop with one query per thread needs
+// no work counter.  Each thread loads its record with three 16-byte loads and writes with streaming stores.
+//
+// The material is the primitive's DMaterial with TB_MAT_NO_FRESNEL and TB_MAT_NO_CLEARCOAT cleared: those skips are
+// exact only for the etas and the front-facing unit vectors a path produces (tb_scene.cuh: make_material,
+// set_fresnel_flags), and a caller may pass any.  TB_MAT_GTR1_WIDE picks GTR1's value, not a skip, and stays.  So
+// the TB_FEAT_ALL instantiation runs the reference's full arithmetic.
+template <bool SAMPLE>
+__global__ void __launch_bounds__(TB_QUERY_THREADS) k_bsdf_query(const __grid_constant__ QueryParams P)
+{
+    const unsigned long long n = (unsigned long long)P.numRays;
+    const unsigned long long stride = (unsigned long long)gridDim.x * TB_QUERY_THREADS;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * TB_QUERY_THREADS + threadIdx.x; i < n; i += stride) {
+        // a: n.xyz, prim bits; b: v.xyz, etaI; c: l.xyz, etaO
+        const float4 a = __ldg(&P.bsdfQueries[3 * i]), b = __ldg(&P.bsdfQueries[3 * i + 1]);
+        const float4 c = __ldg(&P.bsdfQueries[3 * i + 2]);
+        const int prim = __float_as_int(a.w);
+        const bool inScene = prim >= 0 && prim < P.scene.numPrims;
+        DMaterial mat;
+        if (inScene) {
+            mat = P.scene.prims[prim].mat;
+            mat.flags &= ~(uint32_t)(TB_MAT_NO_FRESNEL | TB_MAT_NO_CLEARCOAT);
+        }
+        const V3 N = v3(a.x, a.y, a.z), V = v3(b.x, b.y, b.z);
+        if constexpr (!SAMPLE) {
+            BsdfValue r = {v3s(0.0f), 0.0f};
+            if (inScene) r = query_eval_pdf(mat, b.w, c.w, N, V, v3(c.x, c.y, c.z));
+            __stcs(&P.bsdfValues[i], make_float4(r.f.x, r.f.y, r.f.z, r.pdf));
+        } else {
+            V3 L = v3s(0.0f), f = v3s(0.0f);
+            float pdf = 0.0f;
+            int type = -1;
+            if (inScene) {
+                // path_scatter (tb_shade.cuh), less its path state
+                Rng rng = rng_seed(__ldg(&P.seeds[i]));
+                V3 u, v;
+                basis_from_vector(N, &u, &v);
+                type = TB_REFLECTED;
+                const bool pdfFromBsdf = bsdf_sample_dir<TB_FEAT_ALL>(mat, b.w, c.w, u, v, N, V, L, pdf, type, rng);
+                if (pdfFromBsdf || pdf > 0.0f) {
+                    const BsdfValue r = query_eval_pdf(mat, b.w, c.w, N, V, L);
+                    f = r.f;
+                    if (pdfFromBsdf) pdf = r.pdf;
+                }
+                if (!(pdf > 0.0f)) f = v3s(0.0f);   // PathTrace ends the path before it evaluates
+            }
+            __stcs(&P.bsdfSamples[2 * i], make_float4(L.x, L.y, L.z, pdf));
+            __stcs(&P.bsdfSamples[2 * i + 1], make_float4(f.x, f.y, f.z, __int_as_float(type)));
+        }
+    }
+}
+
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
     if (p.numRays <= 0) return;
-    void (*kernel)(QueryParams) = kind == QueryKind::Closest    ? k_trace_rays<false>
+    const bool bsdf = kind == QueryKind::BsdfEval || kind == QueryKind::BsdfSample;
+    void (*kernel)(QueryParams) = kind == QueryKind::Closest      ? k_trace_rays<false>
                                   : kind == QueryKind::ClosestTri ? k_trace_rays<true>
-                                                                  : k_occluded_rays;
-    // as many CTAs as the SMs hold at once, but no more than there are 32-ray chunks
+                                  : kind == QueryKind::Occluded   ? k_occluded_rays
+                                  : kind == QueryKind::BsdfEval   ? k_bsdf_query<false>
+                                                                  : k_bsdf_query<true>;
+    // as many CTAs as the SMs hold at once, but no more than there are 32-ray chunks (BSDF queries: one per thread)
     int perSM = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kernel, TB_QUERY_THREADS, 0) != cudaSuccess || perSM < 1) perSM = 1;
-    const unsigned long long chunks = ((unsigned long long)p.numRays + 31ull) / 32ull;
-    const unsigned long long warps = (unsigned long long)TB_QUERY_THREADS / 32ull;
     const unsigned long long grid = (unsigned long long)(numSMs > 0 ? numSMs : 1) * (unsigned long long)perSM;
-    cudaMemsetAsync(p.counter, 0, sizeof(unsigned long long), stream);
-    kernel<<<(unsigned)std::min(grid, (chunks + warps - 1ull) / warps), TB_QUERY_THREADS, 0, stream>>>(p);
+    unsigned long long needed;
+    if (bsdf) {
+        needed = ((unsigned long long)p.numRays + TB_QUERY_THREADS - 1ull) / TB_QUERY_THREADS;
+    } else {
+        const unsigned long long chunks = ((unsigned long long)p.numRays + 31ull) / 32ull;
+        const unsigned long long warps = (unsigned long long)TB_QUERY_THREADS / 32ull;
+        needed = (chunks + warps - 1ull) / warps;
+        cudaMemsetAsync(p.counter, 0, sizeof(unsigned long long), stream);
+    }
+    kernel<<<(unsigned)std::min(grid, needed), TB_QUERY_THREADS, 0, stream>>>(p);
     if (launchCount) ++*launchCount;
 }
