@@ -387,6 +387,40 @@ int tb200_bsdf_eval(tb200_renderer* r, const tb200_bsdf_query* q, tb200_bsdf_val
 int tb200_bsdf_sample(tb200_renderer* r, const tb200_bsdf_query* q, const uint32_t* seeds, tb200_bsdf_sampled* out,
                       int64_t n);
 
+/* ---- batched camera samples and film splats --------------------------------------------------
+ * The two ends of a path, for a caller's batch, exactly as the renderer runs them, so that a caller can trace the
+ * image's own samples (depth, normal or primitive maps aligned with the image; an integrator of its own) and put
+ * its own radiance into a film with the image's filter (custom AOVs; tb200_finish and tb200_nlm of its results).
+ *   tb200_camera_rays: per record i, the camera sample the renderer traces for pixel p = samples[i].pixel of a
+ *     W x H image (px = p % W, py = p / W) in frame samples[i].frame (any int32, read as its uint32 bits):
+ *     Random(tb200_sample_seed(p, frame)), then the draws x, y, t (src/render.cpp:476-482), time =
+ *     Lerp(shutterStart, shutterEnd, t) and GenerateRay(px + x, py + y) of the camera (src/util.h:45-83), bit for
+ *     bit.  rays[i] = {origin, time, dir, pad = +inf} (+inf: tb200_occluded_rays reads the same record as "anything
+ *     in front of the camera"); raster[2i..2i+1] = px + x, py + y, where the renderer splats that sample.  A pixel
+ *     outside [0, W*H) gives an all-zero ray (a miss for tb200_trace_rays) and a NaN raster (skipped by
+ *     tb200_splat).  Only options->width and options->height are read.
+ *   tb200_splat: per sample i, AddSample(raster[2i..2i+1], radiance[3i..3i+2]) (src/render.cpp:401-445) into
+ *     `accum`, W*H float4 running sums (sum w*rgb, sum w), added to what is there (the caller zeroes), with the
+ *     options' filter type, width, falloff, offset and clamp, over every row [0, H) (slab and shard settings do
+ *     not apply).  Filter options are refused as by the render calls.  A raster coordinate that is NaN or 2^30 or
+ *     more in magnitude is skipped (AddSample's int conversion is undefined there); every other sample is splatted
+ *     as the renderer splats it, including one outside the image whose footprint reaches in, and a non-finite
+ *     radiance, which poisons its footprint as in the reference.  The sums are formed in the order the reductions
+ *     reach memory, as the renderer's are.  accum = tb200_device_accumulator(r) puts the samples into the
+ *     renderer's own film, for tb200_finish, tb200_nlm and tb200_read_accumulator.
+ * All arrays are DEVICE memory of the renderer's device (a multi-device renderer: its head); alignment: samples 8
+ * bytes, rays 16, raster 8, radiance 4, accum 16; accum spans W*H*16 bytes whatever n is.  Refused before any
+ * launch, besides what tb200_trace_rays refuses (null pointers, n < 0, host or foreign-device memory, spans past
+ * the end of their allocation): null options or camera, width or height <= 0 and W*H > INT32_MAX.  The stream,
+ * synchronisation and side effects are tb200_trace_rays': needs no tb200_init; adds 1 to stats.kernelLaunches,
+ * sets stats.gpuMs to its kernel's time, and changes nothing else but `accum`.  n == 0 launches nothing.  Returns 0
+ * on success. */
+typedef struct tb200_camera_sample { int32_t pixel; int32_t frame; } tb200_camera_sample;   /* 8 B */
+int tb200_camera_rays(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options,
+                      const tb200_camera_sample* samples, tb200_ray* rays, float* raster, int64_t n);
+int tb200_splat(tb200_renderer* r, const tb200_options* options, const float* raster, const float* radiance,
+                float* accum, int64_t n);
+
 /* Sets the frame counter (frame k seeds sample k of every pixel). */
 void tb200_set_frame(tb200_renderer* r, int frame);
 

@@ -92,6 +92,11 @@ def load_library():
     lib.tb200_bsdf_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_bsdf_sample.restype = C.c_int
     lib.tb200_bsdf_sample.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_camera_rays.restype = C.c_int
+    lib.tb200_camera_rays.argtypes = [C.c_void_p, C.POINTER(Camera), C.POINTER(Options), C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_int64]
+    lib.tb200_splat.restype = C.c_int
+    lib.tb200_splat.argtypes = [C.c_void_p, C.POINTER(Options), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_set_frame.restype = None
     lib.tb200_set_frame.argtypes = [C.c_void_p, C.c_int]
     lib.tb200_get_stats.restype = None
@@ -164,6 +169,22 @@ def bsdf_queries(prims, n, v, eta_i, eta_o, l=None):
     put(8, l if l is not None else 0.0, 3, "l")
     put(11, eta_o, 1, "eta_o")
     return q
+
+
+def frame_samples(width, height, frame0, num_frames=1, device="cuda"):
+    """The (pixel, frame) records of whole frames for Renderer.camera_rays: an (num_frames * width * height, 2) int32
+    tensor on `device`, frames frame0, frame0 + 1, ... one after the other, each with its pixels in row-major order.
+    Frame numbers wrap as the renderer's int32 frame counter does."""
+    import torch
+    if width <= 0 or height <= 0 or num_frames < 0:
+        raise ValueError("frame_samples needs a positive width and height and num_frames >= 0, not %r, %r, %r"
+                         % (width, height, num_frames))
+    npix = width * height
+    frames = (torch.arange(num_frames, dtype=torch.int64) + int(frame0) + 2 ** 31) % 2 ** 32 - 2 ** 31
+    out = torch.empty((num_frames, npix, 2), dtype=torch.int32)
+    out[:, :, 0] = torch.arange(npix, dtype=torch.int32)
+    out[:, :, 1] = frames.to(torch.int32)[:, None]
+    return out.reshape(num_frames * npix, 2).to(device)
 
 
 def scene_cache_save(scene, path):
@@ -374,12 +395,12 @@ class Renderer:
         if not self._external_stream:
             torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()
 
-    def _query(self, entry, records, inputs, outputs):
+    def _query(self, entry, records, inputs, outputs, before=(), after=()):
         """What the batched queries share.  records: (tensor, name, width, dtype), the (N, width) records that set N;
         inputs: further input arrays and outputs: output arrays, each (tensor or None, name, shape after N, dtype).
         Checks them all, allocating on the head device the outputs not given (an input must be given); when N > 0,
-        waits for torch and calls the library's `entry` on the records, the inputs and the outputs, raising on a
-        refusal.  Returns the output tensors."""
+        waits for torch and calls the library's `entry` on the `before` arguments, the records, the inputs, the
+        outputs and the `after` arguments, raising on a refusal.  Returns the output tensors."""
         import torch
         x, name, width, dtype = records
         n = self._check_records(x, name, width, dtype)
@@ -395,7 +416,7 @@ class Renderer:
             out.append(y)
         if n > 0:
             self._wait_for_torch()
-            self._check(getattr(self.lib, entry)(self.h, *[y.data_ptr() for y in args + out], n), entry)
+            self._check(getattr(self.lib, entry)(self.h, *before, *[y.data_ptr() for y in args + out], *after, n), entry)
         return out
 
     def trace_rays(self, rays, hits=None, prims=None):
@@ -453,6 +474,42 @@ class Renderer:
         out, = self._query("tb200_bsdf_sample", (queries, "queries", 12, torch.float32), [(seeds, "seeds", (), torch.int32)],
                            [(out, "out", (8,), torch.float32)])
         return out[:, 0:3], out[:, 3], out[:, 4:7], out[:, 7].view(torch.int32)
+
+    def camera_rays(self, camera, options, samples, rays=None, raster=None):
+        """The renderer's camera sample of every (pixel, frame) record (tb200_camera_rays): Random(sample_seed(pixel,
+        frame)), the draws x, y, t (src/render.cpp:476-482) and GenerateRay through the camera of an options.width x
+        options.height image, bit for bit.  samples: (N, 2) int32 tensor on the head device, the pixel (row-major) and
+        the frame (frame_samples makes whole frames).  Returns (rays (N, 8) float32: origin.xyz, time, dir.xyz, +inf,
+        ready for trace_rays and occluded; raster (N, 2) float32: the position the renderer splats the sample at), in
+        `rays` / `raster` when given.  A pixel outside the image gives a zero ray and a NaN raster.  Stream behaviour
+        as for trace_rays."""
+        import torch
+        rays, raster = self._query("tb200_camera_rays", (samples, "samples", 2, torch.int32), [],
+                                   [(rays, "rays", (8,), torch.float32), (raster, "raster", (2,), torch.float32)],
+                                   before=(C.byref(camera), C.byref(options)))
+        return rays, raster
+
+    def splat(self, options, raster, radiance, accum=None):
+        """AddSample (src/render.cpp:401-445) of every sample into a film (tb200_splat), with the options' filter and
+        clamp, as the renderer splats its own samples.  raster (N, 2) and radiance (N, 3): float32 tensors on the head
+        device; a raster coordinate that is NaN or 2^30 or more in magnitude is skipped.  accum: a contiguous
+        (options.height, options.width, 4) float32 tensor on the head device, added to (the caller zeroes it); None:
+        the renderer's own accumulator, which finish(), nlm() and read_accumulator() then see, and options.width /
+        height must be those of the last Init.  Returns `accum` (None for the renderer's own).  Stream behaviour as
+        for trace_rays."""
+        import torch
+        W, H = options.width, options.height
+        if accum is None:
+            if (W, H) != (self.width, self.height) or not self.width:
+                raise ValueError("splat into the renderer's accumulator: options.width/height %dx%d differ from the last "
+                                 "Init (%dx%d)" % (W, H, self.width, self.height))
+            ptr = self.device_accumulator_ptr()
+        else:
+            self._check_tensor(accum, "accum", (H, W, 4), torch.float32)
+            ptr = accum.data_ptr()
+        self._query("tb200_splat", (raster, "raster", 2, torch.float32), [(radiance, "radiance", (3,), torch.float32)], [],
+                    before=(C.byref(options),), after=(C.c_void_p(ptr),))
+        return accum
 
     def set_frame(self, frame):
         self.lib.tb200_set_frame(self.h, frame)

@@ -1,6 +1,8 @@
 """ctypes mirrors of include/tinsel_b200.h (the C ABI).  Field order and types must match the header."""
 import ctypes as C
 
+import numpy as np
+
 c_float_p = C.POINTER(C.c_float)
 c_int_p = C.POINTER(C.c_int32)
 
@@ -176,6 +178,15 @@ class BsdfSampled(C.Structure):
 BSDF_REFLECTED, BSDF_TRANSMITTED, BSDF_SPECULAR = 0, 1, 2
 
 
+class CameraSample(C.Structure):
+    """tb200_camera_sample: one record of tb200_camera_rays, a pixel (row-major index) and a frame (8 bytes)."""
+    _fields_ = [("pixel", C.c_int32), ("frame", C.c_int32)]
+
+
+# tb200_camera_sample as a numpy record (Renderer.camera_rays takes the same records as an (N, 2) int32 tensor)
+CAMERA_SAMPLE_DTYPE = np.dtype([("pixel", "<i4"), ("frame", "<i4")])
+
+
 class BvhBuildInfo(C.Structure):
     _fields_ = [("numNodes", C.c_int32), ("rounds", C.c_int32), ("kernelLaunches", C.c_uint64), ("buildMs", C.c_double)]
 
@@ -221,6 +232,8 @@ EXPORTS = [
     "tb200_occluded_rays",
     "tb200_bsdf_eval",
     "tb200_bsdf_sample",
+    "tb200_camera_rays",
+    "tb200_splat",
     "tb200_set_frame",
     "tb200_get_stats",
     "tb200_last_kernel",

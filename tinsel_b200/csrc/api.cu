@@ -736,6 +736,25 @@ bool filter_options_ok(const tb200_options* o)
     return true;
 }
 
+// The film of options that filter_options_ok accepted: their image size, filter, clamp and path depth, over every
+// row [0, height).  The render calls (fill_params) and tb200_splat splat through it.
+DFilm film_setup(const tb200_options& o)
+{
+    DFilm f;
+    f.width = o.width;
+    f.height = o.height;
+    f.filterType = o.filterType;
+    f.filterWidth = o.filterWidth;
+    f.filterFalloff = o.filterFalloff;
+    f.filterOffset = o.filterOffset;
+    f.clamp = o.clamp;
+    f.maxDepth = o.maxDepth;
+    f.filterArgZero = film_filter_arg_zero(o.filterOffset);
+    f.rowLo = 0;
+    f.rowHi = o.height;
+    return f;
+}
+
 bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_options* o, LaunchParams* P)
 {
     if (!r->mem.accum) return set_error("tb200_init has not been called");
@@ -745,22 +764,12 @@ bool fill_params(tb200_renderer* r, const tb200_camera* camera, const tb200_opti
     memset(P, 0, sizeof(*P));
     P->scene = r->scene;
     camera_setup(*camera, o->width, o->height, &P->camera);
-    P->film.width = o->width;
-    P->film.height = o->height;
-    P->film.filterType = o->filterType;
-    P->film.filterWidth = o->filterWidth;
-    P->film.filterFalloff = o->filterFalloff;
-    P->film.filterOffset = o->filterOffset;
-    P->film.clamp = o->clamp;
-    P->film.maxDepth = o->maxDepth;
-    P->film.filterArgZero = film_filter_arg_zero(o->filterOffset);
+    P->film = film_setup(*o);
     P->accum = r->boundAccum ? r->boundAccum : r->mem.accum.get();
     P->sampleCounter = r->mem.counter.get();
     P->cold = r->mem.cold.get();
     P->firstRow = 0;
     P->numRows = o->height;
-    P->film.rowLo = 0;
-    P->film.rowHi = o->height;
     if (r->slabRows >= 0) {
         // owner-computes slab: trace the owned rows plus every row whose samples can reach them
         // (render.cpp:404-407: a sample of row y splats into rows int(y' - w) .. int(y' + w), y' in [y, y+1]),
@@ -1831,12 +1840,15 @@ static bool check_device_span(const char* entry, const tb200_renderer* r, const 
     return true;
 }
 
-// One array of a query, as the caller passed it: checked by check_device_span for `count` records
+// One array of a query, as the caller passed it: checked by check_device_span for `count` records of bytesPerItem
+// bytes, or, for an array whose size does not depend on the count (bytesPerItem 0, tb200_splat's film), for
+// fixedBytes bytes
 struct QuerySpan {
     const void* ptr;
     size_t bytesPerItem;
     size_t align;
     const char* what;   // its name in refusals
+    size_t fixedBytes = 0;
 };
 
 // Every batched query: checks the renderer, the record count (named `countName` in refusals), then the input and
@@ -1859,7 +1871,7 @@ static int run_query(const char* entry, tb200_renderer* r, QueryKind kind, const
     cudaSetDevice(r->device);   // a multi-device renderer answers on its head, which holds a full copy of the scene
     const size_t n = (size_t)count;
     for (const QuerySpan& s : spans)
-        if (!check_device_span(entry, r, s.ptr, n * s.bytesPerItem, s.align, s.what)) return -1;
+        if (!check_device_span(entry, r, s.ptr, s.bytesPerItem ? n * s.bytesPerItem : s.fixedBytes, s.align, s.what)) return -1;
     Q.scene = r->scene;
     Q.numRays = count;
     Q.counter = r->mem.counter.get();   // the wavefront's work counter: free between launches on this stream
@@ -1930,6 +1942,61 @@ int tb200_bsdf_sample(tb200_renderer* r, const tb200_bsdf_query* q, const uint32
     return run_query("tb200_bsdf_sample", r, QueryKind::BsdfSample, "n", n,
                      {{q, sizeof(tb200_bsdf_query), 16, "q"}, {seeds, sizeof(uint32_t), 4, "seeds"},
                       {out, sizeof(tb200_bsdf_sampled), 16, "out"}}, Q);
+}
+
+static_assert(sizeof(tb200_camera_sample) == 8, "the camera-ray kernel reads one int2 per sample");
+
+// The image of a camera-ray or splat call: options given, width and height positive, at most INT32_MAX pixels (the
+// kernels index pixels with int), and with `filter` the filter options the render calls accept.  Refusals name `entry`.
+static bool query_image_ok(const char* entry, const tb200_options* o, bool filter)
+{
+    const std::string e = std::string(entry) + ": ";
+    if (!o) return set_error(e + "options is null");
+    const std::string size = std::to_string(o->width) + " x " + std::to_string(o->height);
+    if (o->width <= 0 || o->height <= 0) return set_error(e + "options.width/height " + size + " are not both positive");
+    if ((int64_t)o->width * o->height > (int64_t)INT32_MAX) return set_error(e + "options.width/height " + size + " have more than 2^31-1 pixels");
+    if (filter && !filter_options_ok(o)) return set_error(e + tb200_last_error());
+    return true;
+}
+
+int tb200_camera_rays(tb200_renderer* r, const tb200_camera* camera, const tb200_options* options,
+                      const tb200_camera_sample* samples, tb200_ray* rays, float* raster, int64_t n)
+{
+    QueryParams Q = {};
+    if (r && n > 0) {
+        if (!query_image_ok("tb200_camera_rays", options, false)) return -1;
+        if (!camera) {
+            set_error("tb200_camera_rays: camera is null");
+            return -1;
+        }
+        camera_setup(*camera, options->width, options->height, &Q.camera);
+        Q.film.width = options->width;
+        Q.film.height = options->height;
+    }
+    Q.cameraSamples = reinterpret_cast<const int2*>(samples);
+    Q.cameraRays = reinterpret_cast<float4*>(rays);
+    Q.rasterOut = reinterpret_cast<float2*>(raster);
+    return run_query("tb200_camera_rays", r, QueryKind::CameraRays, "n", n,
+                     {{samples, sizeof(tb200_camera_sample), 8, "samples"}, {rays, sizeof(tb200_ray), 16, "rays"},
+                      {raster, 2 * sizeof(float), 8, "raster"}}, Q);
+}
+
+int tb200_splat(tb200_renderer* r, const tb200_options* options, const float* raster, const float* radiance, float* accum,
+                int64_t n)
+{
+    QueryParams Q = {};
+    size_t accumBytes = 0;
+    if (r && n > 0) {
+        if (!query_image_ok("tb200_splat", options, true)) return -1;
+        Q.film = film_setup(*options);
+        accumBytes = (size_t)options->width * (size_t)options->height * sizeof(float4);
+    }
+    Q.rasterIn = reinterpret_cast<const float2*>(raster);
+    Q.radiance = radiance;
+    Q.accum = reinterpret_cast<float4*>(accum);
+    return run_query("tb200_splat", r, QueryKind::Splat, "n", n,
+                     {{raster, 2 * sizeof(float), 8, "raster"}, {radiance, 3 * sizeof(float), 4, "radiance"},
+                      {accum, 0, 16, "accum", accumBytes}}, Q);
 }
 
 #ifdef TB_WF2_STAGE_CLOCKS

@@ -52,23 +52,16 @@ TB_DEV bool decode_sample(const LaunchParams& P, unsigned long long idx64, int& 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Shared per-sample prologue: seed Random per (pixel, frame), draw x,y,t in the oracle's order
-// (render.cpp:476-482), generate the camera ray.
+// Shared per-sample prologue: the camera sample of (pixel, frame) (tb_film.cuh: camera_sample), then the path's
+// start from its ray and the Random state after its draws.
 // ------------------------------------------------------------------------------------------------
 TB_DEV void sample_begin(const LaunchParams& P, int px, int py, int frame, PathState& ps, float& rasterX, float& rasterY)
 {
-    Rng rng = rng_seed(tb_sample_seed((uint32_t)(py * P.film.width + px), (uint32_t)frame));
-    float x = rng_float(rng);
-    float y = rng_float(rng);
-    const float t = rng_float(rng);
-    const float time = tb_lerp(P.camera.shutterStart, P.camera.shutterEnd, t);
-    x += px;
-    y += py;
+    Rng rng;
     V3 origin, dir;
-    generate_ray(P.camera, x, y, origin, dir);
+    float time;
+    camera_sample(P.camera, P.film.width, px, py, (uint32_t)frame, rng, origin, dir, time, rasterX, rasterY);
     path_init(ps, origin, dir, time, rng);
-    rasterX = x;
-    rasterY = y;
 }
 
 TB_DEV void sample_end(const LaunchParams& P, int px, int py, float rasterX, float rasterY, V3 radiance)

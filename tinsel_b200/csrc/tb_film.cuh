@@ -37,6 +37,25 @@ TB_DEV void generate_ray(const DCamera& cam, float rx, float ry, V3& origin, V3&
     dir = normalize(p - origin);
 }
 
+// The camera sample of pixel (px, py) in `frame` of a `width`-pixel-wide image (render.cpp:476-482, with the
+// per-(pixel, frame) seed): Random(tb_sample_seed(pixel, frame)), the draws x, y, t in the oracle's order, the shutter
+// time, and GenerateRay through the jittered raster position (rasterX, rasterY), which is also where the sample is
+// splatted.  `rng` is left after the three draws.  The renderer (sample_begin) and tb200_camera_rays both call this.
+TB_DEV void camera_sample(const DCamera& cam, int width, int px, int py, uint32_t frame, Rng& rng, V3& origin, V3& dir,
+                          float& time, float& rasterX, float& rasterY)
+{
+    rng = rng_seed(tb_sample_seed((uint32_t)(py * width + px), frame));
+    float x = rng_float(rng);
+    float y = rng_float(rng);
+    const float t = rng_float(rng);
+    time = tb_lerp(cam.shutterStart, cam.shutterEnd, t);
+    x += px;
+    y += py;
+    generate_ray(cam, x, y, origin, dir);
+    rasterX = x;
+    rasterY = y;
+}
+
 // DFilm::filterArgZero for a filter offset (host).  Gaussian() is exactly +0 wherever expf(arg) < offset; keep a
 // 1e-3 relative margin so the shortcut never depends on the last bits of expf.  -inf (shortcut off) unless the
 // offset lies in (0, 1) and tbm_expf confirms the cut-off.

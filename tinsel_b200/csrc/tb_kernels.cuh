@@ -129,13 +129,16 @@ struct NlmParams {
 void launch_nlm(const NlmParams& p, cudaStream_t stream, unsigned long long* launchCount);
 
 // The batched queries (tb_query.cuh): the ray queries, each Trace (render.cpp:17-62) of every ray of a caller's
-// batch, and the BSDF queries, one Disney BSDF call (disney.h) per query record:
+// batch; the BSDF queries, one Disney BSDF call (disney.h) per query record; and the two ends of a path, the
+// renderer's camera sample and the film's AddSample, per sample record:
 enum class QueryKind {
     Closest,      // tb200_trace_rays: the closest hit
     ClosestTri,   // tb200_trace_rays_tri: the closest hit and the winner's triangle and barycentric weights
     Occluded,     // tb200_occluded_rays: whether Trace hits something before the ray's tmax
     BsdfEval,     // tb200_bsdf_eval: BSDFEval and BSDFPdf
     BsdfSample,   // tb200_bsdf_sample: BSDFSample, then BSDFEval of the sampled direction
+    CameraRays,   // tb200_camera_rays: the camera ray and raster position of a (pixel, frame) sample
+    Splat,        // tb200_splat: AddSample of a caller's radiance at a raster position
 };
 // Every query's parameters.  The input and output pointers a query does not use stay null.
 struct QueryParams {
@@ -149,8 +152,17 @@ struct QueryParams {
     const uint32_t* seeds;      // BsdfSample: 1 per query: the Random seed
     float4* bsdfValues;         // BsdfEval: 1 per query: f.rgb, pdf
     float4* bsdfSamples;        // BsdfSample: 2 per query: l.xyz, pdf; f.rgb, type bits
-    long long numRays;    // records in the batch (rays or BSDF queries)
+    long long numRays;    // records in the batch (rays, BSDF queries or samples)
     unsigned long long* counter;   // work counter of the ray queries, cleared by the launch
+    // (the members below come after the others, so that the five kernels above keep their parameter offsets)
+    DCamera camera;       // CameraRays: the camera, set up for film.width x film.height
+    DFilm film;           // CameraRays: the image size; Splat: the film and its filter, rows [0, height)
+    const int2* cameraSamples;   // CameraRays: 1 per sample: pixel, frame
+    float4* cameraRays;          // CameraRays: 2 per sample: origin.xyz, time; dir.xyz, +inf
+    float2* rasterOut;           // CameraRays: 1 per sample: raster position
+    const float2* rasterIn;      // Splat: 1 per sample: raster position
+    const float* radiance;       // Splat: 3 per sample: rgb
+    float4* accum;               // Splat: film.width * film.height running sums
 };
 // Unlike the launches above, it leaves tb200_last_kernel alone and so returns no kernel name.
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);

@@ -2,7 +2,9 @@
 // render.cpp:17-62 for every ray of a caller's batch, bit for bit, through the same trace_closest() the
 // renderer runs; the same query reporting the hit triangle and its barycentric weights (tb200_trace_rays_tri); and
 // the batched occlusion query (tb200_occluded_rays) over trace_occluded(); and the batched BSDF queries
-// (tb200_bsdf_eval, tb200_bsdf_sample) over the renderer's Disney BSDF functions.  Included once, by kernels.cu.
+// (tb200_bsdf_eval, tb200_bsdf_sample) over the renderer's Disney BSDF functions; and the two ends of a path: the
+// renderer's camera samples (tb200_camera_rays, over camera_sample) and the film's splat (tb200_splat, over
+// add_sample_small).  Included once, by kernels.cu.
 //
 // The ray queries run a persistent kernel: as many CTAs as the SMs hold at once, for the whole batch.  Their warps
 // claim chunks of 32 rays from a global counter: a static split would leave SMs idle, because a ray that hits a plane
@@ -132,21 +134,68 @@ __global__ void __launch_bounds__(TB_QUERY_THREADS) k_bsdf_query(const __grid_co
     }
 }
 
+// The camera rays (QueryKind::CameraRays): per sample record (pixel, frame), what sample_begin computes for that
+// pixel in that frame (camera_sample), bit for bit.  A pixel outside [0, width*height) gets an all-zero ray, which
+// trace_rays answers with a miss, and a NaN raster position, which k_splat skips.  Grid-stride, one sample per
+// thread: one 8-byte load, three streaming stores.
+__global__ void __launch_bounds__(TB_QUERY_THREADS) k_camera_rays(const __grid_constant__ QueryParams P)
+{
+    const unsigned long long n = (unsigned long long)P.numRays;
+    const unsigned long long stride = (unsigned long long)gridDim.x * TB_QUERY_THREADS;
+    const int W = P.film.width;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * TB_QUERY_THREADS + threadIdx.x; i < n; i += stride) {
+        const int2 s = __ldg(&P.cameraSamples[i]);   // pixel, frame
+        float4 a = make_float4(0.0f, 0.0f, 0.0f, 0.0f), b = a;
+        float2 raster = make_float2(__int_as_float(0x7fffffff), __int_as_float(0x7fffffff));
+        if (s.x >= 0 && s.x < W * P.film.height) {   // the host refuses images of more than INT32_MAX pixels
+            Rng rng;
+            V3 o, d;
+            float time;
+            camera_sample(P.camera, W, s.x % W, s.x / W, (uint32_t)s.y, rng, o, d, time, raster.x, raster.y);
+            a = make_float4(o.x, o.y, o.z, time);
+            b = make_float4(d.x, d.y, d.z, __int_as_float(0x7f800000));   // +inf: occluded_rays reads it as tmax
+        }
+        __stcs(&P.cameraRays[2 * i], a);
+        __stcs(&P.cameraRays[2 * i + 1], b);
+        __stcs(&P.rasterOut[i], raster);
+    }
+}
+
+// The splat (QueryKind::Splat): per sample, AddSample (render.cpp:401-445) of its radiance at its raster position
+// into P.accum through add_sample_small, the lane-owned wavefront kernel's splat, over every row of the film.  A
+// raster coordinate that is NaN or 2^30 or more in magnitude is skipped: AddSample's int conversion of
+// raster +- filterWidth is undefined there (the host has refused filter widths of 2^30 or more).  Grid-stride, one
+// sample per thread; the reductions go to L2 (tb_film.cuh: accum_add).
+__global__ void __launch_bounds__(TB_QUERY_THREADS) k_splat(const __grid_constant__ QueryParams P)
+{
+    const unsigned long long n = (unsigned long long)P.numRays;
+    const unsigned long long stride = (unsigned long long)gridDim.x * TB_QUERY_THREADS;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * TB_QUERY_THREADS + threadIdx.x; i < n; i += stride) {
+        const float2 r = __ldg(&P.rasterIn[i]);
+        if (!(fabsf(r.x) < 1073741824.0f && fabsf(r.y) < 1073741824.0f)) continue;
+        const V3 c = v3(__ldg(&P.radiance[3 * i]), __ldg(&P.radiance[3 * i + 1]), __ldg(&P.radiance[3 * i + 2]));
+        add_sample_small(P.film, P.accum, r.x, r.y, c);
+    }
+}
+
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
     if (p.numRays <= 0) return;
-    const bool bsdf = kind == QueryKind::BsdfEval || kind == QueryKind::BsdfSample;
+    const bool perThread = kind != QueryKind::Closest && kind != QueryKind::ClosestTri && kind != QueryKind::Occluded;
     void (*kernel)(QueryParams) = kind == QueryKind::Closest      ? k_trace_rays<false>
                                   : kind == QueryKind::ClosestTri ? k_trace_rays<true>
                                   : kind == QueryKind::Occluded   ? k_occluded_rays
                                   : kind == QueryKind::BsdfEval   ? k_bsdf_query<false>
-                                                                  : k_bsdf_query<true>;
-    // as many CTAs as the SMs hold at once, but no more than there are 32-ray chunks (BSDF queries: one per thread)
+                                  : kind == QueryKind::BsdfSample ? k_bsdf_query<true>
+                                  : kind == QueryKind::CameraRays ? k_camera_rays
+                                                                  : k_splat;
+    // as many CTAs as the SMs hold at once, but no more than there are 32-ray chunks (the grid-stride queries: one
+    // record per thread)
     int perSM = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kernel, TB_QUERY_THREADS, 0) != cudaSuccess || perSM < 1) perSM = 1;
     const unsigned long long grid = (unsigned long long)(numSMs > 0 ? numSMs : 1) * (unsigned long long)perSM;
     unsigned long long needed;
-    if (bsdf) {
+    if (perThread) {
         needed = ((unsigned long long)p.numRays + TB_QUERY_THREADS - 1ull) / TB_QUERY_THREADS;
     } else {
         const unsigned long long chunks = ((unsigned long long)p.numRays + 31ull) / 32ull;
