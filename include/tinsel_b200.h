@@ -421,6 +421,41 @@ int tb200_camera_rays(tb200_renderer* r, const tb200_camera* camera, const tb200
 int tb200_splat(tb200_renderer* r, const tb200_options* options, const float* raster, const float* radiance,
                 float* accum, int64_t n);
 
+/* ---- batched next-event estimation and sky queries -------------------------------------------
+ * The two stages of PathTrace (src/render.cpp:230-388) the queries above leave out, for a caller's batch:
+ *   tb200_sample_lights: per query i, radiance[3i..3i+2] = SampleLights(scene, prims[prim], etaI, etaO, p, n, wo,
+ *     time, Random(seeds[i])) (src/render.cpp:103-227), bit for bit (a NaN may have another payload): the probe
+ *     sample and its shadow ray when the sky has a probe, then for every primitive with lightSamples > 0, in scene
+ *     order, its samples, each with a full closest-hit Trace shadow ray at `time`, the |t - dist| <= 1e-2
+ *     acceptance, the light-normal test and the balance-heuristic MIS, weighted by the emission of whatever the
+ *     shadow ray hit.  That is the `sum` PathTrace multiplies by the path throughput; PathTrace calls it at every
+ *     hit, a hit on a light included.  The record follows PathTrace's convention: p the hit point, n the shading
+ *     normal as tb200_trace_rays returns it (face-forwarded), wo = -dir of the incoming ray, and the etas of
+ *     tb200_bsdf_eval; all are used as given, never normalised, and the etas may take any value.  The BSDF is the
+ *     material the path tracer shades `prim` with.  A prim outside [0, numPrimitives) gives zeros and traces
+ *     nothing, so the prims of tb200_trace_rays can be passed straight through on misses (-1).  The three floats
+ *     per query are the layout tb200_splat reads its radiance in.  `time` must be finite, as the renderer's own
+ *     ray times are: the device takes a static primitive's transform as it is, where the reference interpolates it
+ *     and a NaN or infinite time would make it NaN; any finite time, inside the shutter or not, is exact.
+ *   tb200_sky_eval: per ray i (only rays[i].dir is read, so the records of tb200_trace_rays and tb200_camera_rays can
+ *     be passed as they are), out[4i..4i+2] = Sky::Eval(dir) (src/scene.h:168-178) and out[4i+3] = ProbePdf(dir)
+ *     (src/probe.h:136-160) when the sky has a probe, else 0; bit for bit.  The miss branch's MIS weight
+ *     (src/render.cpp:365-384) depends on path state and stays with the caller.
+ * All arrays are DEVICE memory of the renderer's device (a multi-device renderer: its head); alignment: q and rays
+ * 16 bytes, seeds 4, radiance 4, out 16.  The refusals, stream, synchronisation and side effects are
+ * tb200_trace_rays': null pointers, n < 0, host or foreign-device memory and spans past the end of their
+ * allocation are refused before any launch; needs no tb200_init; adds 1 to stats.kernelLaunches, sets stats.gpuMs
+ * to its kernel's time, and touches nothing else.  n == 0 launches nothing.  Returns 0 on success. */
+typedef struct tb200_light_query {   /* 64 B */
+    float p[3];  float time;     /* surface point; ray time (motion blur of the lights and the shadow rays) */
+    float n[3];  int32_t prim;   /* shading normal as trace_rays returns it (face-forwarded); surface primitive */
+    float wo[3]; float etaI;     /* towards the viewer (-dir of the incoming ray) */
+    float etaO;  float pad[3];
+} tb200_light_query;
+int tb200_sample_lights(tb200_renderer* r, const tb200_light_query* q, const uint32_t* seeds, float* radiance,
+                        int64_t n);
+int tb200_sky_eval(tb200_renderer* r, const tb200_ray* rays, float* out, int64_t n);
+
 /* Sets the frame counter (frame k seeds sample k of every pixel). */
 void tb200_set_frame(tb200_renderer* r, int frame);
 

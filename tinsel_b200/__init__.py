@@ -97,6 +97,10 @@ def load_library():
                                       C.c_int64]
     lib.tb200_splat.restype = C.c_int
     lib.tb200_splat.argtypes = [C.c_void_p, C.POINTER(Options), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_sample_lights.restype = C.c_int
+    lib.tb200_sample_lights.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_sky_eval.restype = C.c_int
+    lib.tb200_sky_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_set_frame.restype = None
     lib.tb200_set_frame.argtypes = [C.c_void_p, C.c_int]
     lib.tb200_get_stats.restype = None
@@ -148,27 +152,56 @@ def bsdf_queries(prims, n, v, eta_i, eta_o, l=None):
     device with n.xyz, the int32 primitive's bits, v.xyz, etaI, l.xyz, etaO per row.  prims: (N,) int32 tensor
     (trace_rays' prims can be passed as they are); n, v, l: (N, 3) float32 tensors (l None: zeros, which sampling
     ignores); eta_i, eta_o: (N,) float32 tensors or Python numbers."""
+    return _pack_records(prims, 12, 3, [(0, n, 3, "n"), (4, v, 3, "v"), (7, eta_i, 1, "eta_i"),
+                                        (8, l if l is not None else 0.0, 3, "l"), (11, eta_o, 1, "eta_o")])
+
+
+def light_queries(prims, p, n, wo, eta_i, eta_o, time):
+    """Packs tb200_light_query records for Renderer.sample_lights: an (N, 16) float32 tensor on `prims`' device with
+    p.xyz, time, n.xyz, the int32 primitive's bits, wo.xyz, etaI, etaO and three zeros per row.  prims: (N,) int32
+    tensor (trace_rays' prims can be passed as they are); p, n, wo: (N, 3) float32 tensors (the hit point, the normal
+    trace_rays returns and -dir of the incoming ray); eta_i, eta_o, time: (N,) float32 tensors or Python numbers."""
+    return _pack_records(prims, 16, 7, [(0, p, 3, "p"), (3, time, 1, "time"), (4, n, 3, "n"), (8, wo, 3, "wo"),
+                                        (11, eta_i, 1, "eta_i"), (12, eta_o, 1, "eta_o"), (13, 0.0, 3, "pad")])
+
+
+def _pack_records(prims, width, prim_col, fields):
+    """An (N, width) float32 tensor on `prims`' device with the int32 prims' bits in column prim_col and each field
+    (col, x, cols, name) in columns [col, col + cols): x a float32 tensor of shape (N, cols), or (N,) for one column,
+    or a Python number for every row."""
     import torch
     if not isinstance(prims, torch.Tensor) or prims.dtype != torch.int32 or prims.dim() != 1:
         raise ValueError("prims must be an (N,) int32 tensor")
     count, dev = prims.shape[0], prims.device
-    q = torch.empty((count, 12), dtype=torch.float32, device=dev)
-
-    def put(col, x, width, name):
+    q = torch.empty((count, width), dtype=torch.float32, device=dev)
+    for col, x, cols, name in fields:
         if not isinstance(x, torch.Tensor):
-            q[:, col:col + width] = float(x)
-            return
-        if x.dtype != torch.float32 or tuple(x.shape) != ((count, width) if width > 1 else (count,)):
-            raise ValueError("%s must be a float32 tensor of shape %s" % (name, (count, width) if width > 1 else (count,)))
-        q[:, col:col + width] = x.to(dev).reshape(count, width)
-
-    put(0, n, 3, "n")
-    q[:, 3] = prims.view(torch.float32)
-    put(4, v, 3, "v")
-    put(7, eta_i, 1, "eta_i")
-    put(8, l if l is not None else 0.0, 3, "l")
-    put(11, eta_o, 1, "eta_o")
+            q[:, col:col + cols] = float(x)
+            continue
+        shape = (count, cols) if cols > 1 else (count,)
+        if x.dtype != torch.float32 or tuple(x.shape) != shape:
+            raise ValueError("%s must be a float32 tensor of shape %s" % (name, shape))
+        q[:, col:col + cols] = x.to(dev).reshape(count, cols)
+    q[:, prim_col] = prims.view(torch.float32)
     return q
+
+
+def primitive_areas(scene):
+    """PrimitiveArea (src/intersection.h:833-853) of every primitive of `scene` (a tb200_scene or a pointer to one),
+    as the renderer computes it in float32: 4 pi r^2 for a sphere, the mesh's area times the end transform's scale
+    for a mesh, 0 for a plane.  With a primitive's lightSamples and emission, it is what PathTrace's emission MIS
+    weight at a hit needs (src/render.cpp:255-310).  Returns an (numPrimitives,) float32 numpy array."""
+    sc = scene.contents if isinstance(scene, C._Pointer) else scene
+    out = np.zeros(sc.numPrimitives, np.float32)
+    pi = np.float32(3.14159265358979323846)
+    for i in range(sc.numPrimitives):
+        p = sc.primitives[i]
+        if p.type == abi.SPHERE:
+            r = np.float32(p.radius)
+            out[i] = np.float32(4) * pi * r * r
+        elif p.type == abi.MESH:
+            out[i] = np.float32(sc.meshes[p.mesh].area) * np.float32(p.end.s)
+    return out
 
 
 def frame_samples(width, height, frame0, num_frames=1, device="cuda"):
@@ -510,6 +543,27 @@ class Renderer:
         self._query("tb200_splat", (raster, "raster", 2, torch.float32), [(radiance, "radiance", (3,), torch.float32)], [],
                     before=(C.byref(options),), after=(C.c_void_p(ptr),))
         return accum
+
+    def sample_lights(self, queries, seeds, out=None):
+        """Next-event estimation at every surface record (tb200_sample_lights): SampleLights (src/render.cpp:103-227)
+        with Random(seed), bit for bit -- the probe sample, every light's samples with their closest-hit shadow rays
+        and MIS -- the `sum` PathTrace multiplies by the throughput at a hit.  queries: contiguous float32 CUDA tensor
+        (N, 16) on the head device, the tb200_light_query records (light_queries packs them); seeds: (N,) int32
+        tensor whose bits are the uint32 seeds.  Returns (N, 3) float32 radiance, `out` when given; a prim outside
+        the scene gives zeros.  Stream behaviour as for trace_rays."""
+        import torch
+        out, = self._query("tb200_sample_lights", (queries, "queries", 16, torch.float32),
+                           [(seeds, "seeds", (), torch.int32)], [(out, "out", (3,), torch.float32)])
+        return out
+
+    def sky(self, rays, out=None, split=False):
+        """The sky of a miss for every ray (tb200_sky_eval): Sky::Eval(dir) (src/scene.h:168-178) and ProbePdf(dir)
+        (src/probe.h:136-160), 0 without a probe, bit for bit.  rays: as for trace_rays, of which only dir is read.
+        Returns (N, 4) float32: rgb, pdf, in `out` when given; with split, (rgb (N, 3), pdf (N,)) views of it.  The
+        miss's MIS weight depends on path state and is the caller's.  Stream behaviour as for trace_rays."""
+        import torch
+        out, = self._query("tb200_sky_eval", (rays, "rays", 8, torch.float32), [], [(out, "out", (4,), torch.float32)])
+        return (out[:, :3], out[:, 3]) if split else out
 
     def set_frame(self, frame):
         self.lib.tb200_set_frame(self.h, frame)

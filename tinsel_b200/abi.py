@@ -183,6 +183,12 @@ class CameraSample(C.Structure):
     _fields_ = [("pixel", C.c_int32), ("frame", C.c_int32)]
 
 
+class LightQuery(C.Structure):
+    """tb200_light_query: one query of tb200_sample_lights, a surface point as PathTrace reaches it (64 bytes)."""
+    _fields_ = [("p", C.c_float * 3), ("time", C.c_float), ("n", C.c_float * 3), ("prim", C.c_int32),
+                ("wo", C.c_float * 3), ("etaI", C.c_float), ("etaO", C.c_float), ("pad", C.c_float * 3)]
+
+
 # tb200_camera_sample as a numpy record (Renderer.camera_rays takes the same records as an (N, 2) int32 tensor)
 CAMERA_SAMPLE_DTYPE = np.dtype([("pixel", "<i4"), ("frame", "<i4")])
 
@@ -234,6 +240,8 @@ EXPORTS = [
     "tb200_bsdf_sample",
     "tb200_camera_rays",
     "tb200_splat",
+    "tb200_sample_lights",
+    "tb200_sky_eval",
     "tb200_set_frame",
     "tb200_get_stats",
     "tb200_last_kernel",

@@ -1999,6 +1999,28 @@ int tb200_splat(tb200_renderer* r, const tb200_options* options, const float* ra
                       {accum, 0, 16, "accum", accumBytes}}, Q);
 }
 
+static_assert(sizeof(tb200_light_query) == 64, "the NEE query kernel reads four float4 per query");
+
+int tb200_sample_lights(tb200_renderer* r, const tb200_light_query* q, const uint32_t* seeds, float* radiance, int64_t n)
+{
+    QueryParams Q = {};
+    Q.lightQueries = reinterpret_cast<const float4*>(q);
+    Q.seeds = seeds;
+    Q.lightRadiance = radiance;
+    return run_query("tb200_sample_lights", r, QueryKind::SampleLights, "n", n,
+                     {{q, sizeof(tb200_light_query), 16, "q"}, {seeds, sizeof(uint32_t), 4, "seeds"},
+                      {radiance, 3 * sizeof(float), 4, "radiance"}}, Q);
+}
+
+int tb200_sky_eval(tb200_renderer* r, const tb200_ray* rays, float* out, int64_t n)
+{
+    QueryParams Q = {};
+    Q.rays = reinterpret_cast<const float4*>(rays);
+    Q.skyOut = reinterpret_cast<float4*>(out);
+    return run_query("tb200_sky_eval", r, QueryKind::Sky, "n", n,
+                     {{rays, sizeof(tb200_ray), 16, "rays"}, {out, 4 * sizeof(float), 16, "out"}}, Q);
+}
+
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds only (-DTB_WF2_STAGE_CLOCKS, tools/stage_clocks.py): copies the lane-owned wavefront
 // layout's per-stage cycle counters of the current device into out[0..n) (n >= 15 words, see wf2_lanes.cuh:

@@ -129,8 +129,9 @@ struct NlmParams {
 void launch_nlm(const NlmParams& p, cudaStream_t stream, unsigned long long* launchCount);
 
 // The batched queries (tb_query.cuh): the ray queries, each Trace (render.cpp:17-62) of every ray of a caller's
-// batch; the BSDF queries, one Disney BSDF call (disney.h) per query record; and the two ends of a path, the
-// renderer's camera sample and the film's AddSample, per sample record:
+// batch; the BSDF queries, one Disney BSDF call (disney.h) per query record; the two ends of a path, the
+// renderer's camera sample and the film's AddSample, per sample record; and the light queries, SampleLights per
+// surface record and the sky of a miss per ray:
 enum class QueryKind {
     Closest,      // tb200_trace_rays: the closest hit
     ClosestTri,   // tb200_trace_rays_tri: the closest hit and the winner's triangle and barycentric weights
@@ -139,6 +140,8 @@ enum class QueryKind {
     BsdfSample,   // tb200_bsdf_sample: BSDFSample, then BSDFEval of the sampled direction
     CameraRays,   // tb200_camera_rays: the camera ray and raster position of a (pixel, frame) sample
     Splat,        // tb200_splat: AddSample of a caller's radiance at a raster position
+    SampleLights, // tb200_sample_lights: SampleLights (next-event estimation) at a surface point
+    Sky,          // tb200_sky_eval: Sky::Eval and ProbePdf of a direction
 };
 // Every query's parameters.  The input and output pointers a query does not use stay null.
 struct QueryParams {
@@ -163,6 +166,10 @@ struct QueryParams {
     const float2* rasterIn;      // Splat: 1 per sample: raster position
     const float* radiance;       // Splat: 3 per sample: rgb
     float4* accum;               // Splat: film.width * film.height running sums
+    // (and these after those, so that the seven kernels above keep theirs)
+    const float4* lightQueries;  // SampleLights: 4 per query: p.xyz, time; n.xyz, prim bits; wo.xyz, etaI; etaO, pad
+    float* lightRadiance;        // SampleLights: 3 per query: rgb (seeds: 1 per query, the Random seed)
+    float4* skyOut;              // Sky: 1 per ray (of rays, whose dir alone is read): Sky::Eval rgb, ProbePdf
 };
 // Unlike the launches above, it leaves tb200_last_kernel alone and so returns no kernel name.
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);

@@ -4,11 +4,12 @@
 // the batched occlusion query (tb200_occluded_rays) over trace_occluded(); and the batched BSDF queries
 // (tb200_bsdf_eval, tb200_bsdf_sample) over the renderer's Disney BSDF functions; and the two ends of a path: the
 // renderer's camera samples (tb200_camera_rays, over camera_sample) and the film's splat (tb200_splat, over
-// add_sample_small).  Included once, by kernels.cu.
+// add_sample_small); and the light queries: next-event estimation (tb200_sample_lights, over nee_generate and
+// nee_connect) and the sky of a miss (tb200_sky_eval, over sky_eval and probe_pdf).  Included once, by kernels.cu.
 //
-// The ray queries run a persistent kernel: as many CTAs as the SMs hold at once, for the whole batch.  Their warps
-// claim chunks of 32 rays from a global counter: a static split would leave SMs idle, because a ray that hits a plane
-// costs a few dozen instructions and one that walks a deep mesh BVH more than ten times that.
+// The ray queries and the NEE query run a persistent kernel: as many CTAs as the SMs hold at once, for the whole
+// batch.  Their warps claim chunks of 32 records from a global counter: a static split would leave SMs idle, because
+// a ray that hits a plane costs a few dozen instructions and one that walks a deep mesh BVH more than ten times that.
 
 #define TB_QUERY_THREADS 256
 
@@ -16,11 +17,11 @@
 // per-thread copy would live in local memory.  The scene tables stay in global memory: staging the primitive
 // records, scene-level BVH pairs and flat scene program in shared memory with TMA bulk copies, as k_wavefront2 does,
 // measured no faster (DESIGN §5.6).  No mesh treelet either (the host leaves DScene::treelet null).
-// Then one atomic per warp claims 32 consecutive rays; each lane loads its ray (two 16-byte loads) and hands it to
-// ray(sc, i, a, b), which writes its answer with streaming stores, so that the outputs do not evict mesh BVH lines
-// from L2.
-template <class Ray>
-static __device__ __forceinline__ void query_claim_rays(const QueryParams& P, Ray ray)
+// Then one atomic per warp claims 32 consecutive records, and each lane hands its record's index to
+// record(sc, i), which loads the record and writes its answer with streaming stores, so that the outputs do not
+// evict mesh BVH lines from L2.
+template <class Record>
+static __device__ __forceinline__ void query_claim(const QueryParams& P, Record record)
 {
     __shared__ struct { DScene scene; } S;
     if (threadIdx.x == 0) S.scene = P.scene;
@@ -34,8 +35,15 @@ static __device__ __forceinline__ void query_claim_rays(const QueryParams& P, Ra
         base = __shfl_sync(0xffffffffu, base, 0);
         if (base >= n) break;
         const unsigned long long i = base + (unsigned long long)lane;
-        if (i < n) ray(S.scene, i, __ldg(&P.rays[2 * i]), __ldg(&P.rays[2 * i + 1]));
+        if (i < n) record(S.scene, i);
     }
+}
+
+// query_claim over the ray records: each lane loads its ray (two 16-byte loads) and hands it to ray(sc, i, a, b).
+template <class Ray>
+static __device__ __forceinline__ void query_claim_rays(const QueryParams& P, Ray ray)
+{
+    query_claim(P, [&](const DScene& sc, unsigned long long i) { ray(sc, i, __ldg(&P.rays[2 * i]), __ldg(&P.rays[2 * i + 1])); });
 }
 
 // Closest hit (QueryKind::Closest) and, with TRI, closest hit with the hit triangle (QueryKind::ClosestTri):
@@ -178,17 +186,83 @@ __global__ void __launch_bounds__(TB_QUERY_THREADS) k_splat(const __grid_constan
     }
 }
 
+// Next-event estimation (QueryKind::SampleLights): per surface record, SampleLights (render.cpp:103-227) from
+// Random(seed), bit for bit, through k_mega's NEE loop: nee_begin, nee_generate over every primitive, a closest-hit
+// shadow trace per sample and nee_connect.  The result is `sum`, which PathTrace multiplies by the throughput.  A
+// prim outside [0, numPrims) gives zeros and traces nothing.  Every query of a scene takes the same number of shadow
+// rays, but their walks differ in cost as the ray queries' do, so the records are claimed as rays are.
+// The BSDF evaluations run on a copy of the surface's material with TB_MAT_NO_FRESNEL and TB_MAT_NO_CLEARCOAT
+// cleared, as in k_bsdf_query and for the same reason: a caller may pass any etas and vectors.  bsdf_eval_pdf()
+// takes that copy by reference and is out of line, so the copy lives in the kernel's local frame (DESIGN §5.11).
+__global__ void __launch_bounds__(TB_QUERY_THREADS) k_sample_lights(const __grid_constant__ QueryParams P)
+{
+    query_claim(P, [&](const DScene& sc, unsigned long long i) {
+        // a: p.xyz, time; b: n.xyz, prim bits; c: wo.xyz, etaI; d: etaO, pad
+        const float4 a = __ldg(&P.lightQueries[4 * i]), b = __ldg(&P.lightQueries[4 * i + 1]);
+        const float4 c = __ldg(&P.lightQueries[4 * i + 2]), d = __ldg(&P.lightQueries[4 * i + 3]);
+        const int prim = __float_as_int(b.w);
+        NeeCursor cur;
+        nee_begin(cur);
+        if (prim >= 0 && prim < sc.numPrims) {
+            Surface sf;
+            sf.prim = prim;
+            sf.p = v3(a.x, a.y, a.z);
+            sf.n = v3(b.x, b.y, b.z);
+            sf.wo = v3(c.x, c.y, c.z);
+            sf.etaI = c.w;
+            sf.etaO = d.x;
+            sf.outAbsorb = v3s(0.0f);   // not read by NEE
+            DMaterial mat = sc.prims[prim].mat;
+            mat.flags &= ~(uint32_t)(TB_MAT_NO_FRESNEL | TB_MAT_NO_CLEARCOAT);
+            Rng rng = rng_seed(__ldg(&P.seeds[i]));
+            ShadowRay sr;
+            while (nee_generate(sc, sf, a.w, cur, rng, sr)) {
+                const Hit sh = trace_closest<TB_FEAT_ALL>(sc, sr.o, sr.d, a.w, false);
+                nee_connect(sc, sf, sr, sh, cur, nullptr, &mat);
+            }
+        }
+        __stcs(&P.lightRadiance[3 * i], cur.sum.x);
+        __stcs(&P.lightRadiance[3 * i + 1], cur.sum.y);
+        __stcs(&P.lightRadiance[3 * i + 2], cur.sum.z);
+    });
+}
+
+// The sky of a miss (QueryKind::Sky): per ray, Sky::Eval(dir) and ProbePdf(dir) (scene.h:168-178, probe.h:136-160),
+// bit for bit, with one ProbeDirToUV shared by both as in path_miss; pdf 0 for the gradient sky.  Only dir is read.
+// Every query costs the same, so grid-stride, one ray per thread: one 16-byte load, one streaming store.
+__global__ void __launch_bounds__(TB_QUERY_THREADS) k_sky(const __grid_constant__ QueryParams P)
+{
+    const unsigned long long n = (unsigned long long)P.numRays;
+    const unsigned long long stride = (unsigned long long)gridDim.x * TB_QUERY_THREADS;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * TB_QUERY_THREADS + threadIdx.x; i < n; i += stride) {
+        const float4 b = __ldg(&P.rays[2 * i + 1]);   // dir.xyz, pad
+        const V3 dir = v3(b.x, b.y, b.z);
+        float u = 0.0f, v = 0.0f, pdf = 0.0f;
+        if (P.scene.probe.valid) {
+            const float2 uv = probe_dir_to_uv(dir);
+            u = uv.x;
+            v = uv.y;
+            pdf = probe_pdf(P.scene.probe, u, v);
+        }
+        const V3 c = sky_eval<TB_FEAT_ALL>(P.scene, dir, u, v);
+        __stcs(&P.skyOut[i], make_float4(c.x, c.y, c.z, pdf));
+    }
+}
+
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
     if (p.numRays <= 0) return;
-    const bool perThread = kind != QueryKind::Closest && kind != QueryKind::ClosestTri && kind != QueryKind::Occluded;
-    void (*kernel)(QueryParams) = kind == QueryKind::Closest      ? k_trace_rays<false>
-                                  : kind == QueryKind::ClosestTri ? k_trace_rays<true>
-                                  : kind == QueryKind::Occluded   ? k_occluded_rays
-                                  : kind == QueryKind::BsdfEval   ? k_bsdf_query<false>
-                                  : kind == QueryKind::BsdfSample ? k_bsdf_query<true>
-                                  : kind == QueryKind::CameraRays ? k_camera_rays
-                                                                  : k_splat;
+    const bool perThread = kind != QueryKind::Closest && kind != QueryKind::ClosestTri && kind != QueryKind::Occluded &&
+                           kind != QueryKind::SampleLights;
+    void (*kernel)(QueryParams) = kind == QueryKind::Closest        ? k_trace_rays<false>
+                                  : kind == QueryKind::ClosestTri   ? k_trace_rays<true>
+                                  : kind == QueryKind::Occluded     ? k_occluded_rays
+                                  : kind == QueryKind::BsdfEval     ? k_bsdf_query<false>
+                                  : kind == QueryKind::BsdfSample   ? k_bsdf_query<true>
+                                  : kind == QueryKind::CameraRays   ? k_camera_rays
+                                  : kind == QueryKind::Splat        ? k_splat
+                                  : kind == QueryKind::SampleLights ? k_sample_lights
+                                                                    : k_sky;
     // as many CTAs as the SMs hold at once, but no more than there are 32-ray chunks (the grid-stride queries: one
     // record per thread)
     int perSM = 0;

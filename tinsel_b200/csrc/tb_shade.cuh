@@ -650,11 +650,14 @@ TB_DEV bool nee_generate(const DScene& sc, const Surface& sf, float time, NeeCur
 
 // Consumes the traced shadow ray of the slot generated last; accumulates into the cursor in the
 // reference's order (render.cpp:122-143 for the probe, :176-224 for area lights).  view: bsdf_view() of the surface,
-// where the caller keeps it for the whole bounce (nullptr: each BSDF evaluation computes its own).
+// where the caller keeps it for the whole bounce (nullptr: each BSDF evaluation computes its own).  surfaceMat: the
+// material the BSDF evaluations use (nullptr: the surface primitive's own; tb200_sample_lights passes a copy with
+// the Fresnel and clearcoat skips cleared, tb_query.cuh: k_sample_lights).
 template <uint32_t FEAT = TB_FEAT_ALL>
-TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr, const Hit& sh, NeeCursor& c, const BsdfView* view = nullptr)
+TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr, const Hit& sh, NeeCursor& c, const BsdfView* view = nullptr,
+                        const DMaterial* surfaceMat = nullptr)
 {
-    const DMaterial& mat = sc.prims[sf.prim].mat;
+    const DMaterial& mat = surfaceMat ? *surfaceMat : sc.prims[sf.prim].mat;
     const bool isProbe = (FEAT & TB_FEAT_PROBE) && sr.light < 0;   // only the probe sample has no light
     // decide first whether BSDFPdf/BSDFEval are needed at all (both are pure), then evaluate them
     // once for whichever kind of sample this is
