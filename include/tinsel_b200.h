@@ -456,6 +456,38 @@ int tb200_sample_lights(tb200_renderer* r, const tb200_light_query* q, const uin
                         int64_t n);
 int tb200_sky_eval(tb200_renderer* r, const tb200_ray* rays, float* out, int64_t n);
 
+/* ---- batched emitter and probe samples -------------------------------------------------------
+ * The two draws SampleLights makes its light samples from, for a caller's batch, so that a caller can build a
+ * light estimator of its own (one light picked by power, resampled candidates, the power heuristic, the start
+ * points of light paths):
+ *   tb200_sample_emitters: per query i, PrimitiveSample(primitives[prim], time, pos, normal, Random(seeds[i]))
+ *     (src/intersection.h:855-904), bit for bit (a NaN may have another payload).  A sphere draws 2 numbers; a
+ *     mesh draws 4: the triangle from the mesh's area CDF, UniformSampleTriangle's two, at the instance transform
+ *     of `time`.  Only the primitives SampleLights samples are sampled: those with lightSamples > 0 (tb200_create
+ *     refuses a mesh light without a CDF).  Any other primitive -- not a light, a plane, or a prim outside
+ *     [0, numPrimitives), so that the prims of tb200_trace_rays can be passed straight through on misses (-1) --
+ *     gives pos = normal = 0.  A degenerate triangle can give a zero normal too, so a zero normal does not mean
+ *     "not a light".  `time` must be finite, as for tb200_sample_lights: the device takes a static primitive's
+ *     transform as it is, where the reference interpolates it and a NaN or infinite time would make it NaN.
+ *     The area pdf of a sample is 1 / PrimitiveArea (tinsel_b200.primitive_areas gives it as the renderer computes
+ *     it: 4 pi r^2 of the unscaled radius for a sphere, the mesh's area times the end transform's scale for a mesh).
+ *   tb200_sample_probe: per seed i, ProbeSample(probe, dir, color, pdf, Random(seeds[i])) (src/probe.h:205-236),
+ *     bit for bit, including pdf = 0 where sinTheta == 0; all zeros when the sky has no probe.  The solid-angle pdf
+ *     of any direction, for MIS against other strategies, is ProbePdf, which tb200_sky_eval returns.
+ * The pads are written as 0.  All arrays are DEVICE memory of the renderer's device (a multi-device renderer: its
+ * head); alignment: q 8 bytes, seeds 4, out 16.  The refusals, stream, synchronisation and side effects are
+ * tb200_trace_rays': null pointers, n < 0, host or foreign-device memory and spans past the end of their
+ * allocation are refused before any launch; needs no tb200_init; adds 1 to stats.kernelLaunches, sets stats.gpuMs
+ * to its kernel's time, and touches nothing else.  n == 0 launches nothing.  Returns 0 on success. */
+typedef struct tb200_emitter_query { int32_t prim; float time; } tb200_emitter_query;                      /* 8 B */
+typedef struct tb200_emitter_sampled { float pos[3]; float pad0; float normal[3]; float pad1; } tb200_emitter_sampled;
+                                                                                                            /* 32 B */
+typedef struct tb200_probe_sampled { float dir[3]; float pdf; float color[3]; float pad; } tb200_probe_sampled;
+                                                                                                            /* 32 B */
+int tb200_sample_emitters(tb200_renderer* r, const tb200_emitter_query* q, const uint32_t* seeds,
+                          tb200_emitter_sampled* out, int64_t n);
+int tb200_sample_probe(tb200_renderer* r, const uint32_t* seeds, tb200_probe_sampled* out, int64_t n);
+
 /* Sets the frame counter (frame k seeds sample k of every pixel). */
 void tb200_set_frame(tb200_renderer* r, int frame);
 

@@ -101,6 +101,10 @@ def load_library():
     lib.tb200_sample_lights.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_sky_eval.restype = C.c_int
     lib.tb200_sky_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_sample_emitters.restype = C.c_int
+    lib.tb200_sample_emitters.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_sample_probe.restype = C.c_int
+    lib.tb200_sample_probe.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_set_frame.restype = None
     lib.tb200_set_frame.argtypes = [C.c_void_p, C.c_int]
     lib.tb200_get_stats.restype = None
@@ -163,6 +167,13 @@ def light_queries(prims, p, n, wo, eta_i, eta_o, time):
     trace_rays returns and -dir of the incoming ray); eta_i, eta_o, time: (N,) float32 tensors or Python numbers."""
     return _pack_records(prims, 16, 7, [(0, p, 3, "p"), (3, time, 1, "time"), (4, n, 3, "n"), (8, wo, 3, "wo"),
                                         (11, eta_i, 1, "eta_i"), (12, eta_o, 1, "eta_o"), (13, 0.0, 3, "pad")])
+
+
+def emitter_queries(prims, time):
+    """Packs tb200_emitter_query records for Renderer.sample_emitters: an (N, 2) float32 tensor on `prims`' device with
+    the int32 primitive's bits and the time per row.  prims: (N,) int32 tensor (trace_rays' prims can be passed as they
+    are); time: (N,) float32 tensor or a Python number."""
+    return _pack_records(prims, 2, 0, [(1, time, 1, "time")])
 
 
 def _pack_records(prims, width, prim_col, fields):
@@ -414,12 +425,13 @@ class Renderer:
             raise ValueError("%s must be contiguous" % name)
 
     def _check_records(self, x, name, width, dtype):
-        """Checks a (N, width) tensor of query records and returns N."""
+        """Checks a (N, width) tensor of query records, or with width None an (N,) one, and returns N."""
         import torch
-        if not isinstance(x, torch.Tensor) or x.dim() != 2:
-            raise ValueError("%s must be a (N, %d) tensor" % (name, width))
+        shape = "(N,)" if width is None else "(N, %d)" % width
+        if not isinstance(x, torch.Tensor) or x.dim() != (1 if width is None else 2):
+            raise ValueError("%s must be a %s tensor" % (name, shape))
         n = x.shape[0]
-        self._check_tensor(x, name, (n, width), dtype)
+        self._check_tensor(x, name, (n,) if width is None else (n, width), dtype)
         return n
 
     def _wait_for_torch(self):
@@ -429,7 +441,8 @@ class Renderer:
             torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()
 
     def _query(self, entry, records, inputs, outputs, before=(), after=()):
-        """What the batched queries share.  records: (tensor, name, width, dtype), the (N, width) records that set N;
+        """What the batched queries share.  records: (tensor, name, width, dtype), the (N, width) records that set N
+        ((N,) with width None);
         inputs: further input arrays and outputs: output arrays, each (tensor or None, name, shape after N, dtype).
         Checks them all, allocating on the head device the outputs not given (an input must be given); when N > 0,
         waits for torch and calls the library's `entry` on the `before` arguments, the records, the inputs, the
@@ -564,6 +577,32 @@ class Renderer:
         import torch
         out, = self._query("tb200_sky_eval", (rays, "rays", 8, torch.float32), [], [(out, "out", (4,), torch.float32)])
         return (out[:, :3], out[:, 3]) if split else out
+
+    def sample_emitters(self, queries, seeds, out=None):
+        """A point on each query's light (tb200_sample_emitters): PrimitiveSample (src/intersection.h:855-904) of
+        primitive `prim` at `time` from Random(seed), bit for bit -- what SampleLights draws for one light sample.
+        queries: contiguous float32 CUDA tensor (N, 2) on the head device, the tb200_emitter_query records, with
+        column 0 holding the int32 primitive index's bits (emitter_queries packs them); seeds: (N,) int32 tensor
+        whose bits are the uint32 seeds.  Returns (pos (N, 3) float32, normal (N, 3) float32), views of one (N, 8)
+        tensor of tb200_emitter_sampled records, which `out` (float32) gives when it is passed.  Only primitives with
+        lightSamples > 0 are sampled; any other prim, or one outside the scene, gives zeros.  The sample's area pdf
+        is 1 / primitive_areas(scene)[prim].  Stream behaviour as for trace_rays."""
+        import torch
+        out, = self._query("tb200_sample_emitters", (queries, "queries", 2, torch.float32),
+                           [(seeds, "seeds", (), torch.int32)], [(out, "out", (8,), torch.float32)])
+        return out[:, 0:3], out[:, 4:7]
+
+    def sample_probe(self, seeds, out=None):
+        """A direction drawn from the sky's probe per seed (tb200_sample_probe): ProbeSample (src/probe.h:205-236)
+        from Random(seed), bit for bit -- what SampleLights draws for its probe sample.  seeds: (N,) int32 CUDA
+        tensor on the head device whose bits are the uint32 seeds.  Returns (dir (N, 3) float32, pdf (N,) float32,
+        color (N, 3) float32), views of one (N, 8) tensor of tb200_probe_sampled records, which `out` (float32)
+        gives when it is passed; zeros when the sky has no probe.  pdf is 0 where sin(theta) is 0; sky() gives the
+        matching ProbePdf of any direction.  Stream behaviour as for trace_rays."""
+        import torch
+        out, = self._query("tb200_sample_probe", (seeds, "seeds", None, torch.int32), [],
+                           [(out, "out", (8,), torch.float32)])
+        return out[:, 0:3], out[:, 3], out[:, 4:7]
 
     def set_frame(self, frame):
         self.lib.tb200_set_frame(self.h, frame)

@@ -189,6 +189,23 @@ class LightQuery(C.Structure):
                 ("wo", C.c_float * 3), ("etaI", C.c_float), ("etaO", C.c_float), ("pad", C.c_float * 3)]
 
 
+class EmitterQuery(C.Structure):
+    """tb200_emitter_query: one query of tb200_sample_emitters, a light primitive and a time (8 bytes)."""
+    _fields_ = [("prim", C.c_int32), ("time", C.c_float)]
+
+
+class EmitterSampled(C.Structure):
+    """tb200_emitter_sampled: a point PrimitiveSample drew on a light and the normal there, from tb200_sample_emitters
+    (32 bytes)."""
+    _fields_ = [("pos", C.c_float * 3), ("pad0", C.c_float), ("normal", C.c_float * 3), ("pad1", C.c_float)]
+
+
+class ProbeSampled(C.Structure):
+    """tb200_probe_sampled: a direction ProbeSample drew, its pdf and the probe's colour there, from tb200_sample_probe
+    (32 bytes)."""
+    _fields_ = [("dir", C.c_float * 3), ("pdf", C.c_float), ("color", C.c_float * 3), ("pad", C.c_float)]
+
+
 # tb200_camera_sample as a numpy record (Renderer.camera_rays takes the same records as an (N, 2) int32 tensor)
 CAMERA_SAMPLE_DTYPE = np.dtype([("pixel", "<i4"), ("frame", "<i4")])
 
@@ -242,6 +259,8 @@ EXPORTS = [
     "tb200_splat",
     "tb200_sample_lights",
     "tb200_sky_eval",
+    "tb200_sample_emitters",
+    "tb200_sample_probe",
     "tb200_set_frame",
     "tb200_get_stats",
     "tb200_last_kernel",

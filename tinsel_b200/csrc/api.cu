@@ -2021,6 +2021,30 @@ int tb200_sky_eval(tb200_renderer* r, const tb200_ray* rays, float* out, int64_t
                      {{rays, sizeof(tb200_ray), 16, "rays"}, {out, 4 * sizeof(float), 16, "out"}}, Q);
 }
 
+static_assert(sizeof(tb200_emitter_query) == 8 && sizeof(tb200_emitter_sampled) == 32 && sizeof(tb200_probe_sampled) == 32,
+              "the sample queries read one float2 per query and write two float4");
+
+int tb200_sample_emitters(tb200_renderer* r, const tb200_emitter_query* q, const uint32_t* seeds,
+                          tb200_emitter_sampled* out, int64_t n)
+{
+    QueryParams Q = {};
+    Q.emitterQueries = reinterpret_cast<const float2*>(q);
+    Q.seeds = seeds;
+    Q.emitterOut = reinterpret_cast<float4*>(out);
+    return run_query("tb200_sample_emitters", r, QueryKind::SampleEmitters, "n", n,
+                     {{q, sizeof(tb200_emitter_query), 8, "q"}, {seeds, sizeof(uint32_t), 4, "seeds"},
+                      {out, sizeof(tb200_emitter_sampled), 16, "out"}}, Q);
+}
+
+int tb200_sample_probe(tb200_renderer* r, const uint32_t* seeds, tb200_probe_sampled* out, int64_t n)
+{
+    QueryParams Q = {};
+    Q.seeds = seeds;
+    Q.probeOut = reinterpret_cast<float4*>(out);
+    return run_query("tb200_sample_probe", r, QueryKind::SampleProbe, "n", n,
+                     {{seeds, sizeof(uint32_t), 4, "seeds"}, {out, sizeof(tb200_probe_sampled), 16, "out"}}, Q);
+}
+
 #ifdef TB_WF2_STAGE_CLOCKS
 // development builds only (-DTB_WF2_STAGE_CLOCKS, tools/stage_clocks.py): copies the lane-owned wavefront
 // layout's per-stage cycle counters of the current device into out[0..n) (n >= 15 words, see wf2_lanes.cuh:

@@ -130,8 +130,9 @@ void launch_nlm(const NlmParams& p, cudaStream_t stream, unsigned long long* lau
 
 // The batched queries (tb_query.cuh): the ray queries, each Trace (render.cpp:17-62) of every ray of a caller's
 // batch; the BSDF queries, one Disney BSDF call (disney.h) per query record; the two ends of a path, the
-// renderer's camera sample and the film's AddSample, per sample record; and the light queries, SampleLights per
-// surface record and the sky of a miss per ray:
+// renderer's camera sample and the film's AddSample, per sample record; the light queries, SampleLights per
+// surface record and the sky of a miss per ray; and the two draws SampleLights is made of, PrimitiveSample per
+// emitter record and ProbeSample per seed:
 enum class QueryKind {
     Closest,      // tb200_trace_rays: the closest hit
     ClosestTri,   // tb200_trace_rays_tri: the closest hit and the winner's triangle and barycentric weights
@@ -142,6 +143,8 @@ enum class QueryKind {
     Splat,        // tb200_splat: AddSample of a caller's radiance at a raster position
     SampleLights, // tb200_sample_lights: SampleLights (next-event estimation) at a surface point
     Sky,          // tb200_sky_eval: Sky::Eval and ProbePdf of a direction
+    SampleEmitters,   // tb200_sample_emitters: PrimitiveSample of a light primitive
+    SampleProbe,      // tb200_sample_probe: ProbeSample of the sky's probe
 };
 // Every query's parameters.  The input and output pointers a query does not use stay null.
 struct QueryParams {
@@ -170,6 +173,10 @@ struct QueryParams {
     const float4* lightQueries;  // SampleLights: 4 per query: p.xyz, time; n.xyz, prim bits; wo.xyz, etaI; etaO, pad
     float* lightRadiance;        // SampleLights: 3 per query: rgb (seeds: 1 per query, the Random seed)
     float4* skyOut;              // Sky: 1 per ray (of rays, whose dir alone is read): Sky::Eval rgb, ProbePdf
+    // (and these after all those, so that the nine kernels above keep theirs)
+    const float2* emitterQueries;   // SampleEmitters: 1 per query: prim bits, time (seeds: 1 per query)
+    float4* emitterOut;             // SampleEmitters: 2 per query: pos.xyz, 0; normal.xyz, 0
+    float4* probeOut;               // SampleProbe: 2 per seed: dir.xyz, pdf; color.rgb, 0
 };
 // Unlike the launches above, it leaves tb200_last_kernel alone and so returns no kernel name.
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);

@@ -5,7 +5,9 @@
 // (tb200_bsdf_eval, tb200_bsdf_sample) over the renderer's Disney BSDF functions; and the two ends of a path: the
 // renderer's camera samples (tb200_camera_rays, over camera_sample) and the film's splat (tb200_splat, over
 // add_sample_small); and the light queries: next-event estimation (tb200_sample_lights, over nee_generate and
-// nee_connect) and the sky of a miss (tb200_sky_eval, over sky_eval and probe_pdf).  Included once, by kernels.cu.
+// nee_connect) and the sky of a miss (tb200_sky_eval, over sky_eval and probe_pdf); and the two draws NEE is made of:
+// emitter samples (tb200_sample_emitters, over prim_sample) and probe samples (tb200_sample_probe, over
+// probe_sample).  Included once, by kernels.cu.
 //
 // The ray queries and the NEE query run a persistent kernel: as many CTAs as the SMs hold at once, for the whole
 // batch.  Their warps claim chunks of 32 records from a global counter: a static split would leave SMs idle, because
@@ -249,20 +251,63 @@ __global__ void __launch_bounds__(TB_QUERY_THREADS) k_sky(const __grid_constant_
     }
 }
 
+// The emitter samples (QueryKind::SampleEmitters): per record (prim, time), PrimitiveSample (intersection.h:855-904)
+// from Random(seed), bit for bit, through the prim_sample nee_generate calls, on the primitive record in global
+// memory.  Only lights (lightSamples > 0) are sampled; any other prim, or one outside [0, numPrims), gives zeros and
+// draws nothing.  A query costs at most one binary search of a mesh's CDF, so grid-stride, one record per thread:
+// one 8-byte load, two streaming stores.
+__global__ void __launch_bounds__(TB_QUERY_THREADS) k_sample_emitters(const __grid_constant__ QueryParams P)
+{
+    const unsigned long long n = (unsigned long long)P.numRays;
+    const unsigned long long stride = (unsigned long long)gridDim.x * TB_QUERY_THREADS;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * TB_QUERY_THREADS + threadIdx.x; i < n; i += stride) {
+        const float2 q = __ldg(&P.emitterQueries[i]);   // prim bits, time
+        const int prim = __float_as_int(q.x);
+        V3 pos = v3s(0.0f), normal = v3s(0.0f);
+        if (prim >= 0 && prim < P.scene.numPrims && P.scene.prims[prim].lightSamples > 0) {
+            Rng rng = rng_seed(__ldg(&P.seeds[i]));
+            prim_sample<TB_FEAT_ALL>(P.scene, P.scene.prims[prim], q.y, pos, normal, rng);
+        }
+        __stcs(&P.emitterOut[2 * i], make_float4(pos.x, pos.y, pos.z, 0.0f));
+        __stcs(&P.emitterOut[2 * i + 1], make_float4(normal.x, normal.y, normal.z, 0.0f));
+    }
+}
+
+// The probe samples (QueryKind::SampleProbe): per seed, ProbeSample (probe.h:205-236) from Random(seed), bit for
+// bit, through the probe_sample nee_generate calls; zeros without a probe.  Two binary searches per seed, so
+// grid-stride, one seed per thread: one 4-byte load, two streaming stores.
+__global__ void __launch_bounds__(TB_QUERY_THREADS) k_sample_probe(const __grid_constant__ QueryParams P)
+{
+    const unsigned long long n = (unsigned long long)P.numRays;
+    const unsigned long long stride = (unsigned long long)gridDim.x * TB_QUERY_THREADS;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * TB_QUERY_THREADS + threadIdx.x; i < n; i += stride) {
+        V3 dir = v3s(0.0f), color = v3s(0.0f);
+        float pdf = 0.0f;
+        if (P.scene.probe.valid) {
+            Rng rng = rng_seed(__ldg(&P.seeds[i]));
+            probe_sample(P.scene.probe, dir, color, pdf, rng);
+        }
+        __stcs(&P.probeOut[2 * i], make_float4(dir.x, dir.y, dir.z, pdf));
+        __stcs(&P.probeOut[2 * i + 1], make_float4(color.x, color.y, color.z, 0.0f));
+    }
+}
+
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount)
 {
     if (p.numRays <= 0) return;
     const bool perThread = kind != QueryKind::Closest && kind != QueryKind::ClosestTri && kind != QueryKind::Occluded &&
                            kind != QueryKind::SampleLights;
-    void (*kernel)(QueryParams) = kind == QueryKind::Closest        ? k_trace_rays<false>
-                                  : kind == QueryKind::ClosestTri   ? k_trace_rays<true>
-                                  : kind == QueryKind::Occluded     ? k_occluded_rays
-                                  : kind == QueryKind::BsdfEval     ? k_bsdf_query<false>
-                                  : kind == QueryKind::BsdfSample   ? k_bsdf_query<true>
-                                  : kind == QueryKind::CameraRays   ? k_camera_rays
-                                  : kind == QueryKind::Splat        ? k_splat
-                                  : kind == QueryKind::SampleLights ? k_sample_lights
-                                                                    : k_sky;
+    void (*kernel)(QueryParams) = kind == QueryKind::Closest          ? k_trace_rays<false>
+                                  : kind == QueryKind::ClosestTri     ? k_trace_rays<true>
+                                  : kind == QueryKind::Occluded       ? k_occluded_rays
+                                  : kind == QueryKind::BsdfEval       ? k_bsdf_query<false>
+                                  : kind == QueryKind::BsdfSample     ? k_bsdf_query<true>
+                                  : kind == QueryKind::CameraRays     ? k_camera_rays
+                                  : kind == QueryKind::Splat          ? k_splat
+                                  : kind == QueryKind::SampleLights   ? k_sample_lights
+                                  : kind == QueryKind::Sky            ? k_sky
+                                  : kind == QueryKind::SampleEmitters ? k_sample_emitters
+                                                                      : k_sample_probe;
     // as many CTAs as the SMs hold at once, but no more than there are 32-ray chunks (the grid-stride queries: one
     // record per thread)
     int perSM = 0;
