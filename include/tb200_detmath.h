@@ -102,6 +102,9 @@ TBM_HD void tbm_sincos_d(double x, double* s, double* c)
     else { *s = -cr; *c = sr; }
 }
 
+/* sin(-0) gives +0, not C99's -0 (r = -0 - kd*P1 with kd = -0 is +0).  No caller passes -0: every phase is a product of
+ * non-negative draws or uv coordinates (tb_shade.cuh, tb_math.cuh's sampling warps), so a select on the hot path would
+ * only serve a case that cannot occur.  Every other |x| < 1e6 gives the correctly rounded value. */
 TBM_HD float tbm_sinf(float x)
 {
     double s, c;
@@ -209,7 +212,15 @@ TBM_HD double tbm_atan2_d(double y, double x)
 TBM_HD float tbm_atan2f(float y, float x)
 {
     if (!(y == y) || !(x == x)) return y + x;
-    return (float)tbm_atan2_d((double)y, (double)x);
+    double yd = (double)y, xd = (double)x;
+    /* C99 F.9.1.4: atan2(+-inf, +inf) = +-pi/4 and atan2(+-inf, -inf) = +-3pi/4, which are atan2(+-1, +-1); inf/inf
+     * would give NaN.  One call site, so that the inlined atan2 is not duplicated. */
+    const double kInfD = tbm_bits_to_double(0x7ff0000000000000ull);
+    if (fabs(yd) == kInfD && fabs(xd) == kInfD) {
+        yd = copysign(1.0, yd);
+        xd = copysign(1.0, xd);
+    }
+    return (float)tbm_atan2_d(yd, xd);
 }
 
 TBM_HD float tbm_acosf(float xf)

@@ -1,12 +1,22 @@
 """include/tb200_detmath.h on the host: correctly rounded results (vs double libm rounded once)
-and agreement with glibc's float functions to 1 ulp.  The device copy is checked against the same
-values in tests/test_parity_gpu.py through the per-sample parity tests."""
+and agreement with glibc's float functions to 1 ulp, over the ranges the hot path uses, over every
+sign and exponent of the one-argument functions, and on a table of special arguments of atan2f and
+powf, where C99 Annex F decides.  tests/test_detmath_gpu.py checks the device build against this
+host build on every float input."""
 import os
 import subprocess
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def _build(tmp_path, src):
+    path = tmp_path / "t.cpp"
+    path.write_text(src)
+    exe = str(tmp_path / "t")
+    subprocess.check_call(["/usr/bin/g++", "-O2", "-ffp-contract=off", "-I", os.path.join(ROOT, "include"), str(path), "-o", exe])
+    return exe
 
 SRC = r"""
 #include "tb200_detmath.h"
@@ -48,11 +58,98 @@ int main(){
 
 
 def test_detmath_is_correctly_rounded(tmp_path):
-    src = tmp_path / "t.cpp"
-    src.write_text(SRC)
-    exe = str(tmp_path / "t")
-    subprocess.check_call(["/usr/bin/g++", "-O2", "-ffp-contract=off", "-I", os.path.join(ROOT, "include"), str(src), "-o", exe])
-    misround, bad, special = map(int, subprocess.check_output([exe]).split())
+    misround, bad, special = map(int, subprocess.check_output([_build(tmp_path, SRC)]).split())
     assert misround <= 4, "results differ from the once-rounded double libm value in %d of 1.6e7 calls" % misround
     assert bad == 0, "more than 1 ulp from glibc float functions"
     assert special == 1
+
+
+SRC_EXPONENTS = r"""
+#include "tb200_detmath.h"
+#include <cstdio>
+#include <cmath>
+#include <cstdint>
+#include <cstring>
+static uint32_t bits(float f){ uint32_t u; memcpy(&u,&f,4); return u; }
+static float flt(uint32_t u){ float f; memcpy(&f,&u,4); return f; }
+static bool same(float a, float b){ return (std::isnan(a) && std::isnan(b)) || bits(a) == bits(b); }
+int main(){
+  uint32_t s=2463534242u; auto rnd=[&](){ s ^= s<<13; s ^= s>>17; s ^= s<<5; return s; };
+  long n=0, big=0, negzero=0, bad=0;
+  auto fail=[&](const char* f, uint32_t u, float got, float want){ if(bad++ < 16) printf("%s %08x %08x %08x\n", f, u, bits(got), bits(want)); };
+  // every sign and exponent (infinities and NaNs included), with the smallest and largest mantissa and random ones
+  for(uint32_t se=0; se<512; ++se) for(int k=0; k<3000; ++k){
+    const uint32_t u = (se<<23) | (k==0 ? 0u : k==1 ? 0x7fffffu : (rnd() & 0x7fffffu));
+    const float x = flt(u); ++n;
+    const float sf = tbm_sinf(x), cf = tbm_cosf(x);
+    float sc, cc; tbm_sincosf(x, &sc, &cc);
+    if(!same(sc, sf) || !same(cc, cf)) fail("sincosf", u, sc, sf);
+    if(!std::isfinite(x)){ if(!std::isnan(sf) || !std::isnan(cf)) fail("sinf/cosf", u, sf, NAN); }
+    // the documented exceptions, as exact values: (+0, 1) for |x| >= 1e6 and sin(-0) = +0
+    else if(std::fabs(x) >= 1e6f || u == 0x80000000u){
+      if(bits(sf) != 0u || bits(cf) != 0x3f800000u) fail("sinf/cosf", u, sf, 0.0f);
+      else if(u == 0x80000000u) negzero++;
+      else big++;
+    } else {
+      const float ws = (float)sin((double)x), wc = (float)cos((double)x);
+      if(!same(sf, ws)) fail("sinf", u, sf, ws);
+      if(!same(cf, wc)) fail("cosf", u, cf, wc);
+    }
+    const float e = tbm_expf(x), we = (float)exp((double)x);
+    if(!same(e, we)) fail("expf", u, e, we);
+    const float a = tbm_acosf(x), wa = std::fabs(x) <= 1.0f ? (float)acos((double)x) : NAN;
+    if(!same(a, wa)) fail("acosf", u, a, wa);
+    const float t = tbm_atan2f(x, 1.0f), wt = (float)atan2((double)x, 1.0);
+    if(!same(t, wt)) fail("atan2f(x,1)", u, t, wt);
+  }
+  printf("end %ld %ld %ld %ld\n", bad, n, big, negzero);
+}
+"""
+
+
+def test_every_sign_and_exponent(tmp_path):
+    lines = subprocess.check_output([_build(tmp_path, SRC_EXPONENTS)]).decode().splitlines()
+    bad, n, big, negzero = map(int, lines[-1].split()[1:])
+    assert bad == 0, "%d results differ from float64 rounded once (function, x, got, want):\n%s" % (bad, "\n".join(lines[:-1]))
+    assert n == 512 * 3000 and big > 0 and negzero == 1
+
+
+SRC_SPECIALS = r"""
+#include "tb200_detmath.h"
+#include <cstdio>
+#include <cmath>
+#include <cstdint>
+#include <cstring>
+#include <vector>
+static uint32_t bits(float f){ uint32_t u; memcpy(&u,&f,4); return u; }
+static float flt(uint32_t u){ float f; memcpy(&f,&u,4); return f; }
+static bool same(float a, float b){ return (std::isnan(a) && std::isnan(b)) || bits(a) == bits(b); }
+int main(){
+  // +-0, the smallest and largest subnormals, +-FLT_MIN, +-0.5, 1, 2, 3, 2.2, 1/2.2, odd and even integers around 2^24,
+  // +-FLT_MAX, +-inf, NaN
+  const float pos[] = {0.0f, flt(1u), flt(0x007fffffu), flt(0x00800000u), 0.5f, 1.0f, 2.0f, 3.0f, 2.2f, 1.0f / 2.2f,
+                       16777213.0f, 16777215.0f, 16777216.0f, 16777218.0f, 33554430.0f, flt(0x7f7fffffu), INFINITY};
+  std::vector<float> sp;
+  for(float p : pos){ sp.push_back(p); sp.push_back(-p); }
+  sp.push_back(NAN);
+  long n=0, bad=0;
+  for(float x : sp) for(float y : sp) for(int f=0; f<2; ++f){
+    // the value, float64 rounded once (C99 Annex F at the special values), glibc's float function
+    const float r = f ? tbm_powf(x, y) : tbm_atan2f(x, y);
+    const float d = f ? (float)pow((double)x, (double)y) : (float)atan2((double)x, (double)y);
+    const float g = f ? powf(x, y) : atan2f(x, y);
+    // glibc's float function may be 1 ulp from the correctly rounded value; no other difference is allowed
+    const long ulp = (long)bits(r) - (long)bits(g);
+    const bool ok = same(r, d) && (same(r, g) || (std::isfinite(r) && std::isfinite(g) && (ulp == 1 || ulp == -1)));
+    ++n;
+    if(!ok && bad++ < 16) printf("%s(%a, %a) %08x float64 %08x glibc %08x\n", f ? "powf" : "atan2f", x, y, bits(r), bits(d), bits(g));
+  }
+  printf("end %ld %ld\n", bad, n);
+}
+"""
+
+
+def test_atan2f_and_powf_on_special_values(tmp_path):
+    lines = subprocess.check_output([_build(tmp_path, SRC_SPECIALS)]).decode().splitlines()
+    bad, n = map(int, lines[-1].split()[1:])
+    assert bad == 0, "%d of %d results differ from float64 or glibc:\n%s" % (bad, n, "\n".join(lines[:-1]))

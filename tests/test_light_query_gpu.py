@@ -220,6 +220,8 @@ def _sky_directions(rng):
     axis = [(0.0, y, 0.0) for y in (0.5, -0.5, 2.0, 0.0, -0.0, 1e-30)]
     odd = [(np.nan, 0.0, 1.0), (0.0, np.nan, 0.0), (1.0, 0.0, np.nan), (np.inf, 1.0, 0.0), (0.0, -np.inf, 0.0),
            (0.0, 0.0, 0.0), (-0.0, -0.0, -0.0)]
+    # two infinite components: atan2f(+-inf, +-inf) is +-pi/4 or +-3pi/4 (C99 Annex F), not NaN
+    odd += [(x, y, z) for x in (np.inf, -np.inf) for z in (np.inf, -np.inf) for y in (0.0, -0.0, 0.5, -1.0, np.inf)]
     return np.concatenate([u, u * F32(3.0), u * F32(1e-3), np.array(poles + axis + odd, F32)]).astype(F32)
 
 
@@ -238,10 +240,16 @@ def test_sky_matches_restatement(name):
     assert not bad.any(), (name, int(bad.sum()), d[bad][:4], got[bad][:4], want[bad][:4])
     rgb, pdf = r.sky(torch.from_numpy(rays).cuda(), split=True)
     assert tuple(rgb.shape) == (len(d), 3) and tuple(pdf.shape) == (len(d),)
-    if not snap.scene.contents.sky.probeValid:
+    sky = snap.scene.contents.sky
+    if not sky.probeValid:
         assert (got[:, 3] == 0).all()
     else:
         assert (got[:, 3] > 0).any()
+        # (inf, 0, inf) looks up u = (pi + pi/4) / (2 pi) = 0.625 and v = acos(0) / pi = 0.5
+        k = int(np.flatnonzero((d[:, 0] == np.inf) & (d[:, 1] == 0) & (d[:, 2] == np.inf))[0])
+        w, h = sky.probeWidth, sky.probeHeight
+        texel = np.ctypeslib.as_array(sky.probeData, shape=(h * w * 4,)).reshape(h, w, 4)[int(0.5 * h), int(0.625 * w), :3]
+        assert (got[k, :3].view(np.uint32) == texel.view(np.uint32)).all(), (name, got[k], texel)
     r.close()
     snap.close()
 
