@@ -112,4 +112,18 @@ void oracle_path_trace_reseeded(const tb200_scene* scene, long long n, const flo
     }
 }
 
+// out[4k..4k+3] = sky_eval() of the scene's sky in direction dirs[3k..3k+2] and probe_pdf() of it (0 without a probe):
+// oracle_sky_eval over n directions.
+void oracle_sky_eval_batch(const tb200_scene* scene, long long n, const float* dirs, float* out)
+{
+    const tb200_sky& s = scene->sky;
+    for (long long k = 0; k < n; ++k) {
+        const vec3 d = from(dirs + 3 * k);
+        const vec3 c = sky_eval(s, d);
+        float* o = out + 4 * k;
+        o[0] = c.x; o[1] = c.y; o[2] = c.z;
+        o[3] = s.probeValid ? probe_pdf(s, d) : 0.0f;
+    }
+}
+
 }  // extern "C"

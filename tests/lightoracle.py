@@ -1,9 +1,9 @@
-"""TEST INFRASTRUCTURE: the CPU restatement's SampleLights over a batch of surface records and its PathTrace with a
-seed per call (tests/light_oracle.cpp), the arms the device's next-event-estimation query and a path built from the
-queries are checked against.  The library is compiled on first use, with oracle/Makefile's flags, from the
-restatement's unchanged source, into a temporary directory keyed by the sources' hash (the repository tree may be
-read-only).  Besides its own two functions it exports every entry point of the restatement (oracle_sky_eval,
-oracle_primitive_sample, ...)."""
+"""TEST INFRASTRUCTURE: the CPU restatement's SampleLights over a batch of surface records, its PathTrace with a
+seed per call and its Sky::Eval over a batch of directions (tests/light_oracle.cpp), the arms the device's
+next-event-estimation and sky queries and a path built from the queries are checked against.  The library is compiled
+on first use, with oracle/Makefile's flags, from the restatement's unchanged source, into a temporary directory keyed
+by the sources' hash (the repository tree may be read-only).  Besides its own three functions it exports every entry
+point of the restatement (oracle_primitive_sample, ...)."""
 import ctypes as C
 import hashlib
 import os
@@ -51,7 +51,7 @@ def load():
     lib.oracle_create.restype = C.c_void_p
     lib.oracle_create.argtypes = [C.POINTER(abi.Scene)]
     lib.oracle_destroy.argtypes = [C.c_void_p]
-    lib.oracle_sky_eval.argtypes = [C.c_void_p, _f32p, _f32p, _f32p]
+    lib.oracle_sky_eval_batch.argtypes = [C.POINTER(abi.Scene), C.c_longlong, _f32p, _f32p]
     lib.oracle_primitive_sample.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_int, _f32p, _f32p, _f32p]
     abi.declare_snapshot_api(lib)
     _lib = lib
@@ -95,16 +95,9 @@ def path_trace_reseeded(scene_ptr, origin, direction, time, max_depth, seeds):
 
 def sky_eval(scene_ptr, dirs):
     """The restatement's Sky::Eval and ProbePdf (0 without a probe) of every direction: (n, 4) float32."""
-    lib = load()
-    h = lib.oracle_create(scene_ptr)
-    assert h, "the restatement refused the scene"
     dirs = np.ascontiguousarray(dirs, np.float32).reshape(-1, 3)
     out = np.zeros((dirs.shape[0], 4), np.float32)
-    c, p = np.zeros(3, np.float32), np.zeros(1, np.float32)
-    for k in range(dirs.shape[0]):
-        lib.oracle_sky_eval(h, _fp(dirs[k]), _fp(c), _fp(p))
-        out[k, :3], out[k, 3] = c, p[0]
-    lib.oracle_destroy(h)
+    load().oracle_sky_eval_batch(scene_ptr, dirs.shape[0], _fp(dirs), _fp(out))
     return out
 
 
