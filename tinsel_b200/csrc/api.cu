@@ -435,6 +435,7 @@ bool image_from_scene(const tb200_scene* s, SceneImage* img)
             d.area = s->meshes[p.mesh].area * p.end.s;
         else
             d.area = 0.0f;
+        set_light_constants(d);
         d.mat = make_material(p.material);
         if (p.lightSamples > 0) img->numNee += p.lightSamples;
     }
@@ -565,7 +566,7 @@ bool build_scene(tb200_renderer* r, const tb200_scene* s)
 // a stamp mismatch is refused and the caller falls back to tb200_create), then the SceneImage fields in
 // declaration order; every array as a 64-bit count followed by its bytes.
 const char kCacheMagic[8] = {'T', 'B', '2', 'C', 'A', 'C', 'H', 'E'};
-const uint32_t kCacheVersion = 3;   // 3: DMaterial::flags
+const uint32_t kCacheVersion = 4;   // 3: DMaterial::flags; 4: DPrim's light constants
 
 struct CacheStamp {
     uint32_t version, sizeofPrim, sizeofPair, sizeofOp;

@@ -117,11 +117,18 @@ TB_DEV void add_sample(const DFilm& f, float4* accum, float rasterX, float raste
     }
 }
 
+// add_sample out of line: add_sample_small's fallback, which a 3x3 Gaussian footprint and a finite sample never take,
+// so that its ~350 instructions stay out of the splat that calls it
+TB_NOINLINE void add_sample_cold(const DFilm& f, float4* accum, float rasterX, float rasterY, V3 sample)
+{
+    add_sample(f, accum, rasterX, rasterY, sample);
+}
+
 // add_sample with the Gaussian's weights evaluated once per column and once per row: for a finite sample whose
 // footprint is at most 3x3 pixels, the six filter_gaussian values are independent, inline expf chains that run
 // side by side (add_sample makes up to twelve out-of-line calls, one after the other).  Each pixel's weight is
 // still gx * gy, and the pixels whose weight is zero are still skipped, so every reduction carries the same bits.
-// Anything else takes add_sample.
+// Anything else takes add_sample (add_sample_cold).
 TB_DEV void add_sample_small(const DFilm& f, float4* accum, float rasterX, float rasterY, V3 sample)
 {
     const int startX = tb_max(0, int(rasterX - f.filterWidth));
@@ -132,7 +139,7 @@ TB_DEV void add_sample_small(const DFilm& f, float4* accum, float rasterX, float
     const float l = length(sample);
     if (l > f.clamp) c = sample * (f.clamp / l);
     if (f.filterType != TB200_FILTER_GAUSSIAN || endX - startX > 2 || endY - startY > 2 || !(isfinite(c.x) && isfinite(c.y) && isfinite(c.z))) {
-        add_sample(f, accum, rasterX, rasterY, sample);
+        add_sample_cold(f, accum, rasterX, rasterY, sample);
         return;
     }
     float gx[3], gy[3];

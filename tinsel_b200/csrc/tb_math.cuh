@@ -108,6 +108,16 @@ TB_HD uint32_t tb_float_bits(float f)
 #endif
 }
 
+#if defined(__CUDA_ARCH__)
+#define TB_COLD __noinline__   // rarely executed on the device: keep a single out-of-line copy
+#else
+#define TB_COLD
+#endif
+
+// rotate_xf's full arithmetic, out of line on the device: inline, its two qmuls were copied into every transform of
+// every kernel, while scenes without rotations (cornell, veach) only ever take the shortcut
+static __host__ __device__ TB_COLD V3 rotate_xf_full(Q4 q, V3 v, bool inverse) { return rotate(inverse ? qconj(q) : q, v); }
+
 // rotate(q, v), or rotate(qconj(q), v) when `inverse`, for the rotation of a transform.  When q is (+0, +0, +0, +1)
 // bit for bit and v is finite, every sum in both qmuls adds only exact zeros to the one product v.c * 1, and the +0
 // among them turns a -0 into +0: the result is v + 0.0f, in either direction.  Any other quaternion (a -0 component
@@ -116,7 +126,7 @@ TB_HD V3 rotate_xf(Q4 q, V3 v, bool inverse)
 {
     const bool unrotated = (tb_float_bits(q.x) | tb_float_bits(q.y) | tb_float_bits(q.z)) == 0u && tb_float_bits(q.w) == 0x3f800000u;
     if (unrotated && fabsf(v.x) <= FLT_MAX && fabsf(v.y) <= FLT_MAX && fabsf(v.z) <= FLT_MAX) return v + v3s(0.0f);
-    return rotate(inverse ? qconj(q) : q, v);
+    return rotate_xf_full(q, v, inverse);
 }
 // 1.0f / s, without the IEEE division for the common unit scale (1.0f / 1.0f is 1.0f)
 TB_HD float inverse_scale(float s) { return s == 1.0f ? 1.0f : 1.0f / s; }
@@ -128,11 +138,6 @@ TB_HD V3 inverse_transform_vector(const Xf& t, V3 v) { return inverse_scale(t.s)
 TB_HD V3 inverse_transform_point(const Xf& t, V3 v) { return inverse_scale(t.s) * rotate_xf(t.r, v - t.p, true); }
 
 // maths.h:1566-1569 with Quat Lerp (maths.h:79-83 over Quat ops) and Normalize(Quat) (maths.h:547-553)
-#if defined(__CUDA_ARCH__)
-#define TB_COLD __noinline__   // rarely executed on the device: keep a single out-of-line copy
-#else
-#define TB_COLD
-#endif
 static __host__ __device__ TB_COLD Xf interpolate_transform(const Xf& a, const Xf& b, float t)
 {
     Xf r;

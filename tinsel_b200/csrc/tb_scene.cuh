@@ -114,8 +114,27 @@ struct DPrim {
     int mesh;
     int lightSamples;
     float area;           // PrimitiveArea, intersection.h:833-853
+    // what the MIS weights of path_hit and nee_connect need of this primitive as a light (render.cpp:255-310,
+    // 176-224) and depends on area and lightSamples alone: set_light_constants
+    float invArea;          // 1.0f / area
+    float cbsdf;            // 1.0f / N, N = int(lightSamples + 1.0f)
+    float clight;           // float(lightSamples) / N
+    float invLightSamples;  // 1.0f / lightSamples
     DMaterial mat;
 };
+
+// DPrim's light constants from its area and lightSamples (host), with the float expressions of the MIS weights.  Host
+// float division is IEEE and correctly rounded as the device's -prec-div=true division is, the int <-> float
+// conversions round the same way and the host build does not contract, so every value has the bits the device would
+// compute (tests/test_light_constants.py).
+inline void set_light_constants(DPrim& d)
+{
+    d.invArea = 1.0f / d.area;
+    const int N = int(d.lightSamples + 1.0f);
+    d.cbsdf = 1.0f / N;
+    d.clight = float(d.lightSamples) / N;
+    d.invLightSamples = 1.0f / d.lightSamples;
+}
 
 struct DProbe {
     int valid, width, height;

@@ -570,10 +570,10 @@ TB_DEV void path_hit(const DScene& sc, PathState& ps, const Hit& h, int bounce, 
     } else {
         const float lightArea = prim.area;
         if (lightArea > 0.0f) {
-            const float lightPdf = ((1.0f / lightArea) * h.t * h.t) / tb_clamp(dot(-ps.d, h.n), 1.e-3f, 1.0f);
-            const int N = int(prim.lightSamples + 1.0f);
-            const float cbsdf = 1.0f / N;
-            const float clight = float(prim.lightSamples) / N;
+            // 1.0f / lightArea and the MIS constants, computed once per scene (tb_scene.cuh: set_light_constants)
+            const float lightPdf = (prim.invArea * h.t * h.t) / tb_clamp(dot(-ps.d, h.n), 1.e-3f, 1.0f);
+            const float cbsdf = prim.cbsdf;
+            const float clight = prim.clight;
             float weight = cbsdf * ps.bsdfPdf / (cbsdf * ps.bsdfPdf + clight * lightPdf);
             if (ps.rayType == TB_SPECULAR) weight = 1.0f;
             ps.L = ps.L + weight * ps.T * prim.mat.emission;
@@ -694,17 +694,16 @@ TB_DEV void nee_connect(const DScene& sc, const Surface& sf, const ShadowRay& sr
     const DPrim& light = sc.prims[sr.light];
     if (need && bsdfPdf > 0.0f) {
         const float tSq = sh.t * sh.t;
-        const float lightPdf = ((1.0f / light.area) * tSq) / nl;
-        const int N = int(light.lightSamples + 1.0f);
-        const float cbsdf = 1.0f / N;
-        const float clight = float(light.lightSamples) / N;
+        const float lightPdf = (light.invArea * tSq) / nl;
+        const float cbsdf = light.cbsdf;
+        const float clight = light.clight;
         const float weight = clight * lightPdf / (cbsdf * bsdfPdf + clight * lightPdf);
         // emission of whatever the shadow ray hit, not of the sampled light (render.cpp:217)
         c.Lacc = c.Lacc + weight * f * sc.prims[sh.prim].mat.emission * (tb_abs(dot(sr.d, sf.n)) / tb_max(1.e-3f, lightPdf));
     }
     c.sample++;
     if (c.sample >= light.lightSamples) {
-        c.sum = c.sum + c.Lacc * (1.0f / light.lightSamples);
+        c.sum = c.sum + c.Lacc * light.invLightSamples;
         c.Lacc = v3s(0.0f);
     }
 }

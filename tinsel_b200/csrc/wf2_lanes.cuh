@@ -179,14 +179,20 @@ void wf2_stage_clocks(unsigned long long* out, bool reset)
 
 // The lane-owned splat (stage R: wf2_stage_r).  It neither decodes the sample index nor draws the raster position
 // again: the slot's RNG chunk carries it in .zw from the sample's generation (wf2_scatter leaves .zw alone), and
-// add_sample_small weighs a 3x3 footprint with one filter evaluation per column and per row.
+// add_sample_small weighs a 3x3 footprint with one filter evaluation per column and per row.  The per-sample capture
+// (P.outRadiance, for trace_frame) is out of line: renders never take it.
+static __device__ __noinline__ void wf2_capture(const LaunchParams& P, uint32_t doneSample, float rasterX, float rasterY, V3 radiance)
+{
+    int px, py, frame;
+    decode_sample(P, (unsigned long long)doneSample, px, py, frame);
+    sample_end(P, px, py, rasterX, rasterY, radiance);
+}
+
 TB_DEV void wf2_splat(const LaunchParams& P, const float4* rec, float4 cl, uint32_t doneSample)
 {
     const float4 cr = cold_ld(rec, CC_RNG);
     if (P.outRadiance) {
-        int px, py, frame;
-        decode_sample(P, (unsigned long long)doneSample, px, py, frame);
-        sample_end(P, px, py, cr.z, cr.w, v3(cl.x, cl.y, cl.z));
+        wf2_capture(P, doneSample, cr.z, cr.w, v3(cl.x, cl.y, cl.z));
     } else {
         add_sample_small(P.film, P.accum, cr.z, cr.w, v3(cl.x, cl.y, cl.z));
     }
