@@ -488,6 +488,43 @@ int tb200_sample_emitters(tb200_renderer* r, const tb200_emitter_query* q, const
                           tb200_emitter_sampled* out, int64_t n);
 int tb200_sample_probe(tb200_renderer* r, const uint32_t* seeds, tb200_probe_sampled* out, int64_t n);
 
+/* ---- the probe's sampling tables, and a new sky for a live renderer ---------------------------
+ *   tb200_probe_tables: Probe::BuildCDF (src/probe.h:31-79) on the device, bit for bit (a NaN may have another
+ *     payload), for the width x height RGBA texels at `probe` (the layout of tb200_sky::probeData; alpha is
+ *     ignored): per texel the weight (r*0.3f + g*0.6f) + b*0.1f; per row its sequential fp32 running sum, pdfX and
+ *     cdfX = weight and running sum times the IEEE 1.0f / row total (a black row gives NaN: 0 * inf); pdfY and cdfY
+ *     = the row total and the rows' sequential running sum, each divided by the sum of all rows.  Writes
+ *     width*height floats to pdfX and cdfX and height floats to pdfY and cdfY, the tb200_sky tables of that probe.
+ *     Non-finite, negative and subnormal texels go through the arithmetic as they are.  All five arrays are DEVICE
+ *     memory of the renderer's device (a multi-device renderer: its head); `probe` 16-byte aligned, the tables 4.
+ *     Refused before any launch: width or height <= 0, width*height + 1 > INT32_MAX (the sampler indexes rows
+ *     with int), and, as by tb200_trace_rays, null pointers, host or foreign-device memory and spans past the end of
+ *     their allocation.  The stream, synchronisation and side effects are tb200_trace_rays': needs no tb200_init;
+ *     adds 3 to stats.kernelLaunches, sets stats.gpuMs to the kernels' time, and touches nothing else.  It does not
+ *     read or change the renderer's sky.  Returns 0 on success.
+ *   tb200_set_sky: replaces the renderer's sky -- its gradient colours and its probe -- and leaves it as
+ *     tb200_create would have built it from the same scene with this sky: every render call and every query after
+ *     it (tb200_sky_eval, tb200_sample_probe, tb200_sample_lights, ...) sees the new sky, the probe's shadow ray per
+ *     hit is counted in or out, and the wavefront kernel is chosen again for the scene with this sky under the knobs
+ *     read at create time (tb200_last_kernel reports the new choice at the next render).  probe == NULL gives the
+ *     gradient sky, and then width and height must be 0.  Otherwise `probe` is width x height RGBA texels as for
+ *     tb200_probe_tables, in HOST memory or in DEVICE memory of the renderer's device (its head; 16-byte aligned,
+ *     spanning width*height*16 bytes); a pointer to another device's memory is refused.  The renderer copies the
+ *     texels (the caller's buffer is free once the call returns) and builds the four tables with tb200_probe_tables'
+ *     kernels.  Colours and texels are taken as given, non-finite ones included.  A multi-device renderer sets the
+ *     same sky on every device (a device probe is copied from the head to each).  Atomic: the new probe is built in
+ *     full before anything changes, and after a refusal or a CUDA failure (-1, tb200_last_error says why) the
+ *     renderer renders exactly as before; on success the previous probe's memory is freed.  The accumulator, the
+ *     frame counter, stats.frames, stats.samples and tb200_last_kernel are left as they are: an image accumulated so
+ *     far keeps its samples of the old sky, and restarting it (tb200_init) is the caller's choice, as it is after a
+ *     camera change.  Adds the bytes copied from the host to stats.h2dBytes and the table build's launches to
+ *     stats.kernelLaunches, and sets stats.gpuMs to the build's time (0 for the gradient sky).  Runs on the
+ *     renderer's stream; returns when the new sky is in place.  Needs no tb200_init.  Returns 0 on success. */
+int tb200_probe_tables(tb200_renderer* r, const float* probe, int width, int height, float* pdfX, float* cdfX,
+                       float* pdfY, float* cdfY);
+int tb200_set_sky(tb200_renderer* r, const float horizon[3], const float zenith[3], const float* probe, int width,
+                  int height);
+
 /* Sets the frame counter (frame k seeds sample k of every pixel). */
 void tb200_set_frame(tb200_renderer* r, int frame);
 

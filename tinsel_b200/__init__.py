@@ -105,6 +105,10 @@ def load_library():
     lib.tb200_sample_emitters.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
     lib.tb200_sample_probe.restype = C.c_int
     lib.tb200_sample_probe.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.tb200_probe_tables.restype = C.c_int
+    lib.tb200_probe_tables.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.tb200_set_sky.restype = C.c_int
+    lib.tb200_set_sky.argtypes = [C.c_void_p, f32p, f32p, C.c_void_p, C.c_int, C.c_int]
     lib.tb200_set_frame.restype = None
     lib.tb200_set_frame.argtypes = [C.c_void_p, C.c_int]
     lib.tb200_get_stats.restype = None
@@ -603,6 +607,75 @@ class Renderer:
         out, = self._query("tb200_sample_probe", (seeds, "seeds", None, torch.int32), [],
                            [(out, "out", (8,), torch.float32)])
         return out[:, 0:3], out[:, 3], out[:, 4:7]
+
+    def _probe_image(self, probe, device_only):
+        """Checks an (H, W, 4) float32 C-contiguous probe image: a numpy array or a CPU tensor (unless device_only), or
+        a CUDA tensor on the head device.  Returns (pointer, W, H, whether it is on the device)."""
+        import torch
+        if isinstance(probe, np.ndarray):
+            if device_only:
+                raise TypeError("probe must be a CUDA tensor, not a numpy array")
+            if probe.dtype != np.float32:
+                raise TypeError("probe must be float32, not %s" % probe.dtype)
+            if probe.ndim != 3 or probe.shape[2] != 4:
+                raise ValueError("probe must have shape (H, W, 4), not %s" % (probe.shape,))
+            if not probe.flags["C_CONTIGUOUS"]:
+                raise ValueError("probe must be C-contiguous")
+            return probe.ctypes.data, probe.shape[1], probe.shape[0], False
+        if not isinstance(probe, torch.Tensor):
+            raise TypeError("probe must be a numpy array or a torch tensor")
+        if probe.dim() != 3 or probe.shape[2] != 4:
+            raise ValueError("probe must have shape (H, W, 4), not %s" % (tuple(probe.shape),))
+        if probe.device.type == "cpu" and not device_only:
+            if probe.dtype != torch.float32:
+                raise TypeError("probe must be torch.float32, not %s" % probe.dtype)
+            if not probe.is_contiguous():
+                raise ValueError("probe must be contiguous")
+        else:
+            self._check_tensor(probe, "probe", tuple(probe.shape), torch.float32)
+        return probe.data_ptr(), probe.shape[1], probe.shape[0], probe.device.type == "cuda"
+
+    def set_sky(self, horizon, zenith, probe=None):
+        """Replaces the renderer's sky (tb200_set_sky): the gradient colours horizon and zenith (3 floats each) and,
+        unless probe is None, an HDR probe of (H, W, 4) float32 RGBA texels, row 0 at the zenith -- a C-contiguous
+        numpy array, a CPU tensor, or a contiguous CUDA tensor on the head device.  The renderer copies the texels and
+        builds the probe's sampling tables on the device; afterwards it renders and answers every query as one created
+        from the same scene with this sky would.  The accumulated image and the frame counter stay as they are (Init
+        restarts them).  A CUDA probe is read after torch's current stream, as the queries read their inputs."""
+        colours = []
+        for name, c in (("horizon", horizon), ("zenith", zenith)):
+            c = [float(v) for v in c]
+            if len(c) != 3:
+                raise ValueError("%s must have 3 values (r, g, b), not %d" % (name, len(c)))
+            colours.append((C.c_float * 3)(*c))
+        h, z = colours
+        if probe is None:
+            self._check(self.lib.tb200_set_sky(self.h, h, z, None, 0, 0), "tb200_set_sky")
+            return
+        ptr, width, height, on_device = self._probe_image(probe, False)
+        if on_device:
+            self._wait_for_torch()
+        self._check(self.lib.tb200_set_sky(self.h, h, z, C.c_void_p(ptr), width, height), "tb200_set_sky")
+
+    def probe_tables(self, probe, pdf_x=None, cdf_x=None, pdf_y=None, cdf_y=None):
+        """Probe::BuildCDF (src/probe.h:31-79) of a probe on the device (tb200_probe_tables), bit for bit: probe is an
+        (H, W, 4) float32 contiguous CUDA tensor on the head device.  Returns (pdf_x (H, W), cdf_x (H, W), pdf_y (H,),
+        cdf_y (H,)) float32 tensors, the given ones when passed.  It does not change the renderer's sky.  Stream
+        behaviour as for trace_rays."""
+        import torch
+        ptr, width, height, _ = self._probe_image(probe, True)
+        dev = torch.device("cuda", self.device)
+        out = []
+        for y, name, shape in ((pdf_x, "pdf_x", (height, width)), (cdf_x, "cdf_x", (height, width)),
+                               (pdf_y, "pdf_y", (height,)), (cdf_y, "cdf_y", (height,))):
+            if y is None:
+                y = torch.empty(shape, dtype=torch.float32, device=dev)
+            self._check_tensor(y, name, shape, torch.float32)
+            out.append(y)
+        self._wait_for_torch()
+        self._check(self.lib.tb200_probe_tables(self.h, C.c_void_p(ptr), width, height, *[y.data_ptr() for y in out]),
+                    "tb200_probe_tables")
+        return tuple(out)
 
     def set_frame(self, frame):
         self.lib.tb200_set_frame(self.h, frame)

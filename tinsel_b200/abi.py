@@ -261,6 +261,8 @@ EXPORTS = [
     "tb200_sky_eval",
     "tb200_sample_emitters",
     "tb200_sample_probe",
+    "tb200_probe_tables",
+    "tb200_set_sky",
     "tb200_set_frame",
     "tb200_get_stats",
     "tb200_last_kernel",

@@ -14,7 +14,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libtinsel_b200.so")
 
 SOURCES = ["kernels.cu", "api.cu", "snapshot.cpp", "bvh_build.cu"]
-HEADERS = ["tb_math.cuh", "tb_scene.cuh", "tb_shade.cuh", "tb_film.cuh", "tb_kernels.cuh", "wf2_common.cuh", "wf2_lanes.cuh", "wf2_rings.cuh", "tb_query.cuh"]
+HEADERS = ["tb_math.cuh", "tb_scene.cuh", "tb_shade.cuh", "tb_film.cuh", "tb_kernels.cuh", "wf2_common.cuh", "wf2_lanes.cuh", "wf2_rings.cuh", "tb_query.cuh", "tb_probe.cuh"]
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 

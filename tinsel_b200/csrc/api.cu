@@ -265,6 +265,7 @@ struct tb200_renderer {
     // releases them all at once, with the renderer's device current and before its streams go.
     struct Memory {
         std::vector<DevPtr<void>> scene;   // the scene's arrays (`scene` below points into them)
+        std::vector<DevPtr<void>> probe;   // the sky's probe and its four tables (tb200_set_sky replaces them)
         DevPtr<float4> accum;
         DevPtr<float> radiance, raster;   // tb200_trace_frame scratch, allocated on first use per image size
         DevPtr<unsigned long long> counter;
@@ -309,6 +310,10 @@ struct tb200_renderer {
 
     Knobs knobs = {};             // read once, at the start of tb200_create* (read_knobs)
     Wf2Route route = {};          // the wavefront kernel's scheduling, decided at upload (kernels.cu: wavefront2_route)
+    // what the route reads besides the sky, kept from the upload so that tb200_set_sky can route again
+    int lightNee = 0;             // shadow rays per hit from the scene's lights (DScene::numNee less the probe's one)
+    int maxTris = 0;              // the largest mesh's triangles
+    uint32_t sceneFeatures = 0;   // scene_features less TB_FEAT_PROBE
     const char* lastKernel = "";  // the kernel the last path-tracing launch ran (tb200_last_kernel)
     // Split trace queue on/off is decided by measurement when route.tune (every variant produces the same bits):
     // the second and third sizeable launches after tb200_create time one setting each, the faster stays.
@@ -477,10 +482,11 @@ uint32_t scene_features(const SceneImage& img)
     return f;
 }
 
-// Copies `host` and padElems zeroed elements after it into a new allocation of r's scene memory; *dev = its
-// address, null for no elements
+// Copies `host` and padElems zeroed elements after it into a new allocation owned by `owner` (default: r's scene
+// memory); *dev = its address, null for no elements
 template <typename T>
-bool upload(tb200_renderer* r, const std::vector<T>& host, const T** dev, size_t padElems = 0)
+bool upload(tb200_renderer* r, const std::vector<T>& host, const T** dev, size_t padElems = 0,
+            std::vector<DevPtr<void>>* owner = nullptr)
 {
     *dev = nullptr;
     const size_t n = host.size() + padElems;
@@ -491,7 +497,7 @@ bool upload(tb200_renderer* r, const std::vector<T>& host, const T** dev, size_t
     if (!host.empty()) TB_CUDA(cudaMemcpy(mem.get(), host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice));
     r->stats.h2dBytes += host.size() * sizeof(T);
     *dev = mem.get();
-    r->mem.scene.push_back(std::move(mem));
+    (owner ? owner : &r->mem.scene)->push_back(std::move(mem));
     return true;
 }
 
@@ -513,6 +519,9 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
     sc.splitValid = img.splitBoxValid;
     sc.splitLo = img.splitLo;
     sc.splitHi = img.splitHi;
+    r->lightNee = img.numNee - (img.probeValid ? 1 : 0);
+    r->maxTris = img.maxTris;
+    r->sceneFeatures = scene_features(img) & ~(uint32_t)TB_FEAT_PROBE;
     r->route = wavefront2_route(img.numNee, img.maxTris, img.splitBoxValid, scene_features(img), r->knobs);
     r->tunePhase = r->route.tune ? 0 : 3;
     // one element of padding each: the kernels' bulk copies round their length up to 16 bytes
@@ -545,8 +554,10 @@ bool upload_image(tb200_renderer* r, const SceneImage& img)
     sc.zenith = img.zenith;
     sc.numNee = img.numNee;
     if (img.probeValid) {
-        if (!upload(r, img.probeData, &sc.probe.data) || !upload(r, img.pdfX, &sc.probe.pdfX) || !upload(r, img.cdfX, &sc.probe.cdfX) ||
-            !upload(r, img.pdfY, &sc.probe.pdfY) || !upload(r, img.cdfY, &sc.probe.cdfY))
+        std::vector<DevPtr<void>>* own = &r->mem.probe;
+        if (!upload(r, img.probeData, &sc.probe.data, 0, own) || !upload(r, img.pdfX, &sc.probe.pdfX, 0, own) ||
+            !upload(r, img.cdfX, &sc.probe.cdfX, 0, own) || !upload(r, img.pdfY, &sc.probe.pdfY, 0, own) ||
+            !upload(r, img.cdfY, &sc.probe.cdfY, 0, own))
             return false;
         sc.probe.valid = 1;
         sc.probe.width = img.probeW;
@@ -1852,6 +1863,26 @@ struct QuerySpan {
     size_t fixedBytes = 0;
 };
 
+// Records evStart on r's stream, calls launch(&launches) to queue kernels there, records evStop, adds the launches to
+// stats.kernelLaunches, waits for the stream and sets stats.gpuMs to the time between the events.  A CUDA failure is
+// reported as `entry`'s.
+static int timed_launch(const char* entry, tb200_renderer* r, const std::function<void(unsigned long long*)>& launch)
+{
+    auto fail = [&](const char* why) {
+        set_error(std::string(entry) + ": " + why);
+        return -1;
+    };
+    unsigned long long launches = 0;
+    if (cudaEventRecord(r->evStart, r->stream) != cudaSuccess) return fail(cudaGetErrorString(cudaGetLastError()));
+    launch(&launches);
+    r->stats.kernelLaunches += launches;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaEventRecord(r->evStop, r->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
+    if (e != cudaSuccess) return fail(cudaGetErrorString(e));
+    return sync_gpu_ms(r) ? 0 : -1;
+}
+
 // Every batched query: checks the renderer, the record count (named `countName` in refusals), then the input and
 // the outputs in the order given (the first refusal sets the error), makes the renderer's device current, runs the
 // query's kernel on r's stream with Q's pointers, waits for it and sets stats.gpuMs to its time.  No records:
@@ -1876,16 +1907,7 @@ static int run_query(const char* entry, tb200_renderer* r, QueryKind kind, const
     Q.scene = r->scene;
     Q.numRays = count;
     Q.counter = r->mem.counter.get();   // the wavefront's work counter: free between launches on this stream
-
-    unsigned long long launches = 0;
-    if (cudaEventRecord(r->evStart, r->stream) != cudaSuccess) return fail(cudaGetErrorString(cudaGetLastError()));
-    launch_query(kind, Q, r->numSMs, r->stream, &launches);
-    r->stats.kernelLaunches += launches;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaEventRecord(r->evStop, r->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
-    if (e != cudaSuccess) return fail(cudaGetErrorString(e));
-    return sync_gpu_ms(r) ? 0 : -1;
+    return timed_launch(entry, r, [&](unsigned long long* launches) { launch_query(kind, Q, r->numSMs, r->stream, launches); });
 }
 
 static_assert(sizeof(tb200_ray) == 32 && sizeof(tb200_hit) == 16, "the query kernels read two float4 per ray and write one hit");
@@ -2044,6 +2066,133 @@ int tb200_sample_probe(tb200_renderer* r, const uint32_t* seeds, tb200_probe_sam
     Q.probeOut = reinterpret_cast<float4*>(out);
     return run_query("tb200_sample_probe", r, QueryKind::SampleProbe, "n", n,
                      {{seeds, sizeof(uint32_t), 4, "seeds"}, {out, sizeof(tb200_probe_sampled), 16, "out"}}, Q);
+}
+
+// A probe size tb200_probe_tables and tb200_set_sky accept: both sides positive, and width*height + 1 elements (a
+// table and its slack element) indexable with int, as ProbeSample's row * width is.  Refusals name `entry`.
+static bool probe_size_ok(const char* entry, const tb200_renderer* r, int width, int height)
+{
+    const std::string e = std::string(entry) + ": ";
+    if (!r) return set_error(e + "null renderer");
+    const std::string size = std::to_string(width) + " x " + std::to_string(height);
+    if (width <= 0 || height <= 0) return set_error(e + "probe size " + size + " is not positive");
+    if ((int64_t)width * height + 1 > (int64_t)INT32_MAX) return set_error(e + "probe size " + size + " has 2^31-1 texels or more");
+    return true;
+}
+
+int tb200_probe_tables(tb200_renderer* r, const float* probe, int width, int height, float* pdfX, float* cdfX, float* pdfY,
+                       float* cdfY)
+{
+    const char* entry = "tb200_probe_tables";
+    if (!probe_size_ok(entry, r, width, height)) return -1;
+    cudaSetDevice(r->device);
+    const size_t n = (size_t)width * height;
+    if (!check_device_span(entry, r, probe, n * sizeof(float4), 16, "probe") || !check_device_span(entry, r, pdfX, n * 4, 4, "pdfX") ||
+        !check_device_span(entry, r, cdfX, n * 4, 4, "cdfX") || !check_device_span(entry, r, pdfY, (size_t)height * 4, 4, "pdfY") ||
+        !check_device_span(entry, r, cdfY, (size_t)height * 4, 4, "cdfY"))
+        return -1;
+    const ProbeTablesParams P = {reinterpret_cast<const float4*>(probe), width, height, pdfX, cdfX, pdfY, cdfY};
+    return timed_launch(entry, r, [&](unsigned long long* launches) { launch_probe_tables(P, r->stream, launches); });
+}
+
+// A member's new probe, built by sky_build before any member's sky is replaced
+struct SkyBuild {
+    std::vector<DevPtr<void>> mem;
+    DProbe probe = {};
+};
+
+// Builds member m's copy of the width x height texels at `probe` (host memory, or with onDevice device memory of
+// device srcDevice) and their four tables, each array with the one zeroed element of slack upload_image gives it;
+// sets m's stats.gpuMs to the tables' build time.
+static int sky_build(tb200_renderer* m, const float* probe, bool onDevice, int srcDevice, int width, int height, SkyBuild* out)
+{
+    cudaSetDevice(m->device);
+    const size_t n = (size_t)width * height, h = (size_t)height;
+    DevPtr<float4> data;
+    DevPtr<float> pdfX, cdfX, pdfY, cdfY;
+    cudaError_t e = dev_alloc(&data, n + 1);
+    if (e == cudaSuccess) e = dev_alloc(&pdfX, n + 1);
+    if (e == cudaSuccess) e = dev_alloc(&cdfX, n + 1);
+    if (e == cudaSuccess) e = dev_alloc(&pdfY, h + 1);
+    if (e == cudaSuccess) e = dev_alloc(&cdfY, h + 1);
+    if (e == cudaSuccess) e = cudaMemsetAsync(data.get() + n, 0, sizeof(float4), m->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(pdfX.get() + n, 0, sizeof(float), m->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(cdfX.get() + n, 0, sizeof(float), m->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(pdfY.get() + h, 0, sizeof(float), m->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(cdfY.get() + h, 0, sizeof(float), m->stream);
+    if (e == cudaSuccess)
+        e = onDevice && srcDevice != m->device ? cudaMemcpyPeerAsync(data.get(), m->device, probe, srcDevice, n * sizeof(float4), m->stream)
+                                               : cudaMemcpyAsync(data.get(), probe, n * sizeof(float4), cudaMemcpyDefault, m->stream);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        set_error(std::string("tb200_set_sky: ") + cudaGetErrorString(e));
+        return -1;
+    }
+    const ProbeTablesParams P = {data.get(), width, height, pdfX.get(), cdfX.get(), pdfY.get(), cdfY.get()};
+    if (timed_launch("tb200_set_sky", m, [&](unsigned long long* launches) { launch_probe_tables(P, m->stream, launches); }) != 0)
+        return -1;
+    if (!onDevice) m->stats.h2dBytes += n * sizeof(float4);
+    out->probe = DProbe{1, width, height, data.get(), pdfX.get(), cdfX.get(), pdfY.get(), cdfY.get()};
+    out->mem.push_back(std::move(data));
+    out->mem.push_back(std::move(pdfX));
+    out->mem.push_back(std::move(cdfX));
+    out->mem.push_back(std::move(pdfY));
+    out->mem.push_back(std::move(cdfY));
+    return 0;
+}
+
+int tb200_set_sky(tb200_renderer* r, const float horizon[3], const float zenith[3], const float* probe, int width, int height)
+{
+    const char* entry = "tb200_set_sky";
+    auto fail = [&](const std::string& why) {
+        set_error(std::string(entry) + ": " + why);
+        return -1;
+    };
+    if (!r) return fail("null renderer");
+    if (!horizon || !zenith) return fail("horizon or zenith is null");
+    bool onDevice = false;
+    if (!probe) {
+        if (width != 0 || height != 0)
+            return fail("without a probe, width and height must be 0, not " + std::to_string(width) + " x " + std::to_string(height));
+    } else {
+        if (!probe_size_ok(entry, r, width, height)) return -1;
+        cudaSetDevice(r->device);
+        cudaPointerAttributes attr;
+        if (cudaPointerGetAttributes(&attr, probe) != cudaSuccess) {
+            cudaGetLastError();   // not known to CUDA: host memory
+            attr.type = cudaMemoryTypeUnregistered;
+        }
+        onDevice = attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged;
+        if (onDevice && !check_device_span(entry, r, probe, (size_t)width * height * sizeof(float4), 16, "probe")) return -1;
+    }
+    // every member builds its new probe first; only when all have succeeded does any member's sky change
+    std::vector<tb200_renderer*> members(1, r);
+    members.insert(members.end(), r->peers.begin(), r->peers.end());
+    std::vector<SkyBuild> builds(members.size());
+    if (probe) {
+        const int rc = group_run(r, [&](tb200_renderer* m) {
+            const size_t k = std::find(members.begin(), members.end(), m) - members.begin();
+            return sky_build(m, probe, onDevice, r->device, width, height, &builds[k]);
+        });
+        if (rc != 0) return -1;
+    }
+    for (size_t k = 0; k < members.size(); ++k) {
+        tb200_renderer* m = members[k];
+        cudaSetDevice(m->device);
+        m->mem.probe = std::move(builds[k].mem);   // frees the previous probe
+        DScene& sc = m->scene;
+        sc.horizon = hv3(horizon);
+        sc.zenith = hv3(zenith);
+        sc.probe = builds[k].probe;
+        sc.numNee = m->lightNee + sc.probe.valid;
+        // upload_image's routing, for the scene with this sky
+        const uint32_t features = m->sceneFeatures | (sc.probe.valid ? (uint32_t)TB_FEAT_PROBE : 0u);
+        m->route = wavefront2_route(sc.numNee, m->maxTris, sc.splitValid, features, m->knobs);
+        m->tunePhase = m->route.tune ? 0 : 3;
+        if (!probe) m->stats.gpuMs = 0.0;
+    }
+    cudaSetDevice(r->device);
+    return 0;
 }
 
 #ifdef TB_WF2_STAGE_CLOCKS

@@ -427,3 +427,8 @@ const char* launch_wavefront2(const LaunchParams& p, const Wf2Route& route, int 
 // Batched closest-hit ray query: see tb_query.cuh
 // ------------------------------------------------------------------------------------------------
 #include "tb_query.cuh"
+
+// ------------------------------------------------------------------------------------------------
+// The probe's sampling tables (Probe::BuildCDF): see tb_probe.cuh
+// ------------------------------------------------------------------------------------------------
+#include "tb_probe.cuh"

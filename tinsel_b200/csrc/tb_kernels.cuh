@@ -180,3 +180,12 @@ struct QueryParams {
 };
 // Unlike the launches above, it leaves tb200_last_kernel alone and so returns no kernel name.
 void launch_query(QueryKind kind, const QueryParams& p, int numSMs, cudaStream_t stream, unsigned long long* launchCount);
+
+// Probe::BuildCDF (src/probe.h:31-79) on the device (tb_probe.cuh): from width*height RGBA texels, pdfX and cdfX
+// (width*height floats each), pdfY and cdfY (height floats each).  width*height < INT32_MAX.  Three launches.
+struct ProbeTablesParams {
+    const float4* probe;
+    int width, height;
+    float *pdfX, *cdfX, *pdfY, *cdfY;
+};
+void launch_probe_tables(const ProbeTablesParams& p, cudaStream_t stream, unsigned long long* launchCount);
