@@ -307,7 +307,10 @@ int tb200_trace_frame(tb200_renderer* r, const tb200_camera* camera, const tb200
  *   hits[i].normal the shading normal after FaceForward(n, -dir)
  * A miss leaves t = FLT_MAX and the face-forwarded zero normal.  `time` drives the motion-blur
  * interpolation of primitive transforms; `pad` is ignored here (tb200_occluded_rays reads it as
- * tmax, so one array of rays can feed both queries).
+ * tmax, so one array of rays can feed both queries).  Any finite `time`, inside the shutter or not, is exact.  A NaN
+ * or infinite time is the one exception: the device keeps a static primitive's transform (a sphere or mesh whose
+ * start and end transforms match bit for bit and have no -0 component), where the reference's interpolation gives
+ * NaN.  A primitive that moves is exact at any time, and so is a plane, which ignores transforms.
  * `rays`, `hits` and `prims` are DEVICE memory of the renderer's device (a multi-device renderer: its
  * head, devices[0]); `rays` and `hits` 16-byte aligned.  Host or foreign-device pointers, null pointers,
  * numRays < 0 and spans past the end of their allocation are refused before anything is launched.
@@ -326,6 +329,10 @@ int tb200_trace_rays(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, 
  * ray's `pad` field; else 0.  t is in units of |dir|, so dir = target - origin with tmax = 1 asks
  * whether anything lies between two points.  tmax <= 0 or NaN gives 0, tmax = +inf "hits anything";
  * a miss (t = FLT_MAX) is never occluded.  The walk stops at the first blocker and computes no normal.
+ * Any finite `time`, inside the shutter or not, is exact.  A NaN or infinite time is the one exception:
+ * the device keeps a static primitive's transform (a sphere or mesh whose start and end transforms match bit for bit
+ * and have no -0 component), where the reference's interpolation gives NaN.  A primitive that moves is exact at any
+ * time, and so is a plane, which ignores transforms.
  * `rays` (16-byte aligned) and `occluded` (numRays bytes) are DEVICE memory of the renderer's
  * device, with the refusals, stream, synchronisation and side effects of tb200_trace_rays: it adds
  * 1 to stats.kernelLaunches, sets stats.gpuMs to its kernel's time, and touches nothing else.
@@ -346,7 +353,10 @@ int tb200_occluded_rays(tb200_renderer* r, const tb200_ray* rays, uint8_t* occlu
  * tri = -1 and u = v = w = 0.  tris (numRays records, 16-byte aligned) is DEVICE memory like the other
  * arrays; the refusals, stream, synchronisation and side effects are tb200_trace_rays': it adds 1 to
  * stats.kernelLaunches, sets stats.gpuMs to its kernel's time, and touches nothing else.  numRays == 0
- * launches nothing.  `pad` is ignored.  Returns 0 on success. */
+ * launches nothing.  `pad` is ignored.  Any finite `time`, inside the shutter or not, is exact.  A NaN or infinite
+ * time is the one exception: the device keeps a static primitive's transform (a sphere or mesh whose start and end
+ * transforms match bit for bit and have no -0 component), where the reference's interpolation gives NaN.  A primitive
+ * that moves is exact at any time, and so is a plane, which ignores transforms.  Returns 0 on success. */
 typedef struct tb200_tri_hit { int32_t tri; float u, v, w; } tb200_tri_hit;   /* 16 B */
 int tb200_trace_rays_tri(tb200_renderer* r, const tb200_ray* rays, tb200_hit* hits, int32_t* prims,
                          tb200_tri_hit* tris, int64_t numRays);
@@ -434,9 +444,11 @@ int tb200_splat(tb200_renderer* r, const tb200_options* options, const float* ra
  *     tb200_bsdf_eval; all are used as given, never normalised, and the etas may take any value.  The BSDF is the
  *     material the path tracer shades `prim` with.  A prim outside [0, numPrimitives) gives zeros and traces
  *     nothing, so the prims of tb200_trace_rays can be passed straight through on misses (-1).  The three floats
- *     per query are the layout tb200_splat reads its radiance in.  `time` must be finite, as the renderer's own
- *     ray times are: the device takes a static primitive's transform as it is, where the reference interpolates it
- *     and a NaN or infinite time would make it NaN; any finite time, inside the shutter or not, is exact.
+ *     per query are the layout tb200_splat reads its radiance in.  Any finite `time`, inside the shutter or not, is
+ *     exact.  A NaN or infinite time is the one exception: the device keeps a static primitive's transform (a sphere
+ *     or mesh whose start and end transforms match bit for bit and have no -0 component), where the reference's
+ *     interpolation gives NaN.  A primitive that moves is exact at any time, and so is a plane, which ignores
+ *     transforms.
  *   tb200_sky_eval: per ray i (only rays[i].dir is read, so the records of tb200_trace_rays and tb200_camera_rays can
  *     be passed as they are), out[4i..4i+2] = Sky::Eval(dir) (src/scene.h:168-178) and out[4i+3] = ProbePdf(dir)
  *     (src/probe.h:136-160) when the sky has a probe, else 0; bit for bit.  The miss branch's MIS weight
@@ -467,8 +479,10 @@ int tb200_sky_eval(tb200_renderer* r, const tb200_ray* rays, float* out, int64_t
  *     refuses a mesh light without a CDF).  Any other primitive -- not a light, a plane, or a prim outside
  *     [0, numPrimitives), so that the prims of tb200_trace_rays can be passed straight through on misses (-1) --
  *     gives pos = normal = 0.  A degenerate triangle can give a zero normal too, so a zero normal does not mean
- *     "not a light".  `time` must be finite, as for tb200_sample_lights: the device takes a static primitive's
- *     transform as it is, where the reference interpolates it and a NaN or infinite time would make it NaN.
+ *     "not a light".  Any finite `time`, inside the shutter or not, is exact.  A NaN or infinite time is the one
+ *     exception: the device keeps a static primitive's transform (a sphere or mesh whose start and end transforms
+ *     match bit for bit and have no -0 component), where the reference's interpolation gives NaN.  A primitive that
+ *     moves is exact at any time, and so is a plane, which ignores transforms.
  *     The area pdf of a sample is 1 / PrimitiveArea (tinsel_b200.primitive_areas gives it as the renderer computes
  *     it: 4 pi r^2 of the unscaled radius for a sphere, the mesh's area times the end transform's scale for a mesh).
  *   tb200_sample_probe: per seed i, ProbeSample(probe, dir, color, pdf, Random(seeds[i])) (src/probe.h:205-236),

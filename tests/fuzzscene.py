@@ -121,7 +121,7 @@ def _nodes(tree):
     return nodes
 
 
-def _save(rng, path, prims, tree, meshes, width, height, probe=None, camera=None, max_depth=None):
+def _save(rng, path, prims, tree, meshes, width, height, probe=None, camera=None, max_depth=None, shutter=(0.0, 1.0)):
     """Sky, camera and options drawn from `rng`, then the snapshot.  meshes: list of MeshData."""
     scene, keep = make_scene_struct(prims, tree, meshes)
     scene.sky.horizon[:] = [float(x) for x in rng.uniform(0.0, 1.0, 3)]
@@ -136,7 +136,7 @@ def _save(rng, path, prims, tree, meshes, width, height, probe=None, camera=None
     cam.position[:] = [0.0, 1.2, 6.0]
     cam.rotation[:] = [0.0, 0.0, 0.0, 1.0]
     cam.fov = float(np.radians(rng.uniform(35.0, 60.0))) if cam.fov < 3.2 else float(rng.uniform(35.0, 60.0))
-    cam.shutterStart, cam.shutterEnd = 0.0, 1.0
+    cam.shutterStart, cam.shutterEnd = shutter
     if camera is not None:
         cam.position[:] = camera
     opt.width, opt.height = width, height
@@ -331,26 +331,27 @@ def _quat(rng):
     return q / np.linalg.norm(q)
 
 
-def _instance(p, mesh_index, mesh, pos, q, s, end_pos=None, end_s=None):
+def _instance(p, mesh_index, mesh, pos, q, s, end_pos=None, end_s=None, end_q=None):
     p.type = abi.MESH
     p.mesh = mesh_index
     _xf(p.start, pos, q, s)
-    _xf(p.end, pos if end_pos is None else end_pos, q, s if end_s is None else end_s)
+    _xf(p.end, pos if end_pos is None else end_pos, q if end_q is None else end_q, s if end_s is None else end_s)
     r = mesh.radius * max(s, s if end_s is None else end_s) * 1.001 + 1e-4
     e = pos if end_pos is None else end_pos
     return (np.minimum(pos, e).astype(np.float32) - np.float32(r), np.maximum(pos, e).astype(np.float32) + np.float32(r))
 
 
-def _sphere(p, pos, radius, material, light_samples=0):
+def _sphere(p, pos, radius, material, light_samples=0, q=(0, 0, 0, 1), end_q=None, end_pos=None):
     p.type = abi.SPHERE
     p.radius = float(radius)
     p.mesh = -1
-    _xf(p.start, pos, (0, 0, 0, 1), 1.0)
-    _xf(p.end, pos, (0, 0, 0, 1), 1.0)
+    e = pos if end_pos is None else end_pos
+    _xf(p.start, pos, q, 1.0)
+    _xf(p.end, e, q if end_q is None else end_q, 1.0)
     p.material = material
     p.lightSamples = light_samples
     r = float(radius) * 1.001 + 1e-4
-    return (np.asarray(pos, np.float32) - np.float32(r), np.asarray(pos, np.float32) + np.float32(r))
+    return (np.minimum(pos, e).astype(np.float32) - np.float32(r), np.maximum(pos, e).astype(np.float32) + np.float32(r))
 
 
 def _floor(p, rng):
@@ -374,7 +375,53 @@ def _probe(rng):
     return img
 
 
-FAMILIES = ("instanced", "ties", "many", "big", "probe", "caterpillar")
+FAMILIES = ("instanced", "ties", "many", "big", "probe", "caterpillar", "rotating", "signed_zero")
+# rotation pairs of the rotating family, by what the reference's quaternion lerp a + (b - a) t does with them
+ROTATIONS = ("random", "antipodal", "near_antipodal", "tiny_lerp", "one_ulp")
+SHUTTER = (-0.5, 0.5)      # the camera shutter of the rotating and signed_zero families: half the times are negative
+
+
+def rotation_pair(rng, kind):
+    """(start, end) float32 quaternions of the kind:
+      random          two random unit quaternions
+      antipodal       q and -q: the lerp is exactly 0 at t = 0.5, where the reference's transform is NaN
+      near_antipodal  -q with one component moved by 1e-3 or by 1-8 ulps: a lerp length near 0 at t = 0.5
+      tiny_lerp       q with a +0 component k and -q with 2e-21 at k: the lerp at t = 0.5 is 1e-21 in component k and
+                      exactly 0 elsewhere, a length below 1e-20 whose normalisation still gives a unit quaternion
+      one_ulp         q and q with one component one ulp away: at t = +-FLT_MAX the lerp overflows"""
+    q = _quat(rng).astype(np.float32)
+    k = int(rng.randint(0, 4))
+    if kind == "random":
+        return q, _quat(rng).astype(np.float32)
+    if kind == "antipodal":
+        return q, -q
+    e = -q
+    if kind == "near_antipodal":
+        if rng.uniform() < 0.5:
+            e[k] += np.float32(1e-3)
+        else:
+            for _ in range(int(rng.randint(1, 9))):
+                e[k] = np.nextafter(e[k], np.float32(np.inf))
+        return q, e
+    if kind == "tiny_lerp":
+        q[k] = 0.0
+        e = -q
+        e[k] = np.float32(2e-21)
+        return q, e
+    assert kind == "one_ulp"
+    e = q.copy()
+    e[k] = np.nextafter(q[k], np.float32(rng.choice([-np.inf, np.inf])))
+    return q, e
+
+
+def _has_negative_zero(t):
+    return any(np.signbit(x) and x == 0.0 for x in list(t.p) + list(t.r) + [t.s])
+
+
+def is_static(p):
+    """Whether the renderer takes primitive p's transform without interpolating it (api.cu: image_from_scene): start and
+    end are the same bit for bit and no component of p, r or s is -0."""
+    return bytes(p.start) == bytes(p.end) and not _has_negative_zero(p.start)
 
 
 def make_mesh_scene(seed, path, family, width=40, height=30, swap_ties=False, levels=None):
@@ -390,7 +437,11 @@ def make_mesh_scene(seed, path, family, width=40, height=30, swap_ties=False, le
                    free-running wavefront, 768-thread CTAs, the mesh-split queue and its tuner
       probe        `instanced` lit by a small random HDR probe
       caterpillar  a stack of parallel triangles in front of the camera, nearer ones deeper in a chain BVH of
-                   `levels` interior levels: the traversal stack fills to levels + 1 entries"""
+                   `levels` interior levels: the traversal stack fills to levels + 1 entries
+      rotating     a mesh instance and a sphere for each kind of rotation_pair, all rotating over the shutter
+                   SHUTTER; some instances also move and scale, some are mesh lights, some spheres sphere lights
+      signed_zero  static spheres, sphere lights, mesh instances and mesh lights with -0 in their position
+                   (on the x = 0 plane) and rotation, each beside a twin written with +0, under SHUTTER"""
     rng = np.random.RandomState(10007 * (FAMILIES.index(family) + 1) + seed)
     prims, bounds, meshes, info = [], [], [], {"family": family, "seed": seed}
     P = (abi.Primitive * 64)()
@@ -401,7 +452,55 @@ def make_mesh_scene(seed, path, family, width=40, height=30, swap_ties=False, le
         return prims[-1]
 
     bounds.append(_floor(add(), rng))
-    if family == "caterpillar":
+    shutter = (0.0, 1.0)
+    if family == "rotating":
+        shutter = SHUTTER
+        for _ in range(int(rng.randint(1, 3))):
+            meshes.append(_random_mesh(rng)[1])
+        kinds = []
+        for k, kind in enumerate(ROTATIONS):
+            qa, qb = rotation_pair(rng, kind)
+            mi = int(rng.randint(0, len(meshes)))
+            q = add()
+            light = (k + seed) % 2 == 0
+            q.material = _material(rng, light)
+            q.lightSamples = int(rng.randint(1, 3)) if light else 0
+            pos = rng.uniform(-2.0, 2.0, 3) * (1, 0.4, 1) + (0, 1.0, 0)
+            s = float(rng.uniform(0.3, 0.8))
+            end = pos + rng.uniform(-0.3, 0.3, 3) if rng.uniform() < 0.5 else None
+            end_s = s * float(rng.uniform(0.7, 1.3)) if rng.uniform() < 0.5 else None
+            bounds.append(_instance(q, mi, meshes[mi], pos, qa, s, end, end_s, qb))
+            qa, qb = rotation_pair(rng, kind)
+            light = (k + seed) % 2 == 1
+            pos = rng.uniform(-2.5, 2.5, 3) * (1, 0.5, 1) + (0, 1.5 if light else 0.8, 0)
+            end = pos + rng.uniform(-0.3, 0.3, 3) if rng.uniform() < 0.5 else None
+            bounds.append(_sphere(add(), pos, rng.uniform(0.1, 0.4), _material(rng, light), int(rng.randint(1, 3)) if light else 0,
+                                  qa, qb, end))
+            kinds += [kind, kind]
+        info["rotations"] = kinds
+    elif family == "signed_zero":
+        shutter = SHUTTER
+        p, n, f = _grid(2)                       # normals (0, 0, 1): rotations of exact zeros
+        meshes.append(MeshData(p, n, f))
+        meshes.append(_random_mesh(rng)[1])
+        rots = [(-0.0, 0.0, 0.0, 1.0), (0.0, -0.0, 0.0, 1.0), (0.0, 0.0, -0.0, 1.0), (-0.0, -0.0, -0.0, 1.0), (-0.0, 0.6, 0.0, 0.8),
+                (0.0, -0.0, 0.6, 0.8)]
+        for k, kind in enumerate(("sphere", "sphere light", "mesh", "mesh light")):
+            qz = rots[int(rng.randint(0, len(rots)))]
+            y, z = 0.4 + 0.6 * k, float(rng.uniform(-1.5, 0.5))
+            light = kind.endswith("light")
+            mat = _material(rng, light)
+            for twin in (False, True):            # the twin is the same primitive written with +0, 2.2 to the right
+                rot = tuple(abs(c) for c in qz) if twin else qz
+                pos = (2.2 if twin else -0.0, y, z if k % 2 or twin else -0.0)
+                q = add()
+                if kind.startswith("mesh"):
+                    q.material = mat
+                    q.lightSamples = 1 if light else 0
+                    bounds.append(_instance(q, k % 2, meshes[k % 2], pos, rot, 0.5))
+                else:
+                    bounds.append(_sphere(q, pos, 0.3, mat, 1 if light else 0, rot))
+    elif family == "caterpillar":
         n = (levels or 30) + 1
         z = -1.0 - 0.05 * np.arange(n)[::-1]                   # item 0 farthest
         p = np.array([[[-3.0, -2.0, zz], [3.0, -2.0, zz], [0.0, 4.0, zz]] for zz in z]).reshape(-1, 3)
@@ -475,11 +574,14 @@ def make_mesh_scene(seed, path, family, width=40, height=30, swap_ties=False, le
         arr[i] = q
     tree = _build_bvh(bounds)
     probe = _probe(rng) if family == "probe" else None
-    opt = _save(rng, path, arr, tree, meshes, width, height, probe=probe, camera=camera)
+    opt = _save(rng, path, arr, tree, meshes, width, height, probe=probe, camera=camera, shutter=shutter)
     info.update(prims=len(prims), meshes=len(meshes), tris=[len(m.idx) for m in meshes], maxDepth=opt.maxDepth,
                 moving_scale=sum(1 for q in prims if q.type == abi.MESH and q.start.s != q.end.s),
                 mesh_lights=sum(1 for q in prims if q.type == abi.MESH and q.lightSamples > 0),
-                zero_area=sum(m.zero_area for m in meshes), probe=probe is not None)
+                zero_area=sum(m.zero_area for m in meshes), probe=probe is not None,
+                rotating=[i for i, q in enumerate(prims) if bytes(q.start)[12:28] != bytes(q.end)[12:28]],
+                negative_zero=[i for i, q in enumerate(prims) if _has_negative_zero(q.start) or _has_negative_zero(q.end)],
+                static=[i for i, q in enumerate(prims) if is_static(q)], shutter=shutter)
     return info
 
 

@@ -13,6 +13,13 @@ import schedenv
 
 SNAPSHOTS = sorted(f[:-6] for f in os.listdir(tb.SCENE_DIR) if f.endswith(".tsnap"))
 N = 1 << 15   # rays per set
+_FMAX = np.finfo(np.float32).max
+_DENORM = np.nextafter(np.float32(0.0), np.float32(1.0))
+# ray times, inside the shutter and outside: zeros of both signs, the smallest denormals, times near 0 and 1, and
+# times where the lerp of a moving primitive overflows
+TIMES = np.array([0.0, -0.0, _DENORM, -_DENORM, 1e-30, -1e-30, 0.25, 0.5, 1.0, np.nextafter(np.float32(1.0), np.float32(0.0)), -0.5,
+                  -1.0, 1.5, 10.0, 1e6, -1e6, 1e30, -1e30, _FMAX, -_FMAX], np.float32)
+NONFINITE_TIMES = np.array([np.inf, -np.inf, np.nan], np.float32)
 # fuzzscene families as (family, seed, swap_ties)
 FUZZ = [("ties", 0, False), ("ties", 0, True), ("ties", 3, True), ("many", 1, False), ("big", 0, False),
         ("caterpillar", 0, False), ("instanced", 0, False), ("instanced", 1, False), ("instanced", 2, False), ("probe", 0, False)]

@@ -197,9 +197,18 @@ def test_mesh_generator_makes_what_it_claims(tmp_path):
     assert all(i["zero_area"] > 0 for f in ("ties", "many", "big") for i in seen[f])
     assert any(i["moving_scale"] > 0 and i["mesh_lights"] > 0 and i["zero_area"] > 0 for i in inst)
     assert all(17 <= i["prims"] <= 40 for i in seen["many"])
-    assert all(i["prims"] <= 16 for f in ("instanced", "ties", "big", "probe", "caterpillar") for i in seen[f])
+    assert all(i["prims"] <= 16 for f in ("instanced", "ties", "big", "probe", "caterpillar", "rotating", "signed_zero") for i in seen[f])
     assert all(max(i["tris"]) > 4096 for i in seen["big"])
     assert all(i["levels"] == LIMIT - 1 for i in seen["caterpillar"])
+    # rotating: every sphere and mesh rotates (only the floor is static), with every kind of rotation pair
+    for i in seen["rotating"]:
+        assert i["rotating"] == list(range(1, i["prims"])) and i["static"] == [0] and i["shutter"] == fuzzscene.SHUTTER, i
+        assert sorted(set(i["rotations"])) == sorted(fuzzscene.ROTATIONS) and i["mesh_lights"] > 0, i
+    assert any(i["moving_scale"] > 0 for i in seen["rotating"])
+    # signed_zero: nothing moves or rotates, and exactly the primitives written with a -0 are not static
+    for i in seen["signed_zero"]:
+        assert not i["rotating"] and i["mesh_lights"] == 2 and i["shutter"] == fuzzscene.SHUTTER, i
+        assert len(i["negative_zero"]) == 4 and sorted(i["static"] + i["negative_zero"]) == list(range(i["prims"])), i
 
 
 @pytest.mark.parametrize("seed", range(5))

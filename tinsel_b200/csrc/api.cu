@@ -80,6 +80,15 @@ Xf to_xf(const tb200_transform& t)
     return x;
 }
 
+// whether a component of p, r or s is -0.0f
+bool has_negative_zero(const tb200_transform& t)
+{
+    const float c[8] = {t.p[0], t.p[1], t.p[2], t.r[0], t.r[1], t.r[2], t.r[3], t.s};
+    for (float x : c)
+        if (tb_float_bits(x) == 0x80000000u) return true;
+    return false;
+}
+
 // BVHNode[] (bvh.h:9-19) -> BvhPair[]; see tb_scene.cuh.  Returns the root reference.  Pairs are laid out
 // in breadth-first order from the root, so that the first K records are the top of the tree: the treelet
 // (DScene::treelet) stages exactly that prefix in shared memory with bulk copies, and the upper levels
@@ -424,8 +433,11 @@ bool image_from_scene(const tb200_scene* s, SceneImage* img)
         memset(&d, 0, sizeof(d));
         d.start = to_xf(p.start);
         d.end = to_xf(p.end);
-        d.isStatic = memcmp(&p.start, &p.end, sizeof(tb200_transform)) == 0;
-        // with start == end, Lerp(a,b,t) = a + (b-a)*t = a + 0*t is time independent
+        // With start == end bit for bit, Lerp(a,b,t) = a + (b-a)*t = a + 0*t.  For a finite t that is a, except for a
+        // component a = -0: -0 + (+0) = +0 at t >= +0, but -0 + (-0) = -0 at t < 0 or t = -0, and rotate_xf treats a
+        // -0 quaternion component as another rotation.  So `fixed` (the transform at t = 0) serves every finite time
+        // only when no component is -0; any other primitive is interpolated at its ray's time.
+        d.isStatic = memcmp(&p.start, &p.end, sizeof(tb200_transform)) == 0 && !has_negative_zero(p.start);
         d.fixed = interpolate_transform(d.start, d.end, 0.0f);
         d.type = p.type;
         d.radius = p.radius;
@@ -577,7 +589,7 @@ bool build_scene(tb200_renderer* r, const tb200_scene* s)
 // a stamp mismatch is refused and the caller falls back to tb200_create), then the SceneImage fields in
 // declaration order; every array as a 64-bit count followed by its bytes.
 const char kCacheMagic[8] = {'T', 'B', '2', 'C', 'A', 'C', 'H', 'E'};
-const uint32_t kCacheVersion = 4;   // 3: DMaterial::flags; 4: DPrim's light constants
+const uint32_t kCacheVersion = 5;   // 3: DMaterial::flags; 4: DPrim's light constants; 5: no -0 in a static DPrim
 
 struct CacheStamp {
     uint32_t version, sizeofPrim, sizeofPair, sizeofOp;

@@ -106,7 +106,7 @@ struct DMesh {
 
 struct DPrim {
     Xf start, end;
-    Xf fixed;             // InterpolateTransform(start,end,t) when isStatic
+    Xf fixed;             // InterpolateTransform(start,end,t) for every finite t when isStatic (api.cu)
     int isStatic;
     int type;
     float radius;
@@ -190,7 +190,7 @@ struct Hit {
 enum : uint32_t {
     TB_FEAT_NONE = 0u,
     TB_FEAT_PROBE = 1u << 0,          // the sky has an environment probe
-    TB_FEAT_MOTION = 1u << 1,         // a primitive moves (start != end transform)
+    TB_FEAT_MOTION = 1u << 1,         // a primitive is not static: its transform is interpolated at the ray's time
     TB_FEAT_TRANSMISSION = 1u << 2,   // a material has transmission != 0, or BSDFPdf must evaluate Fr for it
     TB_FEAT_SUBSURFACE = 1u << 3,     // a material has subsurface != 0
     TB_FEAT_CLEARCOAT = 1u << 4,      // a material has clearcoat != 0, or a clearcoat lobe that is not finite
